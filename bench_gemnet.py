@@ -50,7 +50,7 @@ def main():
     ap.add_argument("--cpu", action="store_true", help="also time the CPU oracle on the first two molecules")
     ap.add_argument("--train", action="store_true", help="time training steps (L1 energy + L2 force loss as GemNetOCLightning, AdamW) instead of inference; "
                                                          "keeps every activation: use a training-sized batch, e.g. --batch 16")
-    ap.add_argument("--simt", action="store_true", help="NB200_GOC_GEMM=simt: functor GEMM fallback instead of tcgen05 (bring-up A/B)")
+    ap.add_argument("--simt", action="store_true", help="NB200_GOC_GEMM=simt: functor GEMM fallback instead of the wgmma GEMMs (bring-up A/B)")
     args = ap.parse_args()
     if args.simt:
         os.environ["NB200_GOC_GEMM"] = "simt"
@@ -127,7 +127,7 @@ def main():
         ms = float(t.item())
         dist.barrier()
     out = {"metric": "molecules/sec (GemNet-OC training step, L1(E) + 100 L2(F), AdamW)" if args.train else "molecules/sec (GemNet-OC E + direct F forward)", "value": world * args.batch / (ms / 1e3), "unit": "molecules/s", "ms_per_step": ms,
-           "n_gpus": world, "scaling": "weak", "batch": args.batch, "atoms": int(b["z"].shape[0]), "counts": net._runner.last_counts, "gemm": "simt" if args.simt else "tcgen05-3xTF32",
+           "n_gpus": world, "scaling": "weak", "batch": args.batch, "atoms": int(b["z"].shape[0]), "counts": net._runner.last_counts, "gemm": "simt" if args.simt else "wgmma-3xTF32",
            "peak_mem_gb": torch.cuda.max_memory_allocated() / 2**30, "dtype": "f32", "data": "synthetic", "finite": bool(torch.isfinite(E).all() and torch.isfinite(F).all())}
     if not args.train:
         # tensor roofline of the dense layers: algorithmic fp32 FLOPs / time against the measured bf16 peak / 6 (TF32 runs at half the bf16

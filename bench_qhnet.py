@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""QHNet Hamiltonian prediction (BASELINE.json configs[3]: def2-SVP, 64-molecule batch, 1xB200): molecules/s of the
+"""QHNet Hamiltonian prediction (BASELINE.json configs[3]: def2-SVP, 64-molecule batch, 1xH100): molecules/s of the
 CUDA path, a per-stage breakdown with CUDA events, and the CPU oracle on one molecule.  Secondary benchmark
 (the driver's headline is bench.py); prints one JSON line."""
 import argparse

@@ -1,5 +1,5 @@
 /*
- * nabla_b200.h -- C ABI of the B200-native nablaDFT model-forward hot path.
+ * nabla_b200.h -- C ABI of the H100-native nablaDFT model-forward hot path.
  *
  * The reference (AIRI-Institute/nablaDFT) is pure Python; its "plugin seam" for this path
  * is `torch.nn.Module.forward(batch)` reached through Hydra `_target_` strings
@@ -154,15 +154,15 @@ int nb200_engine_destroy(nb200_engine* eng);
  * read_timings synchronises on the recorded events, sums elapsed ms per category and resets. */
 int nb200_engine_set_timing(nb200_engine* eng, int32_t enable);
 int nb200_engine_read_timings(nb200_engine* eng, float* ms_per_cat, int32_t* scopes_per_cat, int32_t n_cat);
-/* Node-level dense layers: 1 (default) = hand-written tcgen05 3xTF32 GEMM (fp32-accurate),
+/* Node-level dense layers: 1 (default) = hand-written wgmma 3xTF32 GEMM (fp32-accurate),
  * 0 = cuBLAS SGEMM (kept for A/B comparison). */
 int nb200_engine_set_gemm_backend(nb200_engine* eng, int32_t backend);
 /* PaiNN inference, per-atom part of a layer (PaiNNUpdate.forward painn.py:535-548, x_proj painn.py:459-464, out_energy[0]
- * painn.py:79-83 and their backward): 1 (default) = ONE fused tcgen05 kernel per layer and direction (painn_fused.cu: weights
+ * painn.py:79-83 and their backward): 1 (default) = ONE fused wgmma kernel per layer and direction (painn_fused.cu: weights
  * pre-split into TF32 hi/lo shared-memory images, chained MMAs, elementwise glue in loaders / epilogues),
  * 0 = one launch per Linear / elementwise op (the round-1 sequence; also what the training step uses). */
 int nb200_engine_set_node_backend(nb200_engine* eng, int32_t backend);
-/* C[M,N] = A[M,K] . op(B) (+C) (+bias), optional act = silu(C); fp32 in/out, 3xTF32 on tcgen05.
+/* C[M,N] = A[M,K] . op(B) (+C) (+bias), optional act = silu(C); fp32 in/out, 3xTF32 on wgmma.
  * op(B) = B[N,K]^T (trans_b=0, torch.nn.Linear forward: nablaDFT/painn_pyg/painn.py:459-464)
  *       | B[K,N]   (trans_b=1, its input gradient).  K % 32 == 0, N % 4 == 0, ld* % 4 == 0. */
 int nb200_gemm_tf32x3(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B,
@@ -172,7 +172,7 @@ int nb200_gemm_tf32x3(int32_t M, int32_t N, int32_t K, const float* A, int32_t l
  * nn.Linear of nablaDFT/painn_pyg/painn.py), ACCUMULATED into dW / dbias:
  *   dW[out,in] += alpha * ( (c o G0)^T X0 + G1^T X1 ),   dbias[out] += bias_alpha * colsum(c o G0)
  * G*[M,out] (ldg), X*[M,in] (ldx); G1/X1 NULL = one term; dbias NULL = none; row_scale c NULL = none, else row a is scaled by
- * row_scale[a / rs_div].  tcgen05 3xTF32 split-K over the M rows with atomic fp32 accumulation (wgrad_tc.cu).
+ * row_scale[a / rs_div].  wgmma 3xTF32 split-K over the M rows with atomic fp32 accumulation (wgrad_tc.cu).
  * in <= 128, in % 16 == 0, out % 4 == 0, ld* % 4 == 0, 16-byte aligned pointers; NB200_EINVAL otherwise. */
 int nb200_linear_wgrad(int32_t M, int32_t out, int32_t in, const float* G0, const float* X0, const float* G1,
                        const float* X1, int32_t ldg, int32_t ldx, float* dW, int32_t lddw, float alpha,
@@ -308,7 +308,7 @@ int nb200_qh_tp_self(const float* xl, const float* xr, const float* w, const flo
 /* e3nn o3.Linear over the 25 (l,m) rows: W_l [5][c_in][c_out] pre-scaled by 1/sqrt(c_in); bias on (0,0) */
 int nb200_qh_linear(const float* x, const float* W_l, const float* bias, int32_t n_rows, int32_t c_in,
                     int32_t c_out, int32_t accumulate, float* y, void* stream);
-/* fp32-accurate dense layer (tcgen05 3xTF32) with activation kind 0 silu, 1 ssp, 2 1.8782*ssp */
+/* fp32-accurate dense layer (wgmma 3xTF32) with activation kind 0 silu, 1 ssp, 2 1.8782*ssp */
 int nb200_dense(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb,
                 int32_t trans_b, float* C, int32_t ldc, int32_t accumulate, const float* bias, float* act,
                 int32_t act_kind, void* stream);

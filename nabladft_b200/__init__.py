@@ -1,4 +1,4 @@
-"""nabladft_b200 -- B200-native (sm_100a) engine for nablaDFT's model-forward hot path.
+"""nabladft_b200 -- H100-native (sm_90a) engine for nablaDFT's model-forward hot path.
 
 Only what the path needs: `csrc/` (CUDA kernels + C ABI, built into libnabla_b200.so),
 the ctypes binding (`_lib`), the engine driver and the host-side mirrors of the reference's

@@ -162,7 +162,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise NablaB200Error(
             f"{LIB_PATH} is missing: build it with `python -m nabladft_b200.build` "
-            "(nvcc, sm_100a). There is no CPU / eager fallback for this path."
+            "(nvcc, sm_90a). There is no CPU / eager fallback for this path."
         )
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

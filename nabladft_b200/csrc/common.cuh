@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the nabla_b200 kernels (sm_100a).
+// common.cuh -- shared device helpers for the nabla_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -15,6 +15,12 @@
 #define SCR_PERM 768
 
 extern thread_local int g_nb200_last_cuda_error;
+
+// streaming multiprocessors of the current device (queried once per process): grid sizing of the persistent / grid-stride launches
+static inline int nb_sm_count() {
+    static const int n = [] { int dev = 0, v = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev); return v > 0 ? v : 132; }();
+    return n;
+}
 
 static inline int nb_check_launch() {
     cudaError_t e = cudaGetLastError();
@@ -89,17 +95,6 @@ __device__ __forceinline__ void fma4s(float4& acc, float4 a, float s) {
     acc.x = fmaf(a.x, s, acc.x); acc.y = fmaf(a.y, s, acc.y); acc.z = fmaf(a.z, s, acc.z); acc.w = fmaf(a.w, s, acc.w);
 }
 __device__ __forceinline__ float hsum4(float4 a) { return (a.x + a.y) + (a.z + a.w); }
-// packed fp32 pairs (sm_100 FFMA2): two IEEE fma.rn per instruction, bitwise the same results as two FFMA
-__device__ __forceinline__ unsigned long long pack2f(float a, float b) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void unpack2f(unsigned long long v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ void fma4s_x2(float4& acc, float4 a, float s) {
-    unsigned long long a01 = pack2f(acc.x, acc.y), a23 = pack2f(acc.z, acc.w);
-    const unsigned long long ss = pack2f(s, s);
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a01) : "l"(pack2f(a.x, a.y)), "l"(ss));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a23) : "l"(pack2f(a.z, a.w)), "l"(ss));
-    unpack2f(a01, acc.x, acc.y); unpack2f(a23, acc.z, acc.w);
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

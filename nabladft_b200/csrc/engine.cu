@@ -7,7 +7,7 @@
 // here the backward is hand-derived and runs as the mirrored kernel sequence on one stream,
 // with no host synchronisation anywhere (edge count and error flags stay on the device).
 //
-// Node-level dense layers ([N,128]x[128,384] etc.) run on the tcgen05 3xTF32 GEMM of gemm_tc.cu (fp32-accurate: the reference never
+// Node-level dense layers ([N,128]x[128,384] etc.) run on the wgmma 3xTF32 GEMM of gemm_tc.cu (fp32-accurate: the reference never
 // uses reduced precision, SURVEY.md section 0.9); cuBLAS SGEMM stays selectable for A/B runs (nb200_engine_set_gemm_backend) and carries
 // the weight-gradient GEMMs of the training step (reduction over the atom rows: a plain library GEMM).
 // `run_painn` is the one orchestration for inference, the energy-seeded parameter gradients (painn_train.cu) and the force-loss tangent
@@ -226,7 +226,7 @@ int linear_wgrad(nb200_engine* e, cudaStream_t s, int M, int out, int in, const 
                                                                                                                                       : NB200_ECUDA;
 }
 
-// weight-gradient backend: tcgen05 split-K (wgrad_tc.cu) unless NB200_WGRAD=cublas
+// weight-gradient backend: wgmma split-K (wgrad_tc.cu) unless NB200_WGRAD=cublas
 bool wgrad_tc_on() {
     static const bool on = [] { const char* e = getenv("NB200_WGRAD"); return !(e && e[0] == 'c'); }();
     return on;
@@ -429,7 +429,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
     { Scope sc(eng, s, CAT_READOUT, 1); NB_TRY(nb_readout_bwd(ws.ro_pre, w->R2, N, F / 2, ws.g_ro, s)); }
     NB_TRY(linear_bwd(eng, s, N, F / 2, F, ws.g_ro, F / 2, w->R1, F, ws.gq, F, false));
     // energy-seed weight gradients: dW += (c o g)^T x and dbias += colsum(c o g), c = the per-atom seed (`rs_div` rows of g per atom: 3 for the
-    // (atom, xyz) rows of U).  One tcgen05 split-K launch (wgrad_tc.cu: the row scale is applied while loading g); NB200_WGRAD=cublas keeps the
+    // (atom, xyz) rows of U).  One wgmma split-K launch (wgrad_tc.cu: the row scale is applied while loading g); NB200_WGRAD=cublas keeps the
     // round-1 sequence (scale kernel + cuBLAS SGEMM + column-sum kernel).
     // Weight-gradient launches are LEAVES of the step: they read buffers of the backward chain and only add into `grads`.  They run on a
     // second stream of the engine, next to the chain (whose 76-CTA GEMMs and latency-bound phases leave SMs idle): fork = the side stream

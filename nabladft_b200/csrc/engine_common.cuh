@@ -12,7 +12,7 @@ enum { CAT_NBR = 0, CAT_FILTER, CAT_EMBED, CAT_GEMM, CAT_NODE, CAT_MSG_FWD, CAT_
 struct nb200_engine {
     cublasHandle_t blas;
     bool timing = false;
-    int gemm_backend = 1;         // 1 = tcgen05 3xTF32 (gemm_tc.cu), 0 = cuBLAS SGEMM
+    int gemm_backend = 1;         // 1 = wgmma 3xTF32 (gemm_tc.cu), 0 = cuBLAS SGEMM
     int node_backend = 1;         // PaiNN inference: 1 = fused per-layer node kernels (painn_fused.cu), 0 = one launch per Linear / elementwise op
     cudaStream_t side = nullptr;  // PaiNN training: weight-gradient ("leaf") launches run here, next to the backward chain on the caller's stream
     std::vector<cudaEvent_t> side_ev;

@@ -14,7 +14,7 @@
 // (counting sort, 3 tiny kernels); a CTA then owns (bin, split, layer), keeps the 16 band
 // rows of Wrbf for its 4 channels in REGISTERS and streams its edges: 128 FMA per edge per
 // thread instead of 800, no shared/L1 traffic for weights, output rows written once.  r2: with one record per undirected pair the kernel became
-// FMA-bound (256 FFMA per edge-thread = 192 SM-cycles per edge and layer); the band sums use packed FFMA2 (fma.rn.f32x2, bitwise identical).
+// FMA-bound (256 FFMA per edge-thread = 192 SM-cycles per edge and layer).
 //
 // Algorithmic HBM bytes: E*16 (geom) read + L*E*3F*4*(1 or 2) written  (cfg 2: 1.97 GB / 3.9 GB).
 #include <cstdlib>
@@ -23,7 +23,7 @@
 
 #define FLT_THREADS 96   // 3F/4 float4 channel groups for F = 128
 #define FLT_CHUNK 32     // edges staged per phase
-#define FLT_SPLIT 32     // CTAs per (bin, layer): 4 / 8 / 16 / 32 -> 4.74 / 4.66 / 4.63 / 4.61 ms per single-stream step
+#define FLT_SPLIT 32     // CTAs per (bin, layer)
 #define FLT_WSPLIT 48    // CTAs per bin in the weight-gradient kernels (one layer per launch; partial sums end in atomics)
 #define SORT_THREADS 256
 #define SORT_ITEMS 4
@@ -188,8 +188,8 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter(const float* __restrict_
 #pragma unroll
             for (int q4 = 0; q4 < NB_BAND / 4; ++q4) {
                 const float4 p = row4[q4];
-                fma4s_x2(acc0, wreg[4 * q4 + 0], p.x); fma4s_x2(acc0, wreg[4 * q4 + 1], p.y);
-                fma4s_x2(acc0, wreg[4 * q4 + 2], p.z); fma4s_x2(acc0, wreg[4 * q4 + 3], p.w);
+                fma4s(acc0, wreg[4 * q4 + 0], p.x); fma4s(acc0, wreg[4 * q4 + 1], p.y);
+                fma4s(acc0, wreg[4 * q4 + 2], p.z); fma4s(acc0, wreg[4 * q4 + 3], p.w);
             }
             const float4 sc = row4[2 * NB_BAND / 4];
             const size_t off = (size_t)sedge[t] * row_stride + c4;
@@ -200,8 +200,8 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter(const float* __restrict_
 #pragma unroll
                 for (int q4 = 0; q4 < NB_BAND / 4; ++q4) {
                     const float4 p = row4[NB_BAND / 4 + q4];
-                    fma4s_x2(acc1, wreg[4 * q4 + 0], p.x); fma4s_x2(acc1, wreg[4 * q4 + 1], p.y);
-                    fma4s_x2(acc1, wreg[4 * q4 + 2], p.z); fma4s_x2(acc1, wreg[4 * q4 + 3], p.w);
+                    fma4s(acc1, wreg[4 * q4 + 0], p.x); fma4s(acc1, wreg[4 * q4 + 1], p.y);
+                    fma4s(acc1, wreg[4 * q4 + 2], p.z); fma4s(acc1, wreg[4 * q4 + 3], p.w);
                 }
                 float4 dw = bias * sc.w;
                 fma4s(dw, acc0, sc.y);
@@ -263,8 +263,8 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter_wgrad(const float* __res
                 if (t0 + u < nchunk) {
                     const float* row = sphi[t0 + u];
 #pragma unroll
-                    for (int kk = 0; kk < NB_BAND; ++kk) fma4s_x2(acc[kk], g[u], row[kk]);
-                    fma4s_x2(accb, g[u], row[NB_BAND]);
+                    for (int kk = 0; kk < NB_BAND; ++kk) fma4s(acc[kk], g[u], row[kk]);
+                    fma4s(accb, g[u], row[NB_BAND]);
                 }
             }
         }
@@ -334,8 +334,8 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter_wgrad_tan(const float* _
                 if (t0 + u < nchunk) {
                     const float* row = sphi[t0 + u];
 #pragma unroll
-                    for (int kk = 0; kk < NB_BAND; ++kk) { fma4s_x2(acc[kk], gh[u], row[kk]); fma4s_x2(acc[kk], gd[u], row[NB_BAND + kk]); }
-                    fma4s_x2(accb, gh[u], row[2 * NB_BAND]); fma4s_x2(accb, gd[u], row[2 * NB_BAND + 1]);
+                    for (int kk = 0; kk < NB_BAND; ++kk) { fma4s(acc[kk], gh[u], row[kk]); fma4s(acc[kk], gd[u], row[NB_BAND + kk]); }
+                    fma4s(accb, gh[u], row[2 * NB_BAND]); fma4s(accb, gd[u], row[2 * NB_BAND + 1]);
                 }
             }
         }
@@ -351,7 +351,7 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter_wgrad_tan(const float* _
 
 
 // r2: edge-balanced version of the two weight-gradient kernels above.  The (bin, 48 splits) grid ended every one of its 4800 three-warp CTAs
-// in 68 x 96 float atomics -- 31 M atomics per launch, which (not the 285 MB of gradient rows) set the 220 us per layer.  Here a CTA owns
+// in 68 x 96 float atomics -- 31 M atomics per launch, which (not the gradient rows) set the time per layer.  Here a CTA owns
 // ~FW_TARGET consecutive edges of ONE bin in the sorted order (bins get CTAs in proportion to their edge count: no idle CTAs for the
 // empty short-distance bins, no long tail for the crowded ones), its FW_GROUPS warp groups stream disjoint quarters of them with FW_ROWS
 // gradient rows in flight per thread, the groups' band sums are combined through shared memory and flushed ONCE: ~12 x fewer atomics.
@@ -360,8 +360,8 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter_wgrad_tan(const float* _
 #define FW_RING_BYTES 98304
 // Gradient rows travel through a PER-THREAD cp.async ring in shared memory (thread = 4 channels of every row of its group): D rows (or row
 // pairs) ahead of the arithmetic, no registers held, no synchronisation (a thread only ever touches its own 16 / 8 bytes of a slot).  First
-// balanced version: 12 rows per thread in registers, consumed round by round -- 175 us per tangent launch, 51 % of the HBM rate, 12 warps
-// per SM stalled on long_scoreboard + the group barrier (profiles/r2b_k_filter_wgrad_bal_1_float_ncu_full_summary.csv).
+// balanced version: 12 rows per thread in registers, consumed round by round, 12 warps
+// per SM stalled on long_scoreboard + the group barrier.
 template <int BYTES>
 __device__ __forceinline__ void fw_cp_async(void* smem_dst, const void* gmem_src) {
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
@@ -451,11 +451,11 @@ __global__ void __launch_bounds__(FLT_THREADS* FW_GROUPS, 1)
             const float* row = sphi[grp][tt];
 #pragma unroll
             for (int kk = 0; kk < NB_BAND; ++kk) {
-                fma4s_x2(acc[kk], gh, row[kk]);
-                if (TAN) fma4s_x2(acc[kk], gd, row[NB_BAND + kk]);
+                fma4s(acc[kk], gh, row[kk]);
+                if (TAN) fma4s(acc[kk], gd, row[NB_BAND + kk]);
             }
-            fma4s_x2(acc[NB_BAND], gh, row[TAN ? 2 * NB_BAND : NB_BAND]);
-            if (TAN) fma4s_x2(acc[NB_BAND], gd, row[2 * NB_BAND + 1]);
+            fma4s(acc[NB_BAND], gh, row[TAN ? 2 * NB_BAND : NB_BAND]);
+            if (TAN) fma4s(acc[NB_BAND], gd, row[2 * NB_BAND + 1]);
         }
         asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "n"(FLT_THREADS) : "memory");
     }

@@ -3,13 +3,12 @@
 // Replaces the round-1 3xTF32 kernels of gemm_tc.cu where they were slowest: torch.nn.Linear / e3nn FullyConnectedNet layers applied to every
 // atom pair or edge (QHNet weight generation [1e5 x 8320 x 128], qhnet/layers.py:191-203,376-459; GemNet-OC Dense layers [6e5 x 512 x 512],
 // gemnet_oc/layers/base_layers.py; the unfused PaiNN / SchNet paths).  There the MMA issuer idled 70 % of the time waiting for producer
-// warps that split the WEIGHT operand into TF32 hi / lo again for every 128-row slab (profiles/r1_gemm_variants.md).  Here
+// warps that split the WEIGHT operand into TF32 hi / lo again for every 128-row slab.  Here
 //   * the weight matrix is split ONCE per call into ready-made shared-memory tile images (k_prep_gemm, 128 KB per 128 x 128 tile) in a scratch
 //     buffer, and streamed by single cp.async.bulk copies -- nobody splits weights inside the GEMM;
-//   * the activation slab [128 rows x 128 k] is split once per CTA (K <= 128) or once per (N tile, K chunk);
-//   * D[out feature, row] orientation: an epilogue thread owns one output feature and 32 rows, so C stores are 128-byte coalesced per warp;
-//   * TMEM staging decouples the epilogue of tile t from the MMAs of tile t + 1.
-// Measured (tools/gemm_microbench.py, B200): see profiles/r2_gemm_ps.md.
+//   * the activation slab [64 rows x 128 k] is split once per CTA (K <= 128) or once per (N tile, K chunk);
+//   * D[out feature, row] orientation: an epilogue thread owns one output feature and 32 rows (64 with two worker groups), so C stores are 128-byte coalesced per warp;
+//   * the shared-memory staging tile decouples the epilogue of tile t from the MMAs of tile t + 1.
 #include <map>
 #include <mutex>
 
@@ -69,21 +68,17 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
     const int t_begin = blockIdx.y * P.tiles_per_cta, t_end = min(t_begin + P.tiles_per_cta, P.n_nt);
     if (t_begin >= t_end) return;
     const int n_it = t_end - t_begin, KC = P.KC, n_units = n_it * KC;
-    Ctx c = setup(smem, tid, warp, P.xsplit);
+    Ctx c = setup(smem, tid, P.xsplit);
     NF_PROF_DO(const long long tk0_ = clock64(); long long w_epi_ = 0;)
     // unit u = (N tile t_begin + u / KC, K chunk u % KC).  K <= 128: the activation slab is written once and stays; else once per unit.
     auto flags_of = [&](int u) {
         const int kc = u % KC;
         return ((KC > 1 || u == 0) ? U_NEWX : 0) | (kc == 0 ? U_FIRST : 0) | (kc == KC - 1 ? U_LAST : 0) | ((KC > 1 || u == n_units - 1) ? U_XLAST : 0);
     };
-    if (warp == NWORK) {
-        if (lane == 0) run_producer_t(c, n_units, P.wt, [&](int u) { return (t_begin + u / KC) * KC + u % KC; }, P.spt);
-    } else if (warp == NWORK + 1) {
-        if (lane == 0) {
-            run_issuer_t(c, n_units, flags_of, P.spt);
-            NF_PROF_DO(atomicAdd(&g_nf_prof[0], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[1], (unsigned long long)c.w_x);
-                       atomicAdd(&g_nf_prof[2], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[3], (unsigned long long)c.w_full);)
-        }
+    if (warp >= WARP_ISSUE) {
+        run_issuer_t(c, n_units, flags_of, [&](int u) { return (t_begin + u / KC) * KC + u % KC; }, P.wt, P.spt);
+        NF_PROF_DO(if (warp == WARP_ISSUE && lane == 0) { atomicAdd(&g_nf_prof[0], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[1], (unsigned long long)c.w_x);
+                   atomicAdd(&g_nf_prof[2], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[3], (unsigned long long)c.w_full); })
     } else {
         const int M = P.M, m0 = blockIdx.x * NT;
         const int fl = 32 * (warp & 3) + lane, n0 = CPT * (warp >> 2);
@@ -105,7 +100,6 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
                 const int n = (t_begin + u / KC) * 128 + fl;
                 drain(c, warp);
                 NF_PROF_DO(const long long te0_ = clock64();)
-                // NOTE every lane runs the chunk loop (tcgen05.ld is warp-collective); lanes beyond N only skip their loads / stores
                 const bool n_ok = n < P.N;
                 const float b = (P.bias && n_ok) ? __ldg(P.bias + n) : 0.f;
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
@@ -139,7 +133,6 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
     }
     NF_PROF_DO(if (tid == 0) { atomicAdd(&g_nf_prof[4], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[5], (unsigned long long)c.w_acc);
                             atomicAdd(&g_nf_prof[6], (unsigned long long)c.w_xfree); atomicAdd(&g_nf_prof[7], 1ull); atomicAdd(&g_nf_prof[8], (unsigned long long)w_epi_); })
-    teardown(c, warp);
 }
 
 // grow-only scratch for the prepared weights, one per (thread, stream): calls on one stream are ordered, so the buffer is reused safely
@@ -150,14 +143,14 @@ thread_local std::map<cudaStream_t, Scratch> g_scratch;
 
 // This file is compiled TWICE: as itself (all 16 worker warps load operands and run epilogues, in program order) and, through gemm_ps2.cu, with
 // NF_TWO_GROUPS (8 loader warps run ahead of 8 epilogue warps, tc_pipe.cuh) -- the build used for K > 128, where the finished tile's drain + 64 KB
-// of stores (5.6 k cycles, profiles/r2b_gemm_ps_role_timing.txt) otherwise delay the next activation operand.  The second build exports only
+// of stores otherwise delay the next activation operand.  The second build exports only
 // nb_gemm_ps_impl_2g.
 int nb_gemm_ps_impl_2g(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate, const float* bias,
                        float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, int epi, float epi_alpha);
 #ifndef NB_GEMM_PS_2G
 size_t nb_gemm_ps_ws_bytes(int N, int K) { return (size_t)((N + 127) / 128) * ((K + 127) / 128) * WTILE_BYTES; }
 
-// heuristics measured on B200 (profiles/r2_gemm_ps.md): worth it when the weight preparation is amortised over many row slabs
+// worth it when the weight preparation is amortised over many row slabs
 // (K = 32: the radial-basis layers of QHNet's convolution, [E, 32] x [32, 5376] -- one stage per tile, bound by the output write)
 bool nb_gemm_ps_wanted(int M, int N, int K) { return M >= 2048 && N >= 64 && K >= 32 && K % 4 == 0; }
 #endif
@@ -200,7 +193,7 @@ static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const floa
     P.xsplit = (KC > 1) ? xs_on : 0;
     const int m_tiles = (M + NT - 1) / NT;
     int ny = 1;
-    while (m_tiles * ny < 148 && ny < n_nt) ++ny;  // few row slabs: split the N walk (the activation slab is re-staged per CTA)
+    while (m_tiles * ny < nb_sm_count() && ny < n_nt) ++ny;  // few row slabs: split the N walk (the activation slab is re-staged per CTA)
     P.tiles_per_cta = (n_nt + ny - 1) / ny;
     dim3 grid(m_tiles, (n_nt + P.tiles_per_cta - 1) / P.tiles_per_cta);
     k_gemm_ps<<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
@@ -265,7 +258,7 @@ int nb_gemm_ps_lm(int M, int N, int K, const float* A, int lda, const float* W_l
 #endif  // !NB_GEMM_PS_2G
 
 #if defined(NF_PROF) && !defined(NB_GEMM_PS_2G)
-// role timing of k_gemm_ps (tools/gemm_ps_prof.py): [0] issuer total, [1] issuer waits X, [2] issuer waits TMEM buffers, [3] issuer waits W ring,
+// role timing of k_gemm_ps (tools/gemm_ps_prof.py): [0] issuer total, [1] issuer waits X, [2] issuer waits staging, [3] issuer waits W ring,
 // [4] worker thread 0 total, [5] worker waits accumulator (incl. drain), [6] worker waits X release, [7] CTAs, [8] worker epilogue (stores)
 extern "C" int nb200_debug_gemm_ps_prof(unsigned long long* out16, int reset) {
     if (cudaMemcpyFromSymbol(out16, g_nf_prof, sizeof(unsigned long long) * 16) != cudaSuccess) return -1;

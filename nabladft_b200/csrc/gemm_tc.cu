@@ -1,14 +1,13 @@
-// gemm_tc.cu -- node-level dense layers on the 5th-gen tensor cores (tcgen05 + TMEM), fp32-accurate.
+// gemm_tc.cu -- node-level dense layers on the Hopper tensor cores (wgmma), fp32-accurate.
 //
 // Replaces the cuBLAS SGEMM calls of engine.cu (torch.nn.Linear forward / input-gradient of
-// nablaDFT/painn_pyg/painn.py:459-464,520-525 and the schnetpack Dense layers).  cuBLAS picks
-// a 64x32x16 SIMT tile for these skinny problems (M ~ 10^4 atoms, N,K in {64..384}) and runs at
-// ~25 TFLOP/s: 2.1 ms of a 4.6 ms step (profiles/r1_v0_launches.csv).
+// nablaDFT/painn_pyg/painn.py:459-464,520-525 and the schnetpack Dense layers) for the skinny
+// problems of this model (M ~ 10^4 atoms, N,K in {64..384}).
 //
 // The reference never uses reduced precision (SURVEY.md section 0.9), so single-pass TF32 is
 // out.  We use the 3xTF32 split: x = hi + lo with hi = tf32_rn(x), lo = tf32_rn(x - hi);
 //   A.B ~= A_hi.B_hi + A_hi.B_lo + A_lo.B_hi       (dropped term ~2^-24 relative)
-// three `tcgen05.mma.kind::tf32` per k-step accumulating in fp32 in TMEM.  The operands are
+// three `wgmma.mma_async ... .tf32` per k-step accumulating in fp32 registers.  The operands are
 // split on the fly while they are staged from global into shared memory by the CTA's threads
 // (canonical no-swizzle K-major layout: 16-byte k-chunks, rows contiguous), so activations
 // never need a pre-pass and weights need no transposed copies (`trans_b` loads B^T directly).
@@ -16,70 +15,24 @@
 //   C[M,N] (ldc) = A[M,K] (lda) . op(B)  (+ C if accumulate)  (+ bias[N])
 //   op(B) = B[N,K]^T (ldb, trans_b = 0: Linear forward)  |  B[K,N] (ldb, trans_b = 1: Linear backward)
 //   optional second output  act[M,N] = silu(C)   (C then holds the pre-activation)
-// Two kernels (dispatch in nb_gemm_tf32x3_ex, measurements in profiles/r1_gemm_variants.md):
-//   k_gemm_tf32x3<64>      tile kernel 128 x 64 x 32, 512 threads, two CTAs per SM, double-buffered stages with register prefetch, one
-//                          elected thread issues the MMAs, `tcgen05.commit` -> mbarrier releases a stage.  Used for K > 128 and N = 64.
-//   k_gemm_tf32x3_wide<3>  warp-specialised, A slab resident in shared memory, N = 128 per MMA, rotating TMEM buffers.  K <= 128, N >= 128.
+// k_gemm_tf32x3: tile 128 x 64 x 32, 512 threads = four warpgroups (each a 64 x 32 quarter of the tile), double-buffered stages with
+// register prefetch.  Tall problems go to the pre-split-weight kernel of gemm_ps.cu.
 #include <cstdlib>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int G_BM = 128;
+constexpr int G_BN = 64;
 constexpr int G_BK = 32;
-constexpr int G_THREADS = 512;  // 16 warps: the hi/lo split is SIMT work; with 4 warps per CTA the SM ran at IPC 0.5 (ncu)
+constexpr int G_THREADS = 512;  // 16 warps: the hi/lo split is SIMT work and wants many threads
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): K-major, SWIZZLE_NONE
-// start>>4 [0,14) | LBO>>4 [16,30) (stride between 16-byte k-chunks) | SBO>>4 [32,46) (stride
-// between 8-row groups) | version=1 [46,48) | layout_type=0 [61,64)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=F32 [4,6)=1, A=TF32 [7,10)=2, B=TF32
-// [10,13)=2, A/B K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-__device__ __forceinline__ void mbar_init_(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        "@P1 bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}\n" ::"r"(s_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-
 // round-to-nearest split (cvt.rna.tf32.f32): |x - hi| <= 2^-12 |x| and the rounding of lo costs
-// 2^-24 |x| -- fp32-level and unbiased.  (Masking the low 13 bits instead truncates toward zero:
-// measured 2e-6 relative drift of the model energy against the SGEMM path.)
+// 2^-24 |x| -- fp32-level and unbiased.  (Masking the low 13 bits instead truncates toward zero.)
 __device__ __forceinline__ float tf32_rn(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -94,23 +47,19 @@ __device__ __forceinline__ void split4(const float4 v, float4& hi, float4& lo) {
 }
 
 // element (row r, k) of a [ROWS x 32] stage tile lives at float index ((k/4)*ROWS + r)*4 + k%4
-template <int BN>
 struct Stage {
-    float a_hi[G_BM * G_BK], a_lo[G_BM * G_BK], b_hi[BN * G_BK], b_lo[BN * G_BK];
+    float a_hi[G_BM * G_BK], a_lo[G_BM * G_BK], b_hi[G_BN * G_BK], b_lo[G_BN * G_BK];
 };
 
-template <int BN>
-__global__ void __launch_bounds__(G_THREADS, 2) k_gemm_tf32x3(int M, int N, int K, const float* __restrict__ A, int lda,
+__global__ void __launch_bounds__(G_THREADS, 1) k_gemm_tf32x3(int M, int N, int K, const float* __restrict__ A, int lda,
                                                              const float* __restrict__ B, int ldb, int trans_b, float* C, int ldc,
                                                              int accumulate, const float* __restrict__ bias, float* __restrict__ act, int act_kind,
                                                              int batch_kind, long long a_boff, long long b_boff, long long c_boff) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    Stage<BN>* stages = reinterpret_cast<Stage<BN>*>(smem_raw);
-    uint64_t* mma_done = reinterpret_cast<uint64_t*>(smem_raw + 2 * sizeof(Stage<BN>));
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(mma_done + 2);
+    Stage* stages = reinterpret_cast<Stage*>(smem_raw);
 
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const int m0 = blockIdx.x * G_BM, n0 = blockIdx.y * BN;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int m0 = blockIdx.x * G_BM, n0 = blockIdx.y * G_BN;
     if (batch_kind != 0) {
         // batch over blockIdx.z: A and C advance by a fixed offset; B is selected per batch entry.
         // kind 1 = "lm blocks" of an equivariant feature [rows][(l,m)][channels]: z = (l,m) index,
@@ -124,34 +73,24 @@ __global__ void __launch_bounds__(G_THREADS, 2) k_gemm_tf32x3(int M, int N, int 
         if (batch_kind == 1 && z > 0) bias = nullptr;
     }
 
-    if (tid == 0) {
-        mbar_init_(mma_done, 1);
-        mbar_init_(mma_done + 1, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {  // TMEM: 4 accumulators (3 main round-robin + 1 correction) x BN fp32 columns x 128 lanes
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "n"(4 * BN) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_acc = *tmem_slot;
-
-    constexpr uint32_t IDESC = umma_idesc_tf32(G_BM, BN);
-    constexpr int BPT = BN * (G_BK / 4) / G_THREADS;  // B float4 per thread per chunk (8 for BN=128, 4 for BN=64)
-    constexpr int BSPLIT = G_THREADS / BN;            // threads sharing one B row (1 or 2)
+    constexpr int BPT = G_BN * (G_BK / 4) / G_THREADS;  // B float4 per thread per chunk
     const int n_chunks = K / G_BK;
     constexpr int APT = G_BM * (G_BK / 4) / G_THREADS;  // A float4 per thread per chunk
     const int atile_row = tid % G_BM;                 // this thread stages k-chunks [akc0, akc0 + APT) of row `atile_row` of the A tile
     const int akc0 = (tid / G_BM) * APT;
     const int arow = m0 + atile_row;
     const bool arow_ok = arow < M;
-    const int btile_row = tid % BN;                   // and k-chunks [bkc0, bkc0 + BPT) of row `btile_row` of the B tile
-    const int bkc0 = (tid / BN) * BPT;
+    const int btile_row = tid % G_BN;                 // and k-chunks [bkc0, bkc0 + BPT) of row `btile_row` of the B tile
+    const int bkc0 = (tid / G_BN) * BPT;
     const int brow = n0 + btile_row;
     const bool brow_ok = brow < N;
-    (void)BSPLIT;
+    // warpgroup g computes rows [64 (g & 1), +64) x columns [32 (g >> 1), +32) of the tile
+    const int wg = warp >> 2, mh = wg & 1, nh = wg >> 1;
+    // The tensor core truncates when it adds into the fp32 accumulator, so the error grows with the chain length: the O(2^-11)
+    // correction terms get their own accumulator and the main term alternates over two; the three are summed with RN adds at the end.
+    float corr[16], acc0[16], acc1[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) { corr[i] = 0.f; acc0[i] = 0.f; acc1[i] = 0.f; }
 
     // global -> registers (issued one chunk ahead of the shared-memory stores: the L2 latency of
     // chunk c+1 overlaps the split/store/MMA of chunk c)
@@ -175,11 +114,11 @@ __global__ void __launch_bounds__(G_THREADS, 2) k_gemm_tf32x3(int M, int N, int 
             rb[i] = v;
         }
     };
-    // registers -> hi/lo split -> shared ([k-chunk][row] 16-byte units: conflict-free), then MMAs
+    // registers -> hi/lo split -> shared ([k-chunk][row] 16-byte units: conflict-free), then the MMAs of this warpgroup
     auto process = [&](int ch, const float4 (&ra)[APT], const float4 (&rb)[BPT]) {
-        const int s = ch & 1, use = ch >> 1;
-        if (use > 0) mbar_wait_(mma_done + s, (uint32_t)((use - 1) & 1));  // MMAs that read this buffer are done
-        Stage<BN>& st = stages[s];
+        const int s = ch & 1;
+        __syncthreads();  // every warpgroup has waited for its MMAs of chunk ch - 2, which read this buffer
+        Stage& st = stages[s];
 #pragma unroll
         for (int i = 0; i < APT; ++i) {
             float4 hi, lo;
@@ -191,31 +130,26 @@ __global__ void __launch_bounds__(G_THREADS, 2) k_gemm_tf32x3(int M, int N, int 
         for (int i = 0; i < BPT; ++i) {
             float4 hi, lo;
             split4(rb[i], hi, lo);
-            st4(st.b_hi + ((bkc0 + i) * BN + btile_row) * 4, hi);
-            st4(st.b_lo + ((bkc0 + i) * BN + btile_row) * 4, lo);
+            st4(st.b_hi + ((bkc0 + i) * G_BN + btile_row) * 4, hi);
+            st4(st.b_lo + ((bkc0 + i) * G_BN + btile_row) * 4, lo);
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy smem writes -> visible to the MMA (async proxy)
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            uint64_t dah = umma_desc(s_u32(st.a_hi), G_BM * 16, 128), dal = umma_desc(s_u32(st.a_lo), G_BM * 16, 128);
-            uint64_t dbh = umma_desc(s_u32(st.b_hi), BN * 16, 128), dbl = umma_desc(s_u32(st.b_lo), BN * 16, 128);
+        const uint32_t ah = s_u32(st.a_hi) + mh * 64 * 16, al = s_u32(st.a_lo) + mh * 64 * 16;
+        const uint32_t bh = s_u32(st.b_hi) + nh * 32 * 16, bl = s_u32(st.b_lo) + nh * 32 * 16;
+        wgmma_fence();
 #pragma unroll
-            for (int ks = 0; ks < G_BK / 8; ++ks) {  // one MMA = 8 k-values = two 16-byte chunks
-                // The tensor core truncates when it adds into the fp32 accumulator: the error grows
-                // linearly with the chain length (measured 7.6e-9 * K relative with one accumulator).
-                // So: the O(2^-11) correction terms get their own accumulator, and the main term
-                // rotates over three accumulators; the four are summed with RN adds in the epilogue.
-                const int g = ch * (G_BK / 8) + ks;
-                umma_tf32(tmem_acc + 3 * BN, dal, dbh, IDESC, g > 0 ? 1u : 0u);
-                umma_tf32(tmem_acc + 3 * BN, dah, dbl, IDESC, 1u);
-                umma_tf32(tmem_acc + (g % 3) * BN, dah, dbh, IDESC, g >= 3 ? 1u : 0u);
-                dah += (2 * G_BM * 16) >> 4; dal += (2 * G_BM * 16) >> 4;  // start-address field counts 16-byte units
-                dbh += (2 * BN * 16) >> 4; dbl += (2 * BN * 16) >> 4;
-            }
-            // arrives on the mbarrier when every MMA issued so far has completed (implies fence::before_thread_sync)
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s_u32(mma_done + s)) : "memory");
+        for (int ks = 0; ks < G_BK / 8; ++ks) {  // one MMA = 8 k-values = two 16-byte chunks
+            const uint32_t ao = ks * 2 * G_BM * 16, bo = ks * 2 * G_BN * 16;
+            const uint64_t dah = gmma_desc(ah + ao, G_BM * 16, 128), dal = gmma_desc(al + ao, G_BM * 16, 128);
+            const uint64_t dbh = gmma_desc(bh + bo, G_BN * 16, 128), dbl = gmma_desc(bl + bo, G_BN * 16, 128);
+            wgmma_tf32_n32(corr, dal, dbh);
+            wgmma_tf32_n32(corr, dah, dbl);
+            if (ks & 1) wgmma_tf32_n32(acc1, dah, dbh);
+            else wgmma_tf32_n32(acc0, dah, dbh);
         }
+        wgmma_commit();
+        wgmma_wait<1>();  // chunk ch - 1 has completed (its buffer is rewritten after the next barrier)
     };
 
     {
@@ -230,356 +164,40 @@ __global__ void __launch_bounds__(G_THREADS, 2) k_gemm_tf32x3(int M, int N, int 
             }
         }
     }
-    {   // accumulator complete when the last chunk's commit has arrived (MMAs retire in order)
-        const int last = n_chunks - 1;
-        mbar_wait_(mma_done + (last & 1), (uint32_t)((last >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    // ---- epilogue: warp w owns TMEM lanes [32w, 32w+32) == tile rows; thread = one row, 32 columns per load
-    // warp w may touch TMEM lanes [32 (w % 4), +32) only; the column range is split over the warp quads
-    constexpr int COLS_PER_WARP = BN / (G_THREADS / 128);
-    const int lane_grp = warp & 3;
-    const int row = m0 + lane_grp * 32 + (tid & 31);
-#pragma unroll 1
-    for (int cb = (warp >> 2) * COLS_PER_WARP; cb < ((warp >> 2) + 1) * COLS_PER_WARP; cb += 16) {
-        uint32_t r[4][16];
+    wgmma_wait<0>();
+    // ---- epilogue from the fragments: rows 64 mh + 16 (warp & 3) + lane / 4 (+ 8), columns 32 nh + 8 j + 2 (lane & 3) (+ 1)
+    const int r0 = m0 + 64 * mh + 16 * (warp & 3) + (lane >> 2);
 #pragma unroll
-        for (int acc = 0; acc < 4; ++acc) {
-            const uint32_t taddr = tmem_acc + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(acc * BN + cb);
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                : "=r"(r[acc][0]), "=r"(r[acc][1]), "=r"(r[acc][2]), "=r"(r[acc][3]), "=r"(r[acc][4]), "=r"(r[acc][5]), "=r"(r[acc][6]),
-                  "=r"(r[acc][7]), "=r"(r[acc][8]), "=r"(r[acc][9]), "=r"(r[acc][10]), "=r"(r[acc][11]), "=r"(r[acc][12]), "=r"(r[acc][13]),
-                  "=r"(r[acc][14]), "=r"(r[acc][15])
-                : "r"(taddr)
-                : "memory");
-        }
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        float v16[16];
+    for (int j = 0; j < 4; ++j) {
+        const int n = n0 + 32 * nh + 8 * j + 2 * (lane & 3);
+        if (n >= N) continue;  // N % 4 == 0: n < N implies n + 1 < N
+        const float2 b = bias ? __ldg(reinterpret_cast<const float2*>(bias + n)) : make_float2(0.f, 0.f);
 #pragma unroll
-        for (int t = 0; t < 16; ++t)
-            v16[t] = (__uint_as_float(r[0][t]) + __uint_as_float(r[1][t])) + (__uint_as_float(r[2][t]) + __uint_as_float(r[3][t]));
-        if (row < M) {
-            const int nb = n0 + cb;
-            float* crow = C + (size_t)row * ldc + nb;
-            float* arow_out = act ? act + (size_t)row * ldc + nb : nullptr;
-#pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4) {
-                if (nb + 4 * q4 < N) {
-                    float4 v = make_float4(v16[4 * q4], v16[4 * q4 + 1], v16[4 * q4 + 2], v16[4 * q4 + 3]);
-                    if (bias) v = v + ldg4(bias + nb + 4 * q4);
-                    if (accumulate) v = v + *reinterpret_cast<const float4*>(crow + 4 * q4);
-                    st4(crow + 4 * q4, v);
-                    if (arow_out) st4(arow_out + 4 * q4, make_float4(actf_(v.x, act_kind), actf_(v.y, act_kind), actf_(v.z, act_kind), actf_(v.w, act_kind)));
-                }
-            }
+        for (int hr = 0; hr < 2; ++hr) {
+            const int row = r0 + 8 * hr;
+            if (row >= M) continue;
+            const int e = 4 * j + 2 * hr;
+            float2 v = make_float2((corr[e] + acc0[e]) + acc1[e] + b.x, (corr[e + 1] + acc0[e + 1]) + acc1[e + 1] + b.y);
+            float2* cp = reinterpret_cast<float2*>(C + (size_t)row * ldc + n);
+            if (accumulate) { const float2 o = *cp; v.x += o.x; v.y += o.y; }
+            *cp = v;
+            if (act) *reinterpret_cast<float2*>(act + (size_t)row * ldc + n) = make_float2(actf_(v.x, act_kind), actf_(v.y, act_kind));
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(4 * BN) : "memory");
 }
 
-template <int BN>
 int launch(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
            const float* bias, float* act, int act_kind, int batch_kind, int n_batch, long long a_boff, long long b_boff, long long c_boff,
            cudaStream_t s) {
-    const int smem = 2 * (int)sizeof(Stage<BN>) + 64;
+    const int smem = 2 * (int)sizeof(Stage);
     static bool attr_set = false;
     if (!attr_set) {
-        if (cudaFuncSetAttribute(k_gemm_tf32x3<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return nb_check_launch();
+        if (cudaFuncSetAttribute(k_gemm_tf32x3, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return nb_check_launch();
         attr_set = true;
     }
-    dim3 grid((M + G_BM - 1) / G_BM, (N + BN - 1) / BN, batch_kind ? n_batch : 1);
-    k_gemm_tf32x3<BN><<<grid, G_THREADS, smem, s>>>(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, batch_kind, a_boff,
-                                                    b_boff, c_boff);
-    return nb_check_launch();
-}
-
-constexpr int AS_KMAX = 128;  // K per resident A slab
-// ---------------------------------------------------------------------------------------------------------
-// Warp-specialised wide-N kernel (the shipped one for N >= 128).
-//
-// What the earlier variants taught (profiles/r1_gemm_ws_roles.txt): with N = 32..64 per MMA the issuing thread spends
-// ~67 cycles per `tcgen05.mma` although the math floor is 128 N / 256 = 16 cycles: every M=128,K=8 tf32 MMA re-reads a
-// 4 KB A operand (128 B/clk from shared memory, 64 B/clk from TMEM), so narrow N is operand-fetch bound, and the lock-step
-// kernels added a CTA barrier per tile on top.  Here N = 128 per MMA (fetch 32 + 32 = 64 cycles = math 64 cycles) and the
-// roles never meet at a CTA barrier in steady state:
-//   warps 0-7   epilogue : wait acc_full -> tcgen05.ld (lane group w&3, column half w>>2) -> release each TMEM buffer as soon
-//                          as it is in registers -> RN sum of the buffers, bias / += / activation -> C (256 B runs per thread)
-//   warps 8-11  producer : global B [128 n x 32 k] -> hi/lo split -> shared stage (ring of 3, mbarrier full/empty)
-//   warp  12    issuer   : per 32-k stage 12 x tcgen05.mma (A, B from shared memory) -> commit frees the stage; after the
-//                          last stage of a tile commit -> acc_full
-// A slab [128 x K<=128] is split once per CTA into 128 KB of shared memory.  TMEM = 4 buffers x 128 columns; a tile takes
-// W_NB consecutive buffers (mod 4): one for the O(2^-11) correction terms, W_NB-1 for the main term (rotating: the tensor core
-// truncates on accumulate, so the chain per accumulator is kept short).  W_NB = 2 double-buffers tiles exactly.
-constexpr int W_BN = 128;
-constexpr int W_BK = 32;
-constexpr int W_STAGES = 3;
-// k-chunk stride (UMMA "leading byte offset") padded by 16 B: 8 lanes that stage the 8 chunks of one row then hit 8 different
-// bank groups instead of one (the MMA reads whole 128-byte core matrices and does not care)
-constexpr int W_LBO = G_BM * 16 + 16;                      // bytes; A and B tiles both have 128 rows
-constexpr int W_LBOF = W_LBO / 4;                          // floats
-constexpr int W_A_FLOATS = (AS_KMAX / 4) * W_LBOF;         // one of hi / lo
-constexpr int W_B_FLOATS = (W_BK / 4) * W_LBOF;            // one of hi / lo of a stage
-constexpr int W_EPI_WARPS = 8, W_PROD_WARPS = 4;
-constexpr int W_THREADS = 32 * (W_EPI_WARPS + W_PROD_WARPS + 1);
-#ifdef NB_WS_PROF
-__device__ unsigned long long g_ws_prof[8];  // 0 producer wait-empty, 1 producer total, 2 issuer wait-full, 3 issuer wait-acc, 4 issuer total, 5 epi wait, 6 epi total, 7 CTAs
-#define WS_PROF(...) __VA_ARGS__
-#else
-#define WS_PROF(...)
-#endif
-
-__device__ __forceinline__ void mbar_arrive_(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_commit_(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s_u32(bar)) : "memory");
-}
-
-template <int W_NB>
-__global__ void __launch_bounds__(W_THREADS, 1) k_gemm_tf32x3_wide(int M, int N, int K, const float* __restrict__ A, int lda,
-                                                                  const float* __restrict__ B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-                                                                  const float* __restrict__ bias, float* __restrict__ act, int act_kind,
-                                                                  int tiles_per_cta) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    float* a_hi = reinterpret_cast<float*>(smem_raw);               // [K/4 chunks][128 rows][4]
-    float* a_lo = a_hi + W_A_FLOATS;
-    float* b_buf = a_lo + W_A_FLOATS;                                // [W_STAGES][hi|lo][8 chunks][128 n][4]
-    uint64_t* full = reinterpret_cast<uint64_t*>(b_buf + W_STAGES * 2 * W_B_FLOATS);
-    uint64_t* empty = full + W_STAGES;
-    uint64_t* acc_full = empty + W_STAGES;
-    uint64_t* buf_empty = acc_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(buf_empty + 4);
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m0 = blockIdx.x * G_BM;
-    const int n_tiles_total = (N + W_BN - 1) / W_BN;
-    const int t_begin = blockIdx.y * tiles_per_cta, t_end = min(t_begin + tiles_per_cta, n_tiles_total);
-    if (t_begin >= t_end) return;
-    const int n_it = t_end - t_begin;
-    const int n_kst = K / W_BK;  // stages per tile
-
-    if (tid == 0) {
-        for (int s_ = 0; s_ < W_STAGES; ++s_) { mbar_init_(full + s_, 32 * W_PROD_WARPS); mbar_init_(empty + s_, 1); }
-        for (int a_ = 0; a_ < 2; ++a_) mbar_init_(acc_full + a_, 1);
-        for (int b_ = 0; b_ < 4; ++b_) mbar_init_(buf_empty + b_, 32 * W_EPI_WARPS);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    // ---- A slab -> shared (all threads except the issuer warp), split on the way
-    if (warp < W_EPI_WARPS + W_PROD_WARPS) {
-        const int kch = K / 4;
-        for (int item = tid; item < G_BM * kch; item += 32 * (W_EPI_WARPS + W_PROD_WARPS)) {
-            const int kc = item % kch, r = item / kch;  // consecutive lanes walk a row: coalesced
-            const int row = m0 + r;
-            const float4 v = (row < M) ? ldg4(A + (size_t)row * lda + 4 * kc) : f4(0.f);
-            float4 hi, lo;
-            split4(v, hi, lo);
-            st4(a_hi + kc * W_LBOF + r * 4, hi);
-            st4(a_lo + kc * W_LBOF + r * 4, lo);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    constexpr uint32_t IDESC = umma_idesc_tf32(G_BM, W_BN);
-    WS_PROF(long long ew_total = 0, et_total = 0;)
-    if (warp >= W_EPI_WARPS && warp < W_EPI_WARPS + W_PROD_WARPS) {
-        // ================= producers: stage q = (tile, k-quarter)
-        const int ptid = tid - 32 * W_EPI_WARPS;
-        auto load_b = [&](int q, float4 (&rb)[8]) {
-            const int t = t_begin + q / n_kst, k0 = (q % n_kst) * W_BK;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int item = ptid + i * 128;
-                float4 v = f4(0.f);
-                if (!trans_b) {
-                    const int kc = item & 7, n = item >> 3;  // 8 lanes cover one 128-byte line of a weight row
-                    const int gn = t * W_BN + n;
-                    if (gn < N) v = ldg4(B + (size_t)gn * ldb + k0 + 4 * kc);
-                } else {
-                    const int n = item & 127, kc = item >> 7;  // lanes walk n: coalesced rows of B[K][N]
-                    const int gn = t * W_BN + n;
-                    if (gn < N) {
-                        const float* p = B + (size_t)(k0 + 4 * kc) * ldb + gn;
-                        v = make_float4(__ldg(p), __ldg(p + ldb), __ldg(p + 2 * (size_t)ldb), __ldg(p + 3 * (size_t)ldb));
-                    }
-                }
-                rb[i] = v;
-            }
-        };
-        // two register sets: the loads of stage q + 2 are issued before stage q + 1 is split and stored, so ~2 x 16 KB per CTA stay in
-        // flight -- with one set the producers were the critical path (ncu: 9 warp-cycles of long_scoreboard per issue; the issuer idled
-        // 70 % of the time on `full`): the L2 latency under 700+ CTAs reading the same weight rows is ~1.2 k cycles per stage.
-        float4 ra[8], rb[8];
-        const int n_q = n_it * n_kst;
-        WS_PROF(long long pw = 0; const long long pt0 = clock64();)
-        auto stage = [&](int q, const float4 (&r)[8]) {
-            const int s_ = q % W_STAGES, use = q / W_STAGES;
-            WS_PROF(const long long c0 = clock64();)
-            if (use > 0) mbar_wait_(empty + s_, (uint32_t)((use - 1) & 1));  // the MMAs that read this stage have retired
-            WS_PROF(pw += clock64() - c0;)
-            float* bh = b_buf + s_ * 2 * W_B_FLOATS;
-            float* bl = bh + W_B_FLOATS;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int item = ptid + i * 128;
-                const int kc = trans_b ? (item >> 7) : (item & 7), n = trans_b ? (item & 127) : (item >> 3);
-                float4 hi, lo;
-                split4(r[i], hi, lo);
-                st4(bh + kc * W_LBOF + n * 4, hi);
-                st4(bl + kc * W_LBOF + n * 4, lo);
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_arrive_(full + s_);
-        };
-        load_b(0, ra);
-        if (n_q > 1) load_b(1, rb);
-        for (int q = 0; q < n_q; q += 2) {
-            stage(q, ra);
-            if (q + 2 < n_q) load_b(q + 2, ra);
-            if (q + 1 < n_q) {
-                stage(q + 1, rb);
-                if (q + 3 < n_q) load_b(q + 3, rb);
-            }
-        }
-        WS_PROF(if (ptid == 0) { atomicAdd(&g_ws_prof[0], (unsigned long long)pw); atomicAdd(&g_ws_prof[1], (unsigned long long)(clock64() - pt0)); })
-    } else if (warp == W_EPI_WARPS + W_PROD_WARPS) {
-        // ================= MMA issuer (one lane)
-        if (lane == 0) {
-            WS_PROF(long long wf = 0, wa = 0; const long long it0 = clock64();)
-            const uint64_t da_hi0 = umma_desc(s_u32(a_hi), W_LBO, 128), da_lo0 = umma_desc(s_u32(a_lo), W_LBO, 128);
-            int q = 0;
-            for (int it = 0; it < n_it; ++it) {
-                // buffers of this tile: position p = it * W_NB + j -> buffer p & 3, use count p >> 2
-                const int p0 = it * W_NB;
-                const uint32_t acc_corr = tmem_base + (uint32_t)(((p0)&3) * W_BN);
-                WS_PROF(const long long c1 = clock64();)
-#pragma unroll
-                for (int j = 0; j < W_NB; ++j) {
-                    const int p = p0 + j;
-                    if ((p >> 2) > 0) mbar_wait_(buf_empty + (p & 3), (uint32_t)(((p >> 2) - 1) & 1));
-                }
-                WS_PROF(wa += clock64() - c1;)
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                uint64_t da_hi = da_hi0, da_lo = da_lo0;
-                int ks_tile = 0;
-                for (int kq = 0; kq < n_kst; ++kq, ++q) {
-                    const int s_ = q % W_STAGES;
-                    WS_PROF(const long long c0 = clock64();)
-                    mbar_wait_(full + s_, (uint32_t)((q / W_STAGES) & 1));
-                    WS_PROF(wf += clock64() - c0;)
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t bh = s_u32(b_buf + s_ * 2 * W_B_FLOATS);
-                    uint64_t db_hi = umma_desc(bh, W_LBO, 128), db_lo = umma_desc(bh + W_B_FLOATS * 4, W_LBO, 128);
-#pragma unroll
-                    for (int ks = 0; ks < W_BK / 8; ++ks, ++ks_tile) {
-                        const int jm = 1 + ks_tile % (W_NB - 1);
-                        const uint32_t acc_main = tmem_base + (uint32_t)(((p0 + jm) & 3) * W_BN);
-                        umma_tf32(acc_corr, da_lo, db_hi, IDESC, ks_tile > 0 ? 1u : 0u);
-                        umma_tf32(acc_corr, da_hi, db_lo, IDESC, 1u);
-                        umma_tf32(acc_main, da_hi, db_hi, IDESC, ks_tile >= (W_NB - 1) ? 1u : 0u);
-                        da_hi += (2 * W_LBO) >> 4; da_lo += (2 * W_LBO) >> 4;
-                        db_hi += (2 * W_LBO) >> 4; db_lo += (2 * W_LBO) >> 4;
-                    }
-                    umma_commit_(empty + s_);  // frees the shared-memory stage when these MMAs retire
-                }
-                umma_commit_(acc_full + (it & 1));  // hands the tile's buffers to the epilogue
-            }
-            WS_PROF(atomicAdd(&g_ws_prof[2], (unsigned long long)wf); atomicAdd(&g_ws_prof[3], (unsigned long long)wa);
-                    atomicAdd(&g_ws_prof[4], (unsigned long long)(clock64() - it0)); atomicAdd(&g_ws_prof[7], 1ull);)
-        }
-    } else {
-        // ================= epilogue: warp w reads TMEM lanes [32 (w&3), +32) (tile rows), columns [64 (w>>2), +64)
-        const int lane_grp = warp & 3, chalf = warp >> 2;
-        const int row = m0 + lane_grp * 32 + lane;
-        WS_PROF(long long ew = 0; const long long et0 = clock64();)
-        for (int it = 0; it < n_it; ++it) {
-            const int t = t_begin + it, p0 = it * W_NB;
-            WS_PROF(const long long c0 = clock64();)
-            mbar_wait_(acc_full + (it & 1), (uint32_t)((it >> 1) & 1));
-            WS_PROF(ew += clock64() - c0;)
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            float v[64];
-#define NB_TMEM_LD16(R, OFF, TADDR)                                                                                                          \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"                     \
-                 : "=r"(R[OFF + 0]), "=r"(R[OFF + 1]), "=r"(R[OFF + 2]), "=r"(R[OFF + 3]), "=r"(R[OFF + 4]), "=r"(R[OFF + 5]), "=r"(R[OFF + 6]), \
-                   "=r"(R[OFF + 7]), "=r"(R[OFF + 8]), "=r"(R[OFF + 9]), "=r"(R[OFF + 10]), "=r"(R[OFF + 11]), "=r"(R[OFF + 12]),              \
-                   "=r"(R[OFF + 13]), "=r"(R[OFF + 14]), "=r"(R[OFF + 15])                                                                    \
-                 : "r"(TADDR)                                                                                                                 \
-                 : "memory")
-#pragma unroll
-            for (int j = 0; j < W_NB; ++j) {
-                const int bufi = (p0 + j) & 3;
-                const uint32_t taddr = tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(bufi * W_BN + chalf * 64);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {  // two 32-column halves: 2 loads in flight per wait
-                    uint32_t r[32];
-                    NB_TMEM_LD16(r, 0, taddr + h * 32);
-                    NB_TMEM_LD16(r, 16, taddr + h * 32 + 16);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int q_ = 0; q_ < 32; ++q_) v[h * 32 + q_] = (j == 0) ? __uint_as_float(r[q_]) : v[h * 32 + q_] + __uint_as_float(r[q_]);
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive_(buf_empty + bufi);  // this buffer is in registers: the issuer may overwrite it
-            }
-#undef NB_TMEM_LD16
-            if (row < M) {
-                const int nb = t * W_BN + chalf * 64;
-                float* cp = C + (size_t)row * ldc + nb;
-#pragma unroll
-                for (int q4 = 0; q4 < 16; ++q4) {
-                    if (nb + 4 * q4 < N) {
-                        float4 o = make_float4(v[4 * q4], v[4 * q4 + 1], v[4 * q4 + 2], v[4 * q4 + 3]);
-                        if (bias) o = o + ldg4(bias + nb + 4 * q4);
-                        if (accumulate) o = o + *reinterpret_cast<const float4*>(cp + 4 * q4);
-                        st4(cp + 4 * q4, o);
-                        if (act) st4(act + (size_t)row * ldc + nb + 4 * q4, make_float4(actf_(o.x, act_kind), actf_(o.y, act_kind), actf_(o.z, act_kind), actf_(o.w, act_kind)));
-                    }
-                }
-            }
-        }
-        WS_PROF(ew_total = ew; et_total = clock64() - et0;)
-    }
-    WS_PROF(if (tid == 0) { atomicAdd(&g_ws_prof[5], (unsigned long long)ew_total); atomicAdd(&g_ws_prof[6], (unsigned long long)et_total); })
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
-}
-
-template <int W_NB>
-int launch_wide(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-                const float* bias, float* act, int act_kind, cudaStream_t s) {
-    const int smem = (2 * W_A_FLOATS + W_STAGES * 2 * W_B_FLOATS) * (int)sizeof(float) + 128;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(k_gemm_tf32x3_wide<W_NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return nb_check_launch();
-        attr_set = true;
-    }
-    const int m_tiles = (M + G_BM - 1) / G_BM, n_tiles = (N + W_BN - 1) / W_BN;
-    // split the N walk when there are too few row slabs to fill the 148 SMs, or to smooth the last wave (A restaging is 64 KB per CTA)
-    int ny = 1;
-    while (m_tiles * ny < 148 && ny < n_tiles) ++ny;
-    if (m_tiles >= 148) {
-        double best = 1e30;
-        for (int c = 1; c <= 8 && n_tiles / c >= 8; ++c) {
-            const double ctas = (double)m_tiles * c, waves = (double)((long long)(ctas + 147) / 148);
-            const double cost = waves * ((n_tiles + c - 1) / c + 0.5);
-            if (cost < best) { best = cost; ny = c; }
-        }
-    }
-    const int tiles_per_cta = (n_tiles + ny - 1) / ny;
-    dim3 grid(m_tiles, (n_tiles + tiles_per_cta - 1) / tiles_per_cta);
-    k_gemm_tf32x3_wide<W_NB><<<grid, W_THREADS, smem, s>>>(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, tiles_per_cta);
+    dim3 grid((M + G_BM - 1) / G_BM, (N + G_BN - 1) / G_BN, batch_kind ? n_batch : 1);
+    k_gemm_tf32x3<<<grid, G_THREADS, smem, s>>>(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, batch_kind, a_boff,
+                                                b_boff, c_boff);
     return nb_check_launch();
 }
 
@@ -591,21 +209,12 @@ int nb_gemm_tf32x3_ex(int M, int N, int K, const float* A, int lda, const float*
     if (!A || !B || !C || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
     if (K % G_BK || N % 4 || lda % 4 || ldb % 4 || ldc % 4) return NB200_EUNSUPPORTED;
     if (M == 0) return NB200_OK;
-    // Measured per shape (tools/gemm_microbench.py, profiles/r1_gemm_variants.md): the wide warp-specialised kernel wins whenever
-    // one resident A slab covers K and N fills its 128-column MMA; everything else (K > 128, N = 64) goes to the tile kernel.
-    // NB200_GEMM_VARIANT=tile|wide forces one of them for A/B runs; NB200_GEMM_NB=2 uses one main accumulator instead of two.
-    static const int variant = [] { const char* e = getenv("NB200_GEMM_VARIANT"); return !e ? 0 : (e[0] == 't') ? 1 : (e[0] == 'p') ? 3 : 2; }();
-    // tall problems: weights pre-split once into shared-memory tile images and streamed (gemm_ps.cu); NB200_GEMM_VARIANT=ps forces it,
-    // =tile / =wide keep the round-1 kernels for A/B runs
+    // tall problems: weights pre-split once into shared-memory tile images and streamed (gemm_ps.cu); NB200_GEMM_VARIANT=tile keeps every
+    // shape on the tile kernel below, =ps forces the pre-split kernel
+    static const int variant = [] { const char* e = getenv("NB200_GEMM_VARIANT"); return !e ? 0 : (e[0] == 't') ? 1 : (e[0] == 'p') ? 3 : 0; }();
     if (variant == 3 || (variant == 0 && nb_gemm_ps_wanted(M, N, K)))
         return nb_gemm_ps(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, nullptr, 0, s);
-    static const int nb = [] { const char* e = getenv("NB200_GEMM_NB"); return e ? atoi(e) : 3; }();
-    const bool wide_ok = K <= AS_KMAX;
-    if (wide_ok && (variant == 2 || (variant == 0 && N >= W_BN)))
-        return (nb == 2 ? launch_wide<2> : launch_wide<3>)(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, s);
-    // BN = 64: 4 x 64 TMEM columns and 96 KB of stages per CTA -> two CTAs per SM and twice as many
-    // tiles, which matters more than tile efficiency for these skinny (M ~ 10^4, N <= 384) problems
-    return launch<64>(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, 0, 1, 0, 0, 0, s);
+    return launch(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, 0, 1, 0, 0, 0, s);
 }
 
 // batched over the 25 (l,m) rows of an equivariant feature: see batch_kind 1 in the kernel
@@ -615,9 +224,9 @@ int nb_gemm_tf32x3_lm(int M, int N, int K, const float* A, int lda, const float*
     if (K % G_BK || N % 4 || lda % 4 || ldc % 4) return NB200_EUNSUPPORTED;
     if (M == 0) return NB200_OK;
     // tall inputs (per-pair features of QHNet / PhiSNet: 1e5 rows x 25 slices): pre-split weights, one launch over (row slab, slice)
-    static const bool ps_off = [] { const char* e = getenv("NB200_GEMM_VARIANT"); return e && (e[0] == 't' || e[0] == 'w'); }();
+    static const bool ps_off = [] { const char* e = getenv("NB200_GEMM_VARIANT"); return e && e[0] == 't'; }();
     if (!ps_off && nb_gemm_ps_lm_wanted(M, N, K)) return nb_gemm_ps_lm(M, N, K, A, lda, W_l, w_l_stride, C, ldc, accumulate, bias, n_lm, s);
-    return launch<64>(M, N, K, A, lda, W_l, N, 1, C, ldc, accumulate, bias, nullptr, NB_ACT_SILU, 1, n_lm, K, w_l_stride, N, s);
+    return launch(M, N, K, A, lda, W_l, N, 1, C, ldc, accumulate, bias, nullptr, NB_ACT_SILU, 1, n_lm, K, w_l_stride, N, s);
 }
 
 extern "C" int nb200_gemm_tf32x3(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb,
@@ -625,11 +234,3 @@ extern "C" int nb200_gemm_tf32x3(int32_t M, int32_t N, int32_t K, const float* A
                                  void* stream) {
     return nb_gemm_tf32x3_ex(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, NB_ACT_SILU, (cudaStream_t)stream);
 }
-
-#ifdef NB_WS_PROF
-extern "C" int nb200_debug_ws_prof(unsigned long long* out8, int reset) {
-    if (cudaMemcpyFromSymbol(out8, g_ws_prof, sizeof(unsigned long long) * 8) != cudaSuccess) return -1;
-    if (reset) { unsigned long long z[8] = {0}; cudaMemcpyToSymbol(g_ws_prof, z, sizeof(z)); }
-    return 0;
-}
-#endif

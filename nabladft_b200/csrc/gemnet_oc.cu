@@ -3,14 +3,14 @@
 // Reference: nablaDFT/gemnet_oc/gemnet_oc.py (forward 1121-1251, graphs 694-1000, bases 1001-1120), interaction_indices.py,
 // layers/{interaction_block,atom_update_block,embedding_block,efficient,radial_basis,spherical_basis,base_layers}.py.
 //
-// Design (B200-first, not the reference's): the reference materialises index lists for triplets and quadruplets (526 k quadruplets for
+// Design (GPU-first, not the reference's): the reference materialises index lists for triplets and quadruplets (526 k quadruplets for
 // 79 atoms) and scatters every basis into zero-padded [edges, K_max, .] tensors so that aggregation becomes a batched matmul.  Here
 // nothing of that is stored.  The four graphs are CSR rows by TARGET atom with sources ascending (the order in which the reference's
 // SparseTensor rows enumerate input edges); an aggregation kernel owns one output (edge, channel) element, walks the CSR rows of the
 // atoms involved, evaluates the Legendre bases of the angles on the fly and keeps the [spherical x channel] partial sums in registers;
 // the radial factor is applied once per output.  The order of OUTPUT edges differs from the reference's ([directed | flipped] per
 // molecule) -- a row permutation of every per-edge tensor that cancels in the per-atom sums (energy, forces, h).
-// Dense layers run on the tcgen05 3xTF32 GEMM (gemm_tc.cu) when the shape tiles, else on the functor fallback below.
+// Dense layers run on the wgmma 3xTF32 GEMM (gemm_tc.cu) when the shape tiles, else on the functor fallback below.
 // Every kernel is a functor launched through pfor() (gemnet_pf.cuh) so that the same source compiles for host emulation in tests/emu.
 #include "gemnet_oc_kernels.cuh"
 
@@ -172,10 +172,10 @@ int output_block(const Ctx& c, const Work& w, int blk, int64_t n, int64_t E) {
 // Device form of QuadK (gemnet_oc_kernels.cuh; same sums in the same order, so the host-emulation tests of the functor pin this kernel's
 // arithmetic too).  The functor launches one logical thread per (edge, channel): the 32 channel-threads of an edge all recompute the
 // geometry of every quadruplet -- two cross products, a square root, a division and the Legendre recurrence, more instructions than the
-// 49 FMAs they feed (12 % of the first measured forward, profiles/r2_gemnet_launches_summary.md).  Here a WARP owns the edge (lane =
+// 49 FMAs they feed.  Here a WARP owns the edge (lane =
 // channel): 32 quadruplets at a time, lane j evaluates the dihedral basis of quadruplet j ONCE and stages it in shared memory; the warp
 // then walks the staged rows (two broadcast 16-byte loads per quadruplet); the chunk's x_t rows travel by cp.async while the bases are computed
-// (first version: plain loads four quadruplets ahead -- 3 ms per launch at 77 k edges, one L2 round trip per four quadruplets and warp).
+// (first version: plain loads four quadruplets ahead -- one L2 round trip per four quadruplets and warp).
 constexpr int QW_WARPS = 8;
 __device__ __forceinline__ void qw_cp16(void* smem_dst, const void* gmem_src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(gmem_src) : "memory");
@@ -188,12 +188,9 @@ __global__ void __launch_bounds__(32 * QW_WARPS) k_quad_edges(Graph mn, Graph q,
     for (int64_t e = (int64_t)blockIdx.x * QW_WARPS + warp; e < E; e += (int64_t)gridDim.x * QW_WARPS) {
         const int32_t a = mn.tgt[e], c = mn.src[e];
         const float vca[3] = {mn.V[3 * e], mn.V[3 * e + 1], mn.V[3 * e + 2]};
-        // S[l1][l2] as packed fp32 pairs (l2 = 0..5) + one scalar (l2 = 6): the 7 x 7 update of a quadruplet is 21 FFMA2 + 7 FFMA instead of 49 FFMA
-        // (fma.rn.f32x2: bitwise the same sums; the kernel is instruction-bound, profiles/r2b_k_quad_edges_ncu_full_summary.csv)
-        unsigned long long S2[NS][3];
-        float S6[NS];
+        float S[NS2];  // S[l1 NS + l2]: the 7 x 7 update of a quadruplet
 #pragma unroll
-        for (int l1 = 0; l1 < NS; l1++) { S2[l1][0] = S2[l1][1] = S2[l1][2] = pack2f(0.0f, 0.0f); S6[l1] = 0.0f; }
+        for (int l = 0; l < NS2; l++) S[l] = 0.0f;
         for (int32_t qe = q.ptr[a]; qe < q.ptr[a + 1]; qe++) {
             const int32_t b = q.src[qe];
             if (b == c) continue;
@@ -242,24 +239,15 @@ __global__ void __launch_bounds__(32 * QW_WARPS) k_quad_edges(Graph mn, Graph q,
                     if (yb.w == 0.0f) continue;
                     const float4 ya = *reinterpret_cast<const float4*>(&sY[warp][j][0]);
                     const float xv = sX[warp][j][lane];
-                    const unsigned long long y01 = pack2f(ya.x, ya.y), y23 = pack2f(ya.z, ya.w), y45 = pack2f(yb.x, yb.y);
+                    const float yt[NS] = {ya.x, ya.y, ya.z, ya.w, yb.x, yb.y, yb.z};
 #pragma unroll
                     for (int l1 = 0; l1 < NS; l1++) {
                         const float f = Yp[l1] * xv;
-                        const unsigned long long ff = pack2f(f, f);
-                        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(S2[l1][0]) : "l"(ff), "l"(y01));
-                        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(S2[l1][1]) : "l"(ff), "l"(y23));
-                        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(S2[l1][2]) : "l"(ff), "l"(y45));
-                        S6[l1] = fmaf(f, yb.z, S6[l1]);
+#pragma unroll
+                        for (int l2 = 0; l2 < NS; l2++) S[l1 * NS + l2] = fmaf(f, yt[l2], S[l1 * NS + l2]);
                     }
                 }
             }
-        }
-        float S[NS2];
-#pragma unroll
-        for (int l1 = 0; l1 < NS; l1++) {
-            unpack2f(S2[l1][0], S[l1 * NS + 0], S[l1 * NS + 1]); unpack2f(S2[l1][1], S[l1 * NS + 2], S[l1 * NS + 3]);
-            unpack2f(S2[l1][2], S[l1 * NS + 4], S[l1 * NS + 5]); S[l1 * NS + 6] = S6[l1];
         }
         const float* Re = R + e * ldr;
         for (int i32 = 0; i32 < 32; i32++) {
@@ -337,7 +325,7 @@ int trip_edge_aggregate(nb200_engine* eng, cudaStream_t s, const Graph& o, const
     if (E <= 0) return NB200_OK;
     Scope sc(eng, s, CAT_MSG_FWD, 1);
     const int64_t want = (E + TW_WARPS - 1) / TW_WARPS;
-    k_trip_edges<<<(int)(want < 148 * 8 ? want : 148 * 8), 32 * TW_WARPS, 0, s>>>(o, in, x, R, ldr, O, E);
+    k_trip_edges<<<(int)(want < nb_sm_count() * 8 ? want : nb_sm_count() * 8), 32 * TW_WARPS, 0, s>>>(o, in, x, R, ldr, O, E);
     return nb_check_launch();
 #endif
 }
@@ -351,7 +339,7 @@ int quad_aggregate(nb200_engine* eng, cudaStream_t s, const Graph& mn, const Gra
     if (E <= 0) return NB200_OK;
     Scope sc(eng, s, CAT_MSG_FWD, 1);
     const int64_t want = (E + QW_WARPS - 1) / QW_WARPS;
-    k_quad_edges<<<(int)(want < 148 * 8 ? want : 148 * 8), 32 * QW_WARPS, 0, s>>>(mn, q, q_tin, xt, R, ldr, O, E);
+    k_quad_edges<<<(int)(want < nb_sm_count() * 8 ? want : nb_sm_count() * 8), 32 * QW_WARPS, 0, s>>>(mn, q, q_tin, xt, R, ldr, O, E);
     return nb_check_launch();
 #endif
 }

@@ -256,7 +256,7 @@ struct MulRbfK {
 };
 // The same arithmetic (bitwise), MRB_ROWS rows per logical thread: the 16 weights of channel c stay in registers, consecutive threads are
 // consecutive channels.  MulRbfK read W[c][0..15] again for every output -- 64 bytes per thread at a 64-byte stride, 16 L1 wavefronts per
-// warp load -- and was 10 % of the first measured forward (profiles/r2_gemnet_launches_summary.md); here a warp's per-row traffic is the
+// warp load -- and was 10 % of the first measured forward; here a warp's per-row traffic is the
 // broadcast basis row + one coalesced load + one coalesced store.  i = (row block, channel); n = ceil(M / MRB_ROWS) * C.
 constexpr int MRB_ROWS = 16;
 struct MulRbfRowsK {
@@ -266,7 +266,7 @@ struct MulRbfRowsK {
     GD void operator()(int64_t i) const {
         const int64_t rb = i / C; const int c = (int)(i % C);
         // 16-byte loads (the basis columns start at multiples of 16 floats of 256-byte aligned rows; ldr % 4 == 0): the scalar form issued
-        // 16 + 1 loads and a store per output row and warp and was bound by the load/store unit's instruction rate (285 us per [77 k, 512] launch)
+        // 16 + 1 loads and a store per output row and warp and was bound by the load/store unit's instruction rate
         float w[RB];
         const float4* w4 = reinterpret_cast<const float4*>(W + (int64_t)c * RB);
 #pragma unroll

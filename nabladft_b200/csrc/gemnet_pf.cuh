@@ -3,7 +3,7 @@
 // Every kernel of these engines is a functor with `operator()(int64_t i)`: one logical thread per output element, no shared memory, no warp
 // intrinsics; forward aggregations are gathers over CSR rows (deterministic), only some backward scatters use atomicAdd.  `pfor` launches a
 // functor as a grid-stride kernel sized to the SM count.  The same translation units also compile as plain C++ with -DNB_EMU (tests/emu/):
-// there `pfor` is an OpenMP loop, the library GEMMs (tcgen05, cuBLAS) are replaced by the functor GEMMs, and every workspace array gets a
+// there `pfor` is an OpenMP loop, the library GEMMs (wgmma, cuBLAS) are replaced by the functor GEMMs, and every workspace array gets a
 // guard zone -- which lets the CPU test-suite check every functor against the oracle when no GPU is at hand.  The emulation build is TEST
 // INFRASTRUCTURE: the package never loads it (nabladft_b200/_lib.py loads libnabla_b200.so only).
 #pragma once
@@ -41,14 +41,14 @@ template <class F>
 __global__ void __launch_bounds__(256) k_pfor(int64_t n, F f) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) f(i);
 }
-// grid: enough 256-thread CTAs to cover n, capped at 8 resident CTAs on each of the 148 SMs (grid-stride beyond that)
+// grid: enough 256-thread CTAs to cover n, capped at 8 resident CTAs on each SM (grid-stride beyond that)
 template <class F>
 inline int pfor(nb200_engine* e, cudaStream_t s, int category, int64_t n, const F& f) {
     if (n <= 0) return NB200_OK;
     static_assert(sizeof(F) <= 4000, "functor must fit the kernel parameter space");
     Scope sc(e, s, category, 1);
     const int64_t want = (n + 255) / 256;
-    const int blocks = (int)(want < 148 * 8 ? want : 148 * 8);
+    const int blocks = (int)(want < nb_sm_count() * 8 ? want : nb_sm_count() * 8);
     k_pfor<F><<<blocks, 256, 0, s>>>(n, f);
     return nb_check_launch();
 }
@@ -92,13 +92,12 @@ inline int goc_d2h_sync(void* dst, const void* src, size_t bytes, cudaStream_t s
 inline int goc_d2d(void* dst, const void* src, size_t bytes, cudaStream_t s) {
     return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s) == cudaSuccess ? NB200_OK : NB200_ECUDA;
 }
-// tensor-core GEMM when the shape fits the tcgen05 kernels' tiling, else the functor fallback in gemnet_oc.cu
+// tensor-core GEMM when the shape fits the wgmma kernels' tiling, else the functor fallback in gemnet_oc.cu
 // NB200_GOC_GEMM=simt forces the fallback everywhere (A/B runs, bring-up of new shapes)
 inline bool goc_tc_ok(int N, int K, int lda, int ldw, int ldc) {
     static const bool simt = [] { const char* e = getenv("NB200_GOC_GEMM"); return e && e[0] == 's'; }();
     // N % 32: the 128 x 64 tile kernel masks the columns beyond N, so the quadruplet bilinear layer (1024 -> 32 per edge, ~6 % of the model's
-    // FLOPs) runs on the tensor cores with a half-empty tile instead of the functor fallback (26 % of the forward's kernel time on its first
-    // device run, profiles/r2_gemnet_launches_summary.md)
+    // FLOPs) runs on the tensor cores with a half-empty tile instead of the functor fallback
     return !simt && N % 32 == 0 && K % 32 == 0 && lda % 4 == 0 && ldw % 4 == 0 && ldc % 4 == 0;
 }
 inline int goc_tc_gemm(nb200_engine* e, cudaStream_t s, int M, int N, int K, const float* A, int lda, const float* W, int ldw, float* C, int ldc) {

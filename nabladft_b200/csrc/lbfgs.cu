@@ -12,7 +12,7 @@
 // (numpy: sequential), which moves results by ~1e-16 relative.
 //
 // Traffic per step: the history is read twice (two loops): 2 * min(memory, it) * 3N * (8 + 4) bytes (72 MB at N = 10^4,
-// memory = 100: ~11 us at HBM speed); the kernel is latency-bound on its 2 * min(memory, it) + 3 block reductions instead.
+// memory = 100); the kernel is latency-bound on its 2 * min(memory, it) + 3 block reductions instead.
 #include "common.cuh"
 
 namespace {

@@ -1,36 +1,29 @@
-// painn_fused.cu -- the whole per-atom ("node") part of a PaiNN layer as ONE persistent tcgen05 kernel per direction.
+// painn_fused.cu -- the whole per-atom ("node") part of a PaiNN layer as ONE persistent wgmma kernel per direction.
 //
 // Replaces, per layer, the five nn.Linear GEMMs and the elementwise glue of
 //   PaiNNUpdate.forward            nablaDFT/painn_pyg/painn.py:535-548   (schnetpack PaiNNMixing)
 //   the message MLP x_proj         nablaDFT/painn_pyg/painn.py:459-464   (schnetpack interatomic_context_net)
 //   the readout's first Linear     nablaDFT/painn_pyg/painn.py:79-83     (schnetpack Atomwise.outnet[0])
-// and their autograd backward (painn.py:135-146).  Round 1 ran them as 12 separate 3xTF32 GEMM launches + 6 elementwise launches per
-// layer and direction: 72 GEMM launches = 2.4 ms of a 3.4 ms step at ~0.10 of the tensor roofline (VERDICT r1, weak #5), because every
-// launch re-staged and re-split its activation slab, the producers split the weights again for every row slab, and the fixed costs of a
-// 76-CTA launch were paid 12 times.
+// and their autograd backward (painn.py:135-146), which would otherwise be 12 separate 3xTF32 GEMM launches + 6 elementwise launches per
+// layer and direction, each re-staging and re-splitting its activation slab.
 //
-// Design (measured basis: tools/mma_rate.cu, profiles/r2_mma_rate.txt -- a tcgen05.mma.kind::tf32 M128 N128 K8 with BOTH operands in
-// shared memory issues every 71 cycles next to a 57 B/clk bulk-copy stream; with the A operand in tensor memory it needs 94-106):
-//   * CTA = 128 atoms.  Every GEMM of the chain is computed TRANSPOSED: D[feature, atom] = W[feature, k] . X[atom, k]^T, i.e. the weight
-//     tile is the MMA's A operand (M = 128 output features) and the activations are the B operand (N = 128 atoms).  The accumulator then
-//     has features on TMEM lanes and atoms on columns: an epilogue thread owns one feature and 64 atoms, so every global store / load of
-//     an [atom][feature] array is a 128-byte coalesced warp access, the bias is a per-thread scalar, and writing the next activation
-//     operand into shared memory ([atoms] x K, K-major) is a conflict-free 4-byte store pattern.  No transposes, no row-per-thread access.
+// Design (the pipeline itself is tc_pipe.cuh):
+//   * CTA = 64 atoms.  Every GEMM of the chain is computed TRANSPOSED: D[feature, atom] = W[feature, k] . X[atom, k]^T, i.e. the weight
+//     tile is the MMA's A operand (M = 128 output features, two warpgroups of 64) and the activations are the B operand (N = 64 atoms).
+//     The staged result has features on rows and atoms on columns: an epilogue thread owns one feature and 32 atoms, so every global
+//     store / load of an [atom][feature] array is a 128-byte coalesced warp access, the bias is a per-thread scalar, and writing the next
+//     activation operand into shared memory ([atoms] x K, K-major) is a conflict-free 4-byte store pattern.
 //   * weights are split into TF32 hi / lo ONCE per call by k_prep_painn into ready-made shared-memory images (one 128 x 128 tile =
-//     4 stages x [hi | lo] x 16 KB, canonical no-swizzle K-major); a producer thread streams them with one cp.async.bulk per stage
-//     through a 3-stage mbarrier ring.  Nobody splits weights inside the GEMM any more.
-//   * the activation operand X [128 atoms x 128 k] (hi + lo, 132 KB) is written by the 8 worker warps: either by a LOADER functor
-//     (coalesced global loads, elementwise math fused in: sqrt-norm, the combine backward, silu' ...) or directly from the previous
-//     GEMM's epilogue registers (silu(h) -> next operand) -- chained activations never go through global memory to be re-read as operands.
-//   * one thread issues the MMAs (3xTF32: lo.hi + hi.lo into a correction accumulator, hi.hi alternating over two main accumulators so
-//     that no accumulator chain is longer than 8 per 128 k: the tensor core truncates on accumulate, see gemm_tc.cu); TMEM columns
-//     [0,384) = the three accumulators, [384,512) = a STAGING buffer: the epilogue first sums the three accumulators into it (compact,
-//     non-inlined code), releases them to the issuer one by one, and then walks the staged tile in 16-atom chunks inside ROLLED loops.
-//     (First version: v[64] per thread, everything unrolled -> 25 k SASS instructions = 400 KB executed once per CTA: the kernel was
-//     instruction-fetch bound, 250 k cycles of "busy" workers.  tools/nf_prof.py, profiles/r2_fused_role_timing.md.)
-//     K > 128 (backward) accumulates over several X operands in place.
-//   * roles meet only through mbarriers: W ring full/empty, X ready/free, accumulator full, accumulator buffer empty.
-// Forward  kernel = update(l) [+ message MLP(l+1) | readout Linear]   (15 tiles of 48 MMAs)
+//     4 stages x [hi | lo] x 16 KB, canonical no-swizzle K-major), streamed with one cp.async.bulk per stage through a 3-stage mbarrier ring.
+//   * the activation operand X [64 atoms x 128 k] (hi + lo) is written by the 8 worker warps: either by a LOADER functor (coalesced global
+//     loads, elementwise math fused in: sqrt-norm, the combine backward, silu' ...) or directly from the previous GEMM's epilogue registers
+//     (silu(h) -> next operand) -- chained activations never go through global memory to be re-read as operands.
+//   * 3xTF32: lo.hi + hi.lo into a correction accumulator, hi.hi alternating over two main accumulators so that no accumulator chain is
+//     longer than 8 per 128 k (the tensor core truncates on accumulate, see gemm_tc.cu); the MMA warpgroups sum them into a shared-memory
+//     staging tile, which the epilogues walk in 16-atom chunks inside ROLLED loops (compact code).  K > 128 (backward) accumulates over
+//     several X operands in place.
+//   * roles meet only through mbarriers: W ring full/empty, X ready/free, staging full / free.
+// Forward  kernel = update(l) [+ message MLP(l+1) | readout Linear]
 // Backward kernel = [message-MLP backward(l+1) | readout backward] + update backward(l)
 #include "painn_node.cuh"
 
@@ -149,18 +142,14 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
         }
         if (P.do_ro) prog_add(prog, P.tile_ro, U_NEWX | U_FIRST | U_LAST | U_XLAST);
     }
-    Ctx c = setup(smem, tid, warp, P.xsplit);
+    Ctx c = setup(smem, tid, P.xsplit);
     NF_PROF_DO(const long long tk0_ = clock64(); c.t_last = tk0_;)
 #define NF_BASE 0
 
-    if (warp == NWORK) {
-        if (lane == 0) run_producer(c, prog, P.wt);
-    } else if (warp == NWORK + 1) {
-        if (lane == 0) {
-            run_issuer(c, prog);
-            NF_PROF_DO(atomicAdd(&g_nf_prof[0], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[1], (unsigned long long)c.w_x);
-                       atomicAdd(&g_nf_prof[2], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[3], (unsigned long long)c.w_full);)
-        }
+    if (warp >= WARP_ISSUE) {
+        run_issuer(c, prog, P.wt);
+        NF_PROF_DO(if (warp == WARP_ISSUE && lane == 0) { atomicAdd(&g_nf_prof[0], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[1], (unsigned long long)c.w_x);
+                   atomicAdd(&g_nf_prof[2], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[3], (unsigned long long)c.w_full); })
     } else {
         const int N = P.n_atoms, A0 = blockIdx.x * NT;
         const int fl = 32 * (warp & 3) + lane;   // my feature inside a 128-row weight tile
@@ -193,8 +182,8 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
             NF_LOAD([&](int r, int kc) { return A0 + r < N ? ldg4(P.q_mid + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
             NF_MARK(3);
             if (isL) {   // while the tensor core works on q_mid: nrm = sqrt(sum_x V_x^2 + eps) and dot = sum_x V_x Wv_x, 2 atoms per round
-                // (keeping |V|^2 and <V,Wv> in registers across the U tiles was tried: 64 persistent registers spill, and with 230 KB of
-                //  shared memory there is no L1 left for local memory -- 1.42 ms instead of 1.37 ms per step for the node kernels)
+                // (|V|^2 and <V,Wv> are not kept in registers across the U tiles: 64 persistent registers would spill, and with ~195 KB of
+                //  shared memory per CTA little L1 is left for local memory)
                 dep_wait(c, 0);
                 const int kc = ltid & 31, w = ltid >> 5;
 #pragma unroll 1
@@ -383,7 +372,6 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
 #undef NF_BASE
     NF_PROF_DO(if (tid == 0) { atomicAdd(&g_nf_prof[4], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[5], (unsigned long long)c.w_acc);
                             atomicAdd(&g_nf_prof[6], (unsigned long long)c.w_xfree); atomicAdd(&g_nf_prof[7], 1ull); })
-    teardown(c, warp);
 }
 
 // ================================================================================================== backward
@@ -426,17 +414,13 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
             }
         }
     }
-    Ctx c = setup(smem, tid, warp, P.xsplit);
+    Ctx c = setup(smem, tid, P.xsplit);
     NF_PROF_DO(const long long tk0_ = clock64();)
 
-    if (warp == NWORK) {
-        if (lane == 0) run_producer(c, prog, P.wt);
-    } else if (warp == NWORK + 1) {
-        if (lane == 0) {
-            run_issuer(c, prog);
-            NF_PROF_DO(atomicAdd(&g_nf_prof[8], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[9], (unsigned long long)c.w_x);
-                       atomicAdd(&g_nf_prof[10], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[11], (unsigned long long)c.w_full);)
-        }
+    if (warp >= WARP_ISSUE) {
+        run_issuer(c, prog, P.wt);
+        NF_PROF_DO(if (warp == WARP_ISSUE && lane == 0) { atomicAdd(&g_nf_prof[8], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[9], (unsigned long long)c.w_x);
+                   atomicAdd(&g_nf_prof[10], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[11], (unsigned long long)c.w_full); })
     } else {
         const int N = P.n_atoms, A0 = blockIdx.x * NT;
         const int fl = 32 * (warp & 3) + lane;
@@ -579,7 +563,6 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
     }
     NF_PROF_DO(if (tid == 0) { atomicAdd(&g_nf_prof[12], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[13], (unsigned long long)c.w_acc);
                             atomicAdd(&g_nf_prof[14], (unsigned long long)c.w_xfree); atomicAdd(&g_nf_prof[15], 1ull); })
-    teardown(c, warp);
 }
 
 template <class K>
@@ -611,7 +594,7 @@ int nb_fused_prep(const nb200_painn_weights* w, void* wtiles, cudaStream_t s) {
 }
 
 // NB200_NF_XSPLIT=1: hand the activation operands over in two K halves (tc_pipe.cuh).  Measured neutral for these kernels (122.4 k vs 122.8 k
-// molecules/s, gpurun_out/r2b_call10: most of their operands are written by the previous GEMM's epilogue, which the hand-over cannot
+// molecules/s, A/B run: most of their operands are written by the previous GEMM's epilogue, which the hand-over cannot
 // start earlier), so the whole-operand protocol stays the default here; the pre-split-weight GEMM uses it for K > 128.
 static int nf_xsplit() {
     static const int on = [] { const char* e = getenv("NB200_NF_XSPLIT"); return (e && e[0] == '1') ? 1 : 0; }();

@@ -17,14 +17,12 @@
 #include "common.cuh"
 
 // One warp per CTA (16 CTAs per SM): a CTA's shared memory and registers return to the SM as soon as ITS atom is done.  With 8 warps per
-// CTA the slot was held until the slowest of 8 atoms (degrees 15..40) finished: ncu showed 18.8 % achieved vs 25 % theoretical occupancy.
-// Measured per step (6 launches each): 8 warps 0.494 / 0.768 ms (fwd / bwd), 4 warps 0.475 / 0.753, 1 warp 0.455 / 0.736.
+// CTA the slot was held until the slowest of 8 atoms (degrees 15..40) finished.
 #define MSG_WARPS 1
 #define MSG_THREADS (MSG_WARPS * 32)
 
-// The v0 kernels (plain LDG for the filter rows) were latency-bound: ncu showed 36 % DRAM
-// throughput with >90 % of stalls on long_scoreboard and ~3 loads in flight per warp
-// (profiles/r1_v0_msg_fwd_ncu_full_summary.csv).  v1 streams the filter rows -- the only HBM
+// The v0 kernels (plain LDG for the filter rows) were latency-bound: low DRAM
+// throughput with most stalls on long_scoreboard and ~3 loads in flight per warp.  v1 streams the filter rows -- the only HBM
 // stream -- through a per-warp cp.async ring in shared memory: every lane prefetches its own
 // 16-byte column of the next STAGES-1 edges, so ~100 KB of HBM requests stay in flight per SM
 // without holding registers, and the gathers of the current edge overlap that stream.
@@ -38,9 +36,9 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 __device__ __forceinline__ float4 lds4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
 // Forward (v4): two rings per warp with independent depths.
-//   * filter rows (the HBM stream, ~1.5 us loaded latency): FWD_WS = 5 stages, filled by the TMA engine --
+//   * filter rows (the HBM stream, microsecond-scale loaded latency): FWD_WS = 5 stages, filled by the TMA engine --
 //     one elected lane issues a 1536-byte `cp.async.bulk` per edge, completion on a per-stage mbarrier;
-//   * gathered neighbour rows xh[j], mu[j] (L2, ~0.6 us): FWD_GS = 2 stages of per-lane cp.async (LDGSTS).
+//   * gathered neighbour rows xh[j], mu[j] (L2): FWD_GS = 2 stages of per-lane cp.async (LDGSTS).
 // cp.async groups retire in order, so one shared queue cannot give the two streams different depths (v2 had 3 / 3
 // and reached 64 % of the HBM roofline; bytes of the HBM stream in flight were the limiter, not issue slots -- v3).
 #define FWD_WS 5
@@ -175,7 +173,7 @@ __global__ void __launch_bounds__(MSG_THREADS, 16) k_painn_msg_fwd(const float* 
 //   dE/du'(e')[x] = sum_ch (Wb*b_j) * gmu_i[x]
 // The four edge scalars are warp-reduced and accumulated into egrad[e] (slot of e, values of e').
 // Backward v3: two rings per warp like the forward (v4).  v2 streamed (W, dW) through a 3-stage cp.async ring but gathered the far atom's
-// gradient rows g_q[i], g_mu[i] (2 KB per edge) with plain loads at the top of every iteration: ncu showed dram 57 %, issue active 22 %,
+// gradient rows g_q[i], g_mu[i] (2 KB per edge) with plain loads at the top of every iteration: the profile showed low DRAM and issue utilisation,
 // 7 warp-cycles of long_scoreboard per issue -- one L2 round trip per edge on the critical path, and at 122 registers no room to pipeline
 // them in registers.  Now: (W, dW) rows by TMA bulk copies (one elected lane, BWD_WS = 3 stages x 3 KB, mbarrier per stage) and the
 // gathered gradient rows by per-lane cp.async into a second ring (BWD_GS = 2 stages x 2 KB).  13 KB per warp, 104 KB per CTA, 2 CTAs/SM.
@@ -316,10 +314,8 @@ __global__ void __launch_bounds__(MSG_THREADS, 16) k_painn_msg_bwd(const float* 
             if ((lane & 7) == 0) {
                 // lane 0 -> .w (gd), lane 8 -> .x (gu0), lane 16 -> .y (gu1), lane 24 -> .z (gu2)
                 const int comp = (lane == 0) ? 3 : (lane >> 3) - 1;
-                // fire-and-forget reduction (RED.ADD): `*p += k` put one L2 round trip per edge on the warp's critical path (the load feeds the
-                // add): 0.806 -> 0.768 ms per step.  Exactly one thread of one warp touches this address per launch: still deterministic.
-                // (Also tried: edge geometry carried in the TMA stage as a third 16-byte bulk copy -- neutral here, and the extra copy per
-                // edge cost the forward kernel 10 %: the TMA engine is paced by the number of copies, not only by bytes.)
+                // fire-and-forget reduction (RED.ADD): `*p += k` would put one L2 round trip per edge on the warp's critical path (the load
+                // feeds the add).  Exactly one thread of one warp touches this address per launch: still deterministic.
                 atomicAdd(egrad + 4 * (size_t)e + comp, k);
             }
         }

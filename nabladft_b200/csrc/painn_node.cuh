@@ -51,7 +51,7 @@ int nb_filter_wgrad_tan(const float* geom, const float* t_geom, const int32_t* s
                         int radial_mode, float cutoff, float rbf_coeff, float rbf_xscale, const float* t_gW, const float* gWd, float sign, float* g_w,
                         float* g_b, cudaStream_t s, int e_cap = 0, int bf16 = 0);
 
-// fused per-layer node kernels (painn_fused.cu): tcgen05 chain of the update / message-MLP / readout Linear layers with their elementwise glue
+// fused per-layer node kernels (painn_fused.cu): wgmma chain of the update / message-MLP / readout Linear layers with their elementwise glue
 struct NbFusedFwd {
     int n_atoms, n_layers;
     int layer_upd;   // layer whose update runs (-1: none)

@@ -8,7 +8,7 @@
 // component-major [rows][(L+1)^2][F] (channels contiguous), one thread owns one feature channel of one row, keeps a[25], b[25], o[25] in
 // registers and evaluates the 2052 (pair) / 729 (self) non-zero real CG terms as unrolled FMAs (phisnet_cg_gen.inc, generated from the
 // reference's vendored table).  SIMT on purpose: the CG tensors are > 80 % zeros; the dense work of the layer -- the distance-dependent
-// coefficients rbf . W for all 65 paths, [P,128] x [128, 8320] -- runs on the tcgen05 3xTF32 GEMM (nb200_dense) before this kernel.
+// coefficients rbf . W for all 65 paths, [P,128] x [128, 8320] -- runs on the wgmma 3xTF32 GEMM (nb200_dense) before this kernel.
 #include "common.cuh"
 #include "phisnet_cg_gen.inc"
 

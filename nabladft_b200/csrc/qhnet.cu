@@ -234,7 +234,7 @@ __global__ void __launch_bounds__(QH_C) k_qh_tp_pair(const float* __restrict__ x
 
 // r2b experiment (NOT the default, see nb200_qh_tp_pair): the same product with the pair's two weight rows (2 x 33 280 B) fetched by TWO bulk copies
 // into shared memory while the threads gather x[src], x[dst]: k_qh_tp_pair streams them with 4-byte loads per thread and path and reached 45 % of the
-// HBM rate (long_scoreboard 2.9 warps per issue, profiles/r2_k_qh_tp_pair_ncu_full_summary.csv); three CTAs per SM keep ~200 KB of rows in flight.
+// HBM rate; three CTAs per SM keep ~200 KB of rows in flight.
 constexpr int QH_TPS_BYTES = 2 * QH_UUU_WEIGHTS * (int)sizeof(float) + 16;
 __global__ void __launch_bounds__(QH_C) k_qh_tp_pair_s(const float* __restrict__ x, const float* __restrict__ w1, const float* __restrict__ w2,
                                                       const int32_t* __restrict__ tgt, const int32_t* __restrict__ col,
@@ -305,12 +305,12 @@ __constant__ float c_exp_cg[19 * 5 * 5 * 9];  // [ins][i][j][k], zero padded, al
 
 // STAGED (r2b experiment, NOT the default, see nb200_qh_expand): the row's 8320 path weights (33 280 B) arrive by ONE bulk copy per warp into shared memory (2 warps per CTA, 2 CTAs per SM, so a
 // CTA's copy overlaps its neighbour's arithmetic) instead of 19 x 32 dependent 100-byte loads per row: the streaming form ran at ~45 % of the
-// HBM rate (profiles/r2_k_qh_expand_ncu_full_summary.csv).
+// HBM rate.
 template <bool STAGED, int WARPS>
 __global__ void __launch_bounds__(32 * WARPS) k_qh_expand(const float* __restrict__ x, const float* __restrict__ W, const float* __restrict__ Bw,
                                                   int bw_stride, int n_rows, float* __restrict__ blocks) {
     // v1 had lane = input channel w and warp-reduced every (u,v,k): 5 k shuffles per row and 4-byte loads strided by
-    // n1*n2 -- 34 ms for 10^5 pairs (65 % of the QHNet forward, profiles/r1_qhnet_launches.csv).  v2: lane = (u,v)
+    // n1*n2.  v2: lane = (u,v)
     // entry of the instruction's weight slab, serial loop over w: the slab rows W[w][.][.] are contiguous (coalesced,
     // read once), x[w][k] is a shared-memory broadcast, no shuffles, and each lane owns its (u,v) sub-block of the tile.
     __shared__ float sblk[WARPS][32 * 32];
@@ -480,7 +480,7 @@ extern "C" int nb200_qh_tp_conv(const float* x, const float* sh, const float* w1
     if (n_atoms == 0) return NB200_OK;
     if (layer0) k_qh_tp_conv<true><<<n_atoms, QH_C, 0, (cudaStream_t)stream>>>(x, sh, w1, w2, row_ptr, col, add_self, out);
     else {
-        // measured (gpurun_out/r2b_call7): staged 42.7 vs streaming 43.3 ms per forward -- inside the run-to-run spread; the streaming kernel stays the default
+        // the staged variant was not faster than the streaming kernel on the previous target GPU; the streaming kernel stays the default (not re-measured on H100)
         static const bool plain = [] { const char* e = getenv("NB200_QH_TP_CONV"); return !(e && e[0] == 's'); }();
         if (plain || ((reinterpret_cast<uintptr_t>(w1) | reinterpret_cast<uintptr_t>(w2)) & 15)) {
             k_qh_tp_conv<false><<<n_atoms, QH_C, 0, (cudaStream_t)stream>>>(x, sh, w1, w2, row_ptr, col, add_self, out);
@@ -500,9 +500,9 @@ extern "C" int nb200_qh_tp_pair(const float* x, const float* w1, const float* w2
                                 int32_t p_cap, float* out, void* stream) {
     if (!x || !w1 || !w2 || !tgt || !col || !status || !out || p_cap < 0) return NB200_EINVAL;
     if (p_cap == 0) return NB200_OK;
-    // measured (gpurun_out/r2b_call6, r2b_call7): the staged kernel gains NOTHING -- 43.1 vs 43.3 ms per config-4 forward on the same kind of box (run-to-run
-    // spread of the forward: 40.8-43.3 ms): 66.5 KB of shared memory leave 3 CTAs = 12 warps per SM (streaming form: 20), and what the copy engine saves in
-    // load latency the lower occupancy loses on the gathers and the FMA chains of the 2052-term product.  NB200_QH_TP_PAIR=staged selects it.
+    // The staged kernel's 66.5 KB of shared memory leave 3 CTAs = 12 warps per SM (streaming form: 20), and what the copy engine saves in load latency
+    // the lower occupancy loses on the gathers and the FMA chains of the 2052-term product (no gain on the previous target GPU; not re-measured on H100).
+    // NB200_QH_TP_PAIR=staged selects it.
     static const bool plain = [] { const char* e = getenv("NB200_QH_TP_PAIR"); return !(e && e[0] == 's'); }();
     const bool aligned = ((reinterpret_cast<uintptr_t>(w1) | reinterpret_cast<uintptr_t>(w2)) & 15) == 0;   // bulk copies need 16-byte aligned rows
     if (plain || !aligned) {
@@ -526,7 +526,7 @@ extern "C" int nb200_qh_tp_self(const float* xl, const float* xr, const float* w
 }
 
 // o3.Linear over the 25 (l,m) rows: y[r][lm][:] = x[r][lm][:] . W_l (+ bias on lm = 0).  W_l: [5][c_in][c_out],
-// already scaled by 1/sqrt(c_in) on export.  c_in must be a multiple of 32 (tcgen05 GEMM k-chunk).
+// already scaled by 1/sqrt(c_in) on export.  c_in must be a multiple of 32 (wgmma GEMM k-chunk).
 extern "C" int nb200_qh_linear(const float* x, const float* W_l, const float* bias, int32_t n_rows, int32_t c_in, int32_t c_out, int32_t accumulate,
                                float* y, void* stream) {
     if (!x || !W_l || !y) return NB200_EINVAL;
@@ -550,8 +550,8 @@ extern "C" int nb200_qh_expand_setup(const int32_t* ins_host, const float* cg_ho
 extern "C" int nb200_qh_expand(const float* x, const float* W, const float* Bw, int32_t bw_stride, int32_t n_rows, float* blocks, void* stream) {
     if (!x || !W || !Bw || !blocks || n_rows < 0 || bw_stride < 50) return NB200_EINVAL;
     if (n_rows == 0) return NB200_OK;
-    // measured (gpurun_out/r2b_call6): the staged kernel is SLOWER -- 48.0 vs 43.1 ms per config-4 forward (4 warps per SM instead of 28: the 19 x 32 serial
-    // steps of a row need occupancy more than they need the copy engine).  NB200_QH_EXPAND=staged selects it.
+    // The staged kernel runs 4 warps per SM instead of 28, and the 19 x 32 serial steps of a row need occupancy more than they need the copy engine
+    // (it was slower on the previous target GPU; not re-measured on H100).  NB200_QH_EXPAND=staged selects it.
     static const bool plain = [] { const char* e = getenv("NB200_QH_EXPAND"); return !(e && e[0] == 's'); }();
     if (plain || (reinterpret_cast<uintptr_t>(W) & 15)) {
         k_qh_expand<false, 4><<<(n_rows + 3) / 4, 128, 0, (cudaStream_t)stream>>>(x, W, Bw, bw_stride, n_rows, blocks);

@@ -368,7 +368,7 @@ inline int64_t chunks(int64_t M) { return (M + WG_ROWS - 1) / WG_ROWS; }
 
 struct Run {
     nb200_engine* e; cudaStream_t s;
-    // dense layers: the tcgen05 3xTF32 GEMM of gemm_tc.cu on the device (shapes of the classes its unit tests cover: N, K in {64, 128},
+    // dense layers: the wgmma 3xTF32 GEMM of gemm_tc.cu on the device (shapes of the classes its unit tests cover: N, K in {64, 128},
     // bias epilogue, trans_b, accumulate), the functor fallback under host emulation or NB200_GOC_GEMM=simt
     int lin(int64_t M, int N, int K, const float* A, const float* W, const float* bias, float* C, bool acc = false) const {
         if (M <= 0) return NB200_OK;

@@ -1,25 +1,22 @@
-// tc_pipe.cuh -- the warp-specialised tcgen05 pipeline shared by the fused PaiNN node kernels (painn_fused.cu) and the pre-split-weight
-// GEMM (gemm_ps.cu): weight tiles as ready-made TF32 hi / lo shared-memory images streamed by cp.async.bulk through an mbarrier ring, the
-// activation operand X written by worker warps (loader functors or epilogue registers), one MMA-issuing thread (3xTF32, correction + two
-// alternating main accumulators), TMEM staging of the summed accumulators, epilogues in rolled 16-column chunks.  D[feature, row] =
-// W[feature, k] . X[row, k]^T: features on TMEM lanes, rows (atoms / edges / pairs) on columns.  See painn_fused.cu for the measurements.
+// tc_pipe.cuh -- the warp-specialised wgmma pipeline shared by the fused PaiNN node kernels (painn_fused.cu) and the pre-split-weight GEMM
+// (gemm_ps.cu): weight tiles as ready-made TF32 hi / lo shared-memory images streamed by cp.async.bulk through an mbarrier ring, the
+// activation operand X written by worker warps (loader functors or epilogue registers), one MMA warpgroup (3xTF32: a correction and a main
+// accumulator in registers), a shared-memory staging tile of the summed accumulators, epilogues in rolled 16-column chunks.
+// D[feature, row] = W[feature, k] . X[row, k]^T: features on the staging rows, rows (atoms / edges / pairs) on its columns.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 
 constexpr int F = NB_F;
-// CTA = NT atoms.  Shipped: NT = 128, one CTA per SM, 16 worker warps, 3 ring stages of 32 k.
-// Tried (NF_SMALL_TILES): NT = 64 with TWO CTAs resident per SM (108 KB of shared memory, 256 TMEM columns, 320 threads each, 5 ring stages
-// of 8 k) so that one CTA's store / load / TMEM-drain phases overlap its neighbour's MMAs and a 9.7 k-atom batch covers all 148 SMs:
-// 1.55 ms instead of 1.35 ms per step -- an N = 64 MMA re-reads the 4 KB weight operand for half as many columns (139 cycles per MMA
-// measured with two CTAs sharing the tensor pipe, 71 at N = 128), and the tensor phase became the long one.
-#ifdef NF_SMALL_TILES
-constexpr int NT = 64, KSTAGE = 8, W_STAGES = 5, NWORK = 8, CTAS_PER_SM = 2;
-#else
-constexpr int NT = 128, KSTAGE = 32, W_STAGES = 3, NWORK = 16, CTAS_PER_SM = 1;
-#endif
+// CTA = NT atoms, 8 worker warps, two MMA warpgroups (features [0, 64) and [64, 128) of a weight tile) whose first thread also issues the
+// weight copies (a separate producer warp made 17 warps, and ptxas then capped the registers at 96); 3 ring stages of 32 k.  An MMA
+// warpgroup holds its 64 features x NT atoms three times (correction + two alternating main accumulators: 96 fp32 registers per thread
+// at NT = 64; one warpgroup for all 128 features spilled), and the staging tile the epilogues read lives in shared memory next to the hi / lo activation operand and
+// the weight ring: 65 + 96 + 34 KB at NT = 64 (NT = 128 would not fit the 227 KB of an SM).
+constexpr int NT = 64, KSTAGE = 32, W_STAGES = 3, NWORK = 8, CTAS_PER_SM = 1;
 constexpr int XLBO = NT * 16 + 16;         // bytes between 16-byte k-chunks of X (padded: the 8 chunk writers of a row hit 8 bank groups)
 constexpr int XLBOF = XLBO / 4;
 constexpr int X_BYTES = 32 * XLBO;         // one of hi / lo, K = 128
@@ -27,8 +24,11 @@ constexpr int WLBO = 128 * 16;             // weight stages are written by the b
 constexpr int WST_BYTES = 2 * (KSTAGE / 4) * WLBO;  // one ring stage: [hi | lo] x KSTAGE/4 chunks x 128 rows x 16 B
 constexpr int STAGES_PER_TILE = 128 / KSTAGE;
 constexpr int WTILE_BYTES = STAGES_PER_TILE * WST_BYTES;  // 128 rows x 128 k, hi + lo = 128 KB
-constexpr int SMEM_BARS = 2 * X_BYTES + W_STAGES * WST_BYTES;
+constexpr int SROW = NT + 4;               // staging row stride (floats): the 16-byte reads of 8 consecutive feature rows hit 8 bank groups
+constexpr int STAGE_BYTES = 128 * SROW * 4;
+constexpr int SMEM_BARS = 2 * X_BYTES + W_STAGES * WST_BYTES + STAGE_BYTES;
 constexpr int SMEM_TOTAL = SMEM_BARS + 256;
+static_assert(SMEM_TOTAL <= 227 * 1024, "shared memory of one CTA");
 // Worker warps.  Default: all NWORK warps load operands AND run epilogues, in program order.  NF_TWO_GROUPS: warps [0, NEPI) only drain /
 // run epilogues / write chained operands, warps [NEPI, NEPI + NLOAD) only run the loader functors and therefore run AHEAD of the epilogues
 // (their global loads overlap epilogue work and MMAs); the groups meet at mbarriers (operand ready / free, and `dep` for data handed over
@@ -38,13 +38,14 @@ constexpr int NEPI = NWORK / 2, NLOAD = NWORK / 2;
 #else
 constexpr int NEPI = NWORK, NLOAD = NWORK;
 #endif
-constexpr int CPT = NT / (NEPI / 4);       // accumulator columns (atoms) per epilogue thread (4 TMEM lane groups x NEPI/4 column parts)
+constexpr int CPT = NT / (NEPI / 4);       // staged columns (atoms) per epilogue thread (4 feature groups of 32 x NEPI/4 column parts)
 constexpr int RPT = NT / NLOAD;            // operand rows per loader thread
-constexpr int NTHREADS = 32 * (NWORK + 2); // + producer warp + MMA issuer warp
-constexpr int TMEM_COLS = 4 * NT;          // three accumulators + staging
+constexpr int WARP_ISSUE = NWORK;          // first warp of the two MMA warpgroups (warpgroups start at a multiple of 4 warps)
+constexpr int NTHREADS = 32 * (NWORK + 8);
+static_assert(NWORK % 4 == 0, "the MMA warpgroups must start on a warpgroup boundary");
 enum { U_NEWX = 1, U_FIRST = 2, U_LAST = 4, U_XLAST = 8 };
 #ifdef NF_PROF
-// role timing (clock64, summed over CTAs): 0 issuer total, 1 issuer waits X, 2 issuer waits TMEM buffers, 3 issuer waits W ring,
+// role timing (clock64, summed over CTAs): 0 issuer total, 1 issuer waits X, 2 issuer waits staging, 3 issuer waits W ring,
 // 4 worker(thread 0) total, 5 worker waits accumulator, 6 worker waits X release, 7 CTAs       [fwd: 0..7, bwd: 8..15]
 __device__ unsigned long long g_nf_prof[16];
 __device__ unsigned long long g_nf_phase[64];  // worker thread 0: cycles between consecutive NF_MARK points [fwd 0..31 | bwd 32..63]
@@ -62,24 +63,6 @@ struct Prog {
 };
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d), "l"(adesc),
-                 "l"(bdesc), "r"(idesc), "r"(accumulate)
-                 : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_u32(bar)), "r"(count) : "memory");
 }
@@ -116,60 +99,59 @@ __device__ __forceinline__ void work_barrier() { asm volatile("bar.sync 1, %0;" 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
 // ------------------------------------------------------------------------------------------------------------------
-constexpr uint32_t TM_CORR = 0, TM_MAIN0 = NT, TM_MAIN1 = 2 * NT, TM_STAGE = 3 * NT;  // TMEM columns
-
 struct Ctx {
     float *x_hi, *x_lo;
     unsigned char* ring;
-    uint64_t *full, *empty, *x_ready, *x_free, *acc_full, *buf_empty, *dep;
+    float* stage;  // [128 features][SROW]: the summed accumulators of the last finished output tile
+    uint64_t *full, *empty, *x_ready, *x_free, *acc_full, *stage_free, *dep;
     // xsplit: the activation operand is handed over in two K halves (k < 64: x_ready / x_free, k >= 64: x_ready2 / x_free2), so that the next
     // operand's first half is written while the MMAs still read the second half of the current one (and the MMAs start on the first half while
-    // the second is written): double buffering at half-operand granularity, no extra shared memory.  r2b measurement that motivated it
-    // (tools/gemm_ps_prof.py, K = 512): issuer waits X 3.5 k + workers wait X release 3.1 k of 8.9 k cycles per (N tile, K chunk).
+    // the second is written): double buffering at half-operand granularity, no extra shared memory.
     uint64_t *x_ready2, *x_free2;
     int xsplit = 0;
-    uint32_t tmem;
     int xg = 0;  // X generations written so far (worker warps) / consumed (issuer)
-    int o = 0;   // output tiles drained so far (worker warps) / committed (issuer)
+    int o = 0;   // output tiles drained so far (worker warps) / staged (issuer)
     NF_PROF_DO(long long w_acc = 0, w_xfree = 0, w_x = 0, w_buf = 0, w_full = 0, t_last = 0;)
 };
 
-// producer: one thread streams the weight tiles of the units (tile_of(u) = index into the prepared buffer), STAGES_PER_TILE stages each
-// (`spt` < STAGES_PER_TILE: K <= 32 * spt, the remaining stages of a tile image are zeros and are neither copied nor multiplied)
-template <class TileFn>
-__device__ __forceinline__ void run_producer_t(const Ctx& c, int n_units, const unsigned char* wt, TileFn tile_of, int spt = STAGES_PER_TILE) {
-    int q = 0;
-#pragma unroll 1
-    for (int u = 0; u < n_units; ++u) {
-        const unsigned char* src = wt + (size_t)tile_of(u) * WTILE_BYTES;
-#pragma unroll 1
-        for (int st = 0; st < spt; ++st, ++q) {
-            const int slot = q % W_STAGES, use = q / W_STAGES;
-            if (use > 0) mbar_wait(c.empty + slot, (uint32_t)((use - 1) & 1));
-            mbar_expect_tx(c.full + slot, WST_BYTES);
-            bulk_g2s(c.ring + slot * WST_BYTES, src + (size_t)st * WST_BYTES, WST_BYTES, c.full + slot);
-        }
-    }
-}
-__device__ __forceinline__ void run_producer(const Ctx& c, const Prog& prog, const unsigned char* wt) {
-    run_producer_t(c, prog.n, wt, [&](int u) { return (int)prog.tile[u]; });
-}
-
-// MMA issuer: one thread walks the program.  An accumulator buffer is waited for right before its first MMA of an output tile, so the
-// correction MMAs start as soon as the epilogue has read the previous tile's correction buffer.
-template <class FlagFn>
-__device__ __forceinline__ void run_issuer_t(Ctx& c, int n_units, FlagFn flags_of, int spt = STAGES_PER_TILE) {
-    constexpr uint32_t IDESC = umma_idesc_tf32(128, NT);
-    const uint64_t dx_hi0 = umma_desc(s_u32(c.x_hi), XLBO, 128), dx_lo0 = umma_desc(s_u32(c.x_lo), XLBO, 128);
-    int q = 0, ks_out = 0;
+// MMA warpgroups (all 256 threads walk the program; warpgroup h owns features [64 h, +64) of the weight tile).  Per k-step of 8: lo.hi + hi.lo
+// into the correction accumulator, hi.hi alternating over two main accumulators (the tensor core truncates when it accumulates: chains of 8
+// per 128 k, one main accumulator measured 1.3e-5 Ha of PaiNN energy drift); both stay in registers across the units of an output tile (K > 128 accumulates over several
+// X operands).  A ring stage is released when the wgmma group that read it has completed (one arrival per warp), the operand X after the last
+// unit that reads it, and a finished tile is summed (RN) into the staging tile once the epilogues have called drain() for the previous one.
+// The weight tiles of the units (tile_of(u) = index into the prepared buffer, STAGES_PER_TILE stages each; `spt` < STAGES_PER_TILE: K <= 32 spt,
+// the remaining stages of a tile image are zeros and are neither copied nor multiplied) are streamed by the first thread of the warpgroups:
+// one cp.async.bulk per stage, W_STAGES ahead; a slot is refilled once both warpgroups have released it.
+template <class FlagFn, class TileFn>
+__device__ __forceinline__ void run_issuer_t(Ctx& c, int n_units, FlagFn flags_of, TileFn tile_of, const unsigned char* wt, int spt = STAGES_PER_TILE) {
+    const int wl = ((threadIdx.x >> 5) - WARP_ISSUE) & 3, h = ((threadIdx.x >> 5) - WARP_ISSUE) >> 2, lane = threadIdx.x & 31;
+    float corr[NT / 2], main0[NT / 2], main1[NT / 2];
+    const uint32_t x_hi0 = s_u32(c.x_hi), x_lo0 = s_u32(c.x_lo);
+    const int n_q = n_units * spt;
+    const bool leader = threadIdx.x == 32 * WARP_ISSUE;
+    int q = 0, pending = -1;  // pending: the stage whose wgmma group may still be reading its ring slot
+    auto release = [&](uint64_t* bar) { if (lane == 0) mbar_arrive(bar); };
+    auto copy = [&](int qq) {
+        if (!leader || qq >= n_q) return;
+        const int slot = qq % W_STAGES;
+        mbar_expect_tx(c.full + slot, WST_BYTES);
+        bulk_g2s(c.ring + slot * WST_BYTES, wt + (size_t)tile_of(qq / spt) * WTILE_BYTES + (size_t)(qq % spt) * WST_BYTES, WST_BYTES, c.full + slot);
+    };
+    auto free_stage = [&](int pq) {
+        const int slot = pq % W_STAGES;
+        release(c.empty + slot);
+        if (leader) { mbar_wait(c.empty + slot, (uint32_t)((pq / W_STAGES) & 1)); copy(pq + W_STAGES); }
+    };
+    for (int qq = 0; qq < W_STAGES; ++qq) copy(qq);
 #pragma unroll 1
     for (int u = 0; u < n_units; ++u) {
         const int fl = flags_of(u);
         const bool newx = (fl & U_NEWX) != 0;
         if (newx) { NF_PROF_DO(const long long t0_ = clock64();) mbar_wait(c.x_ready, (uint32_t)(c.xg & 1)); ++c.xg; NF_PROF_DO(c.w_x += clock64() - t0_;) }
-        if (fl & U_FIRST) ks_out = 0;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint64_t dx_hi = dx_hi0, dx_lo = dx_lo0;
+        if (fl & U_FIRST) {
+#pragma unroll
+            for (int i = 0; i < NT / 2; ++i) { corr[i] = 0.f; main0[i] = 0.f; main1[i] = 0.f; }
+        }
 #pragma unroll 1
         for (int st = 0; st < spt; ++st, ++q) {
             const int slot = q % W_STAGES;
@@ -181,36 +163,50 @@ __device__ __forceinline__ void run_issuer_t(Ctx& c, int n_units, FlagFn flags_o
             NF_PROF_DO(const long long t1_ = clock64();)
             mbar_wait(c.full + slot, (uint32_t)((q / W_STAGES) & 1));
             NF_PROF_DO(c.w_full += clock64() - t1_;)
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t wh = s_u32(c.ring + slot * WST_BYTES);
-            uint64_t dw_hi = umma_desc(wh, WLBO, 128), dw_lo = umma_desc(wh + (KSTAGE / 4) * WLBO, WLBO, 128);
+            const uint32_t wh = s_u32(c.ring + slot * WST_BYTES), wlo = wh + (KSTAGE / 4) * WLBO;
+            const uint32_t xoff = (uint32_t)(st * (KSTAGE / 4) * XLBO);
+            wgmma_fence();
 #pragma unroll
-            for (int ks = 0; ks < KSTAGE / 8; ++ks, ++ks_out) {  // k-step of 8: lo.hi + hi.lo -> correction, hi.hi -> alternating main accumulator
-                if (ks_out < 2 && c.o > 0) {  // first touch of the buffers in this output tile: the epilogue of the previous tile has read them
-                    NF_PROF_DO(const long long t2_ = clock64();)
-                    if (ks_out == 0) mbar_wait(c.buf_empty + 0, (uint32_t)((c.o - 1) & 1));
-                    mbar_wait(c.buf_empty + 1 + ks_out, (uint32_t)((c.o - 1) & 1));
-                    NF_PROF_DO(c.w_buf += clock64() - t2_;)
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                }
-                umma_tf32(c.tmem + TM_CORR, dw_lo, dx_hi, IDESC, ks_out > 0 ? 1u : 0u);
-                umma_tf32(c.tmem + TM_CORR, dw_hi, dx_lo, IDESC, 1u);
-                umma_tf32(c.tmem + ((ks_out & 1) ? TM_MAIN1 : TM_MAIN0), dw_hi, dx_hi, IDESC, ks_out >= 2 ? 1u : 0u);
-                dw_hi += (2 * WLBO) >> 4; dw_lo += (2 * WLBO) >> 4;
-                dx_hi += (2 * XLBO) >> 4; dx_lo += (2 * XLBO) >> 4;
+            for (int ks = 0; ks < KSTAGE / 8; ++ks) {
+                const uint64_t dxh = gmma_desc(x_hi0 + xoff + 2 * ks * XLBO, XLBO, 128), dxl = gmma_desc(x_lo0 + xoff + 2 * ks * XLBO, XLBO, 128);
+                const uint64_t dwh = gmma_desc(wh + 2 * ks * WLBO + h * 1024, WLBO, 128), dwl = gmma_desc(wlo + 2 * ks * WLBO + h * 1024, WLBO, 128);
+                wgmma_tf32_n64(corr, dwl, dxh);
+                wgmma_tf32_n64(corr, dwh, dxl);
+                if (ks & 1) wgmma_tf32_n64(main1, dwh, dxh);
+                else wgmma_tf32_n64(main0, dwh, dxh);
             }
-            umma_commit(c.empty + slot);  // frees the ring stage when these MMAs retire
-            if (c.xsplit && (fl & U_XLAST) && st == STAGES_PER_TILE / 2 - 1) umma_commit(c.x_free);  // first K half: no later MMA reads it
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous stage's group has completed: free its ring slot
+            if (pending >= 0) free_stage(pending);
+            pending = q;
+            if (c.xsplit && (fl & U_XLAST) && st == STAGES_PER_TILE / 2 - 1) {  // first K half: no later MMA reads it
+                wgmma_wait<0>();
+                free_stage(pending); pending = -1;
+                release(c.x_free);
+            }
         }
+        wgmma_wait<0>();
+        if (pending >= 0) { free_stage(pending); pending = -1; }
         if (fl & U_XLAST) {
-            if (!c.xsplit) umma_commit(c.x_free);
-            else { if (spt < STAGES_PER_TILE / 2) umma_commit(c.x_free); umma_commit(c.x_free2); }
+            if (!c.xsplit) release(c.x_free);
+            else { if (spt < STAGES_PER_TILE / 2) release(c.x_free); release(c.x_free2); }
         }
-        if (fl & U_LAST) { umma_commit(c.acc_full); ++c.o; }
+        if (fl & U_LAST) {
+            if (c.o > 0) { NF_PROF_DO(const long long t2_ = clock64();) mbar_wait(c.stage_free, (uint32_t)((c.o - 1) & 1)); NF_PROF_DO(c.w_buf += clock64() - t2_;) }
+            const int f = 64 * h + 16 * wl + (lane >> 2);
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j) {
+                const int n = 8 * j + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(c.stage + f * SROW + n) = make_float2(corr[4 * j] + (main0[4 * j] + main1[4 * j]), corr[4 * j + 1] + (main0[4 * j + 1] + main1[4 * j + 1]));
+                *reinterpret_cast<float2*>(c.stage + (f + 8) * SROW + n) = make_float2(corr[4 * j + 2] + (main0[4 * j + 2] + main1[4 * j + 2]), corr[4 * j + 3] + (main0[4 * j + 3] + main1[4 * j + 3]));
+            }
+            mbar_arrive(c.acc_full);
+            ++c.o;
+        }
     }
 }
-__device__ __forceinline__ void run_issuer(Ctx& c, const Prog& prog) {
-    run_issuer_t(c, prog.n, [&](int u) { return (int)prog.flag[u]; });
+__device__ __forceinline__ void run_issuer(Ctx& c, const Prog& prog, const unsigned char* wt) {
+    run_issuer_t(c, prog.n, [&](int u) { return (int)prog.flag[u]; }, [&](int u) { return (int)prog.tile[u]; }, wt);
 }
 
 // worker warps: fill the activation operand with f(row 0..127 of the tile, chunk 0..31) -> 4 consecutive k values.
@@ -293,78 +289,35 @@ struct XPut {
     }
 };
 
-#define NF_R32(R) "=r"(R[0]), "=r"(R[1]), "=r"(R[2]), "=r"(R[3]), "=r"(R[4]), "=r"(R[5]), "=r"(R[6]), "=r"(R[7]), "=r"(R[8]), "=r"(R[9]), "=r"(R[10]),   \
-          "=r"(R[11]), "=r"(R[12]), "=r"(R[13]), "=r"(R[14]), "=r"(R[15]), "=r"(R[16]), "=r"(R[17]), "=r"(R[18]), "=r"(R[19]), "=r"(R[20]),   \
-          "=r"(R[21]), "=r"(R[22]), "=r"(R[23]), "=r"(R[24]), "=r"(R[25]), "=r"(R[26]), "=r"(R[27]), "=r"(R[28]), "=r"(R[29]), "=r"(R[30]),   \
-          "=r"(R[31])
-#define NF_TMEM_LD32(R, TADDR)                                                                                                                \
-    asm volatile(                                                                                                                             \
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,"   \
-        "%25,%26,%27,%28,%29,%30,%31}, [%32];"                                                                                               \
-        : NF_R32(R)                                                                                                                          \
-        : "r"(TADDR)                                                                                                                         \
-        : "memory")
-#define NF_TMEM_ST32(TADDR, R)                                                                                                                \
-    asm volatile(                                                                                                                             \
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,"   \
-        "%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(TADDR),                                                                                    \
-        "r"(R[0]), "r"(R[1]), "r"(R[2]), "r"(R[3]), "r"(R[4]), "r"(R[5]), "r"(R[6]), "r"(R[7]), "r"(R[8]), "r"(R[9]), "r"(R[10]), "r"(R[11]),        \
-        "r"(R[12]), "r"(R[13]), "r"(R[14]), "r"(R[15]), "r"(R[16]), "r"(R[17]), "r"(R[18]), "r"(R[19]), "r"(R[20]), "r"(R[21]), "r"(R[22]),         \
-        "r"(R[23]), "r"(R[24]), "r"(R[25]), "r"(R[26]), "r"(R[27]), "r"(R[28]), "r"(R[29]), "r"(R[30]), "r"(R[31])                                  \
-        : "memory")
-
-// worker warps: wait for output tile `o`, RN-sum its three accumulators (correction + two main) into the staging columns of this thread's
-// TMEM lane, releasing each accumulator to the issuer as soon as it is in registers.  One copy of this code for all 15 call sites.
-__device__ __noinline__ void drain_to_stage(uint32_t tmem, uint64_t* acc_full, uint64_t* buf_empty, int o, int warp, int add_stage) {
-    mbar_wait(acc_full, (uint32_t)(o & 1));
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t base = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * CPT);
-#pragma unroll 1
-    for (int h = 0; h < CPT / 32; ++h) {  // passes of 32 of this thread's columns: 32 + 32 live registers
-        uint32_t acc[32], r[32];
-        NF_TMEM_LD32(acc, base + TM_CORR + h * 32);
-        NF_TMEM_LD32(r, base + TM_MAIN0 + h * 32);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = __float_as_uint(__uint_as_float(acc[i]) + __uint_as_float(r[i]));
-        NF_TMEM_LD32(r, base + TM_MAIN1 + h * 32);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = __float_as_uint(__uint_as_float(acc[i]) + __uint_as_float(r[i]));
-        if (add_stage) {  // K > 128 split over two output tiles (forward g1pre): the first half waits in the staging columns
-            NF_TMEM_LD32(r, base + TM_STAGE + h * 32);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int i = 0; i < 32; ++i) acc[i] = __float_as_uint(__uint_as_float(acc[i]) + __uint_as_float(r[i]));
-        }
-        if (h == CPT / 32 - 1) {  // all columns of the three buffers are in registers / staged: hand them back
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(buf_empty + 0); mbar_arrive(buf_empty + 1); mbar_arrive(buf_empty + 2);
-        }
-        NF_TMEM_ST32(base + TM_STAGE + h * 32, acc);
-    }
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
+// worker warps: wait for output tile `o` in the staging tile (after telling the issuer that this thread is done with the previous one).
+// add_stage: K > 128 split over two output tiles (forward g1pre): this thread's part of the previous tile is kept and added to the new one.
 __device__ __forceinline__ void drain(Ctx& c, int warp, int add_stage = 0) {
     NF_PROF_DO(const long long t0_ = clock64();)
-    drain_to_stage(c.tmem, c.acc_full, c.buf_empty, c.o, warp, add_stage);
+    float* mine = c.stage + (32 * (warp & 3) + (threadIdx.x & 31)) * SROW + (warp >> 2) * CPT;
+    if (add_stage) {
+        float4 keep[CPT / 4];
+#pragma unroll
+        for (int i = 0; i < CPT / 4; ++i) keep[i] = reinterpret_cast<const float4*>(mine)[i];
+        if (c.o > 0) mbar_arrive(c.stage_free);
+        mbar_wait(c.acc_full, (uint32_t)(c.o & 1));
+#pragma unroll
+        for (int i = 0; i < CPT / 4; ++i) reinterpret_cast<float4*>(mine)[i] = reinterpret_cast<const float4*>(mine)[i] + keep[i];
+    } else {
+        if (c.o > 0) mbar_arrive(c.stage_free);
+        mbar_wait(c.acc_full, (uint32_t)(c.o & 1));
+    }
     NF_PROF_DO(c.w_acc += clock64() - t0_;)
     ++c.o;
 }
 
 // 16 staged values of this thread: atoms CPT (warp >> 2) + 16 cb .. + 15 of its feature
 __device__ __forceinline__ void stage_ld16(const Ctx& c, int warp, int cb, float (&v)[16]) {
-    uint32_t r[16];
-    const uint32_t taddr = c.tmem + ((uint32_t)((warp & 3) * 32) << 16) + TM_STAGE + (uint32_t)((warp >> 2) * CPT + cb * 16);
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-                   "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr)
-                 : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    const float4* src = reinterpret_cast<const float4*>(c.stage + (32 * (warp & 3) + (threadIdx.x & 31)) * SROW + (warp >> 2) * CPT + cb * 16);
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < 4; ++i) {
+        const float4 t = src[i];
+        v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+    }
 }
 
 __device__ __forceinline__ void prog_add(Prog& p, int tile, int flags) {
@@ -373,44 +326,32 @@ __device__ __forceinline__ void prog_add(Prog& p, int tile, int flags) {
     ++p.n;
 }
 
-// common prologue: carve shared memory, init barriers, allocate TMEM
-__device__ __forceinline__ Ctx setup(unsigned char* smem, int tid, int warp, int xsplit = 0) {
+// common prologue: carve shared memory, init barriers
+__device__ __forceinline__ Ctx setup(unsigned char* smem, int tid, int xsplit = 0) {
     Ctx c;
     c.xsplit = xsplit;
     c.x_hi = reinterpret_cast<float*>(smem);
     c.x_lo = reinterpret_cast<float*>(smem + X_BYTES);
     c.ring = smem + 2 * X_BYTES;
+    c.stage = reinterpret_cast<float*>(smem + 2 * X_BYTES + W_STAGES * WST_BYTES);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SMEM_BARS);
     c.full = bars; c.empty = bars + W_STAGES; c.x_ready = bars + 2 * W_STAGES; c.x_free = c.x_ready + 1; c.acc_full = c.x_ready + 2;
-    c.buf_empty = c.x_ready + 3;
+    c.stage_free = c.x_ready + 3;
     c.dep = c.x_ready + 6;  // 4 hand-over barriers between the worker groups
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(c.x_ready + 10);
     c.x_ready2 = c.x_ready + 11; c.x_free2 = c.x_ready + 12;
     if (tid == 0) {
-        for (int s = 0; s < W_STAGES; ++s) { mbar_init(c.full + s, 1); mbar_init(c.empty + s, 1); }
+        for (int s = 0; s < W_STAGES; ++s) { mbar_init(c.full + s, 1); mbar_init(c.empty + s, 8); }  // empty / x_free: one arrival per MMA warp
         mbar_init(c.x_ready, xsplit ? 16 * NLOAD : 32 * NLOAD);  // == 32 * NEPI: one group writes a whole operand generation (half of it with xsplit)
-        mbar_init(c.x_free, 1);
+        mbar_init(c.x_free, 8);
         mbar_init(c.x_ready2, 16 * NLOAD);
-        mbar_init(c.x_free2, 1);
-        mbar_init(c.acc_full, 1);
-        for (int b = 0; b < 3; ++b) mbar_init(c.buf_empty + b, 32 * NEPI);
+        mbar_init(c.x_free2, 8);
+        mbar_init(c.acc_full, 256);
+        mbar_init(c.stage_free, 32 * NEPI);
         for (int b = 0; b < 4; ++b) mbar_init(c.dep + b, 32 * NLOAD);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    c.tmem = *tmem_slot;
     return c;
-}
-__device__ __forceinline__ void teardown(const Ctx& c, int warp) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(c.tmem), "n"(TMEM_COLS) : "memory");
 }
 
 // ---- worker roles

@@ -1,23 +1,22 @@
-// wgrad_tc.cu -- weight gradients of the training step on the tensor cores (sm_100a):
+// wgrad_tc.cu -- weight gradients of the training step on the tensor cores (wgmma, sm_90a):
 //
 //     dW[o, i]  += alpha      * sum_t sum_a  G_t[a, o] * X_t[a, i]          (t = 1 or 2 terms: the tangent pass has tg^T x + g^T tx)
 //     dbias[o]  += bias_alpha *       sum_a  G_b[a, o]                      (optional; b = the term that carries the bias gradient)
 //
 // i.e. what the reference gets from autograd for every nn.Linear of the model (torch: grad_weight = grad_out^T @ input,
-// grad_bias = grad_out.sum(0)) -- round 1 ran one cuBLAS SIMT SGEMM + splitKreduce + a column-sum kernel per Linear (275 launches, 3.7 ms
-// of the 21 ms step).  The contraction runs over ATOMS (K = 10^4), the output is at most 384 x 128: a split-K problem.
+// grad_bias = grad_out.sum(0)) -- instead of one cuBLAS SGEMM + splitKreduce + a column-sum kernel per Linear.  The contraction runs over ATOMS (K = 10^4), the output is at most 384 x 128: a split-K problem.
 //
-// One CTA per SM = 128 outputs x a strided set of (term, 128-atom chunk) sub-units, their products summed in fp32 registers and flushed with ONE
-// set of vector atomics per CTA (first version: one CTA and one 64 KB atomic flush per sub-unit, 35 us per launch under ncu).  Both operands are read ONCE from global memory in their natural row-major
-// layout ([atom, feature], 16-byte loads), split into TF32 hi / lo in registers and TRANSPOSED on the way into shared memory: K-major UMMA
-// operands (K = atoms) written with 4-byte stores whose strides (160 B between 8-feature groups, = 16 B mod 128 between 4-atom chunks) make
-// the 32 lanes of a store hit 32 banks.  (Tried first: MN-major operands, which need no transpose -- instruction-descriptor bits 15 / 16 with
-// the no-swizzle canonical layout of 8-atom x 4-feature core matrices: the MMAs return exact zeros on this part, with the same shared-memory
-// image that the K-major mode reads back as expected; not pursued.)  3xTF32 as in gemm_tc.cu:
-// lo.hi + hi.lo into a correction accumulator, hi.hi alternating over two main accumulators (chains of 8: the tensor core truncates on
-// accumulate).  The bias gradient rides along as 16 extra B columns holding the constant 1 (column `in` of D = column sums of G).
-// Epilogue: TMEM -> registers -> shared-memory staging -> row-contiguous red.global.add.v4.f32 into the gradient bucket.  The sum over
-// atom chunks is therefore atomic (fp32 addition order varies from run to run at the 1e-7 relative level; cuBLAS split-K was deterministic).
+// One CTA per SM = 128 outputs x a strided set of (term, 128-atom chunk) sub-units, their products summed in the wgmma register accumulators
+// and flushed with ONE set of vector atomics per CTA.  Both operands are read ONCE from global memory in their natural row-major layout
+// ([atom, feature], 16-byte loads), split into TF32 hi / lo in registers and TRANSPOSED on the way into shared memory: K-major operands
+// (K = atoms) written with 4-byte stores whose strides (160 B between 8-feature groups, = 16 B mod 128 between 4-atom chunks) make the
+// 32 lanes of a store hit 32 banks (wgmma TF32 reads K-major operands only).  3xTF32 as in gemm_tc.cu: lo.hi + hi.lo into a correction
+// accumulator, hi.hi into a main one; both are reset per (term, 128-atom) sub-unit and folded into fp32 register sums at its end (the
+// tensor core truncates when it accumulates: chains of 16 main products, whatever M and the number of CTAs).  The bias gradient rides
+// along as 16 extra B columns holding the constant 1 in the stages of the
+// terms that carry it (column `in` of D = column sums of G).  Four warpgroups: outputs [64 (g & 1), +64) x B columns [72 (g >> 1), +72).
+// Epilogue: registers -> shared-memory staging -> row-contiguous red.global.add.v4.f32 into the gradient bucket.  The sum over atom chunks
+// is therefore atomic (fp32 addition order varies from run to run at the 1e-7 relative level; cuBLAS split-K was deterministic).
 #include "tc_pipe.cuh"
 
 namespace {
@@ -35,10 +34,6 @@ static_assert(WG_B_LBO >= (WG_NB / 8) * WG_SBO && WG_A_LBO % 128 == 16 && WG_B_L
 constexpr int WG_SMEM_BARS = 2 * WG_STAGE;
 constexpr int WG_SMEM = WG_SMEM_BARS + 64;
 constexpr int WG_SROW = 132;                    // staging row stride (floats): 128 + 4, 16-byte stores of a quarter warp hit 8 bank groups
-constexpr uint32_t WG_TM_CORR = 0, WG_TM_M0 = WG_NB, WG_TM_M1 = 2 * WG_NB;
-static_assert(128 * WG_SROW * 4 <= WG_SMEM_BARS, "staging reuses the operand buffers");
-static_assert(3 * WG_NB <= 512, "TMEM columns");
-
 struct WgParams {
     const float* G[3];
     const float* X[3];
@@ -61,29 +56,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const WgParams P) {
     extern __shared__ __align__(1024) unsigned char smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int o0 = blockIdx.y * 128;
-    // sub-units of this CTA: u = blockIdx.x, + gridDim.x, ... over (term, 128-atom chunk); their products are summed in registers
+    // sub-units of this CTA: u = blockIdx.x, + gridDim.x, ... over (term, 128-atom chunk); their products are summed in the accumulators
     const int n_chunks = (P.M + 127) >> 7, n_sub = n_chunks * P.n_terms;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG_SMEM_BARS);  // [0,1] stage free, [2] accumulators complete
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
-    if (tid == 0) {
-        mbar_init(bars + 0, 1); mbar_init(bars + 1, 1); mbar_init(bars + 2, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    // the constant rows of B (inputs 128..143) of both stages: hi = 1 in row 128 (for every atom), everything else 0
-    for (int i = tid; i < 2 * 2 * (WG_KS / 4) * 16; i += WG_THREADS) {  // (stage, hi/lo, 4-atom chunk, row 128 + r)
-        const int r = i & 15, kc = (i >> 4) & 7, hl = (i >> 7) & 1, st = i >> 8;
-        const float one = (hl == 0 && r == 0) ? 1.0f : 0.0f;
-        *reinterpret_cast<float4*>(smem + st * WG_STAGE + 2 * WG_A_BYTES + hl * WG_B_BYTES + kc * WG_B_LBO + (16 + (r >> 3)) * WG_SBO + (r & 7) * 16) =
-            make_float4(one, one, one, one);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = *tmem_slot;
 
     // loader mapping: a warp instruction covers 8 atoms x 16 features (lane = 8 * feature-quad + atom): 64-byte global segments.  Shared-memory
     // word of (feature f, atom a) = (f / 8) SBO + (f % 8) 16 + (a / 4) LBO + (a % 4) 4: for one of the 4 features of a lane's float4 the 32
@@ -112,21 +86,20 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const WgParams P) {
         const int term = u / n_chunks, a0 = (u - term * n_chunks) << 7;
         return (min(128, P.M - a0) + WG_KS - 1) / WG_KS;
     };
-    constexpr uint32_t IDESC = umma_idesc_tf32(128, WG_NB);
-    const int q = warp & 3, cp = warp >> 2, orow = q * 32 + lane;
-    float sum[32];  // this thread's 32 outputs (row orow, columns cp * 32 ..) summed over the sub-units, fp32
+    const int wg = warp >> 2, mh = wg & 1, nh = wg >> 1;
+    float corr[36], acc[36], total[36];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) sum[i] = 0.f;
-    float bsum = 0.f;
-    int gs = 0, it = 0;  // stages / sub-units done so far (shared-memory buffer and barrier phases)
-    load_stage(blockIdx.x, 0);
+    for (int i = 0; i < 36; ++i) { corr[i] = 0.f; acc[i] = 0.f; total[i] = 0.f; }
+    int gs = 0;  // stages done so far (shared-memory buffer)
+    if (blockIdx.x < n_sub) load_stage(blockIdx.x, 0);
 #pragma unroll 1
-    for (int u = blockIdx.x; u < n_sub; u += gridDim.x, ++it) {
+    for (int u = blockIdx.x; u < n_sub; u += gridDim.x) {
         const int n_st = stages_of(u);
+        const bool bias_on = P.dbias != nullptr && ((P.bias_mask >> (u / n_chunks)) & 1);
 #pragma unroll 1
         for (int st = 0; st < n_st; ++st, ++gs) {
             unsigned char* sb = smem + (gs & 1) * WG_STAGE;
-            if (gs >= 2) mbar_wait(bars + (gs & 1), (uint32_t)(((gs >> 1) - 1) & 1));  // the MMAs that read this buffer two stages ago are done
+            __syncthreads();  // every warpgroup has waited for its MMAs of stage gs - 2, which read this buffer
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
                 const int inst = warp + 16 * j, kg = inst >> 3, fb = inst & 7;
@@ -145,67 +118,55 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const WgParams P) {
                 bh[0] = hi.x; bh[4] = hi.y; bh[8] = hi.z; bh[12] = hi.w;
                 bl[0] = lo.x; bl[4] = lo.y; bl[8] = lo.z; bl[12] = lo.w;
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");  // also orders the previous sub-unit's TMEM drain before its overwrite
-            __syncthreads();
-            if (tid == 0) {
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t sa = s_u32(sb);
-#pragma unroll
-                for (int kg = 0; kg < WG_KS / 8; ++kg) {
-                    const int ks = st * (WG_KS / 8) + kg;
-                    const uint64_t a_hi = umma_desc(sa + 2 * kg * WG_A_LBO, WG_A_LBO, WG_SBO), a_lo = umma_desc(sa + WG_A_BYTES + 2 * kg * WG_A_LBO, WG_A_LBO, WG_SBO);
-                    const uint64_t b_hi = umma_desc(sa + 2 * WG_A_BYTES + 2 * kg * WG_B_LBO, WG_B_LBO, WG_SBO),
-                                   b_lo = umma_desc(sa + 2 * WG_A_BYTES + WG_B_BYTES + 2 * kg * WG_B_LBO, WG_B_LBO, WG_SBO);
-                    umma_tf32(tmem + WG_TM_CORR, a_lo, b_hi, IDESC, ks > 0 ? 1u : 0u);
-                    umma_tf32(tmem + WG_TM_CORR, a_hi, b_lo, IDESC, 1u);
-                    umma_tf32(tmem + ((ks & 1) ? WG_TM_M1 : WG_TM_M0), a_hi, b_hi, IDESC, ks >= 2 ? 1u : 0u);
-                }
-                umma_commit(bars + (gs & 1));
-                if (st == n_st - 1) umma_commit(bars + 2);
+            if (tid < 2 * (WG_KS / 4) * 16) {  // the constant rows of B (inputs 128..143): hi = 1 in row 128 for a bias-carrying term, else 0
+                const int r = tid & 15, kc = (tid >> 4) & 7, hl = tid >> 7;
+                const float one = (hl == 0 && r == 0 && bias_on) ? 1.0f : 0.0f;
+                *reinterpret_cast<float4*>(sb + 2 * WG_A_BYTES + hl * WG_B_BYTES + kc * WG_B_LBO + (16 + (r >> 3)) * WG_SBO + (r & 7) * 16) =
+                    make_float4(one, one, one, one);
             }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncthreads();
+            const uint32_t sa = s_u32(sb) + mh * 8 * WG_SBO, sbb = s_u32(sb) + 2 * WG_A_BYTES + nh * 9 * WG_SBO;
+            wgmma_fence();
+#pragma unroll
+            for (int kg = 0; kg < WG_KS / 8; ++kg) {
+                const uint64_t a_hi = gmma_desc(sa + 2 * kg * WG_A_LBO, WG_A_LBO, WG_SBO), a_lo = gmma_desc(sa + WG_A_BYTES + 2 * kg * WG_A_LBO, WG_A_LBO, WG_SBO);
+                const uint64_t b_hi = gmma_desc(sbb + 2 * kg * WG_B_LBO, WG_B_LBO, WG_SBO), b_lo = gmma_desc(sbb + WG_B_BYTES + 2 * kg * WG_B_LBO, WG_B_LBO, WG_SBO);
+                wgmma_tf32_n72(corr, a_lo, b_hi);
+                wgmma_tf32_n72(corr, a_hi, b_lo);
+                wgmma_tf32_n72(acc, a_hi, b_hi);
+            }
+            wgmma_commit();
             // next stage's global loads in flight while the tensor core works on this one (across the sub-unit boundary too)
             if (st + 1 < n_st) load_stage(u, st + 1);
             else if (u + (int)gridDim.x < n_sub) load_stage(u + gridDim.x, 0);
+            wgmma_wait<1>();
         }
-        // ---- this sub-unit's D = corr + main0 + main1 (chains of <= 8 accumulations each) into the fp32 register sums
-        mbar_wait(bars + 2, (uint32_t)(it & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        {
-            uint32_t r[32];
-            const uint32_t base = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(cp * 32);
+        wgmma_wait<0>();  // this sub-unit's products -> fp32 sums (RN adds), accumulators restart
 #pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                NF_TMEM_LD32(r, base + (uint32_t)(k * WG_NB));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        for (int i = 0; i < 36; ++i) { total[i] += corr[i] + acc[i]; corr[i] = 0.f; acc[i] = 0.f; }
+    }
+
+    // ---- epilogue: fragments -> staging rows [output][input] (the operand buffers: every MMA has completed) -> coalesced vector
+    //      reductions into dW, one per CTA and output element.  Fragment: rows 64 mh + 16 (warp & 3) + lane / 4 (+ 8), B columns
+    //      72 nh + 8 j + 2 (lane & 3) (+ 1); column 128 (nh = 1, j = 7, lane & 3 = 0) is the bias gradient.
+    __syncthreads();
+    float* stage = reinterpret_cast<float*>(smem);
+    const int orow = 64 * mh + 16 * (warp & 3) + (lane >> 2);
 #pragma unroll
-                for (int i = 0; i < 32; ++i) sum[i] += __uint_as_float(r[i]);
-            }
-            if (cp == 0 && P.dbias != nullptr && ((P.bias_mask >> (u / n_chunks)) & 1)) {  // warp-uniform: column 128 = sum over atoms of G[:, o]
-                uint32_t b[3][16];
+    for (int j = 0; j < 9; ++j) {
+        const int col = 72 * nh + 8 * j + 2 * (lane & 3);
 #pragma unroll
-                for (int k = 0; k < 3; ++k) {
-                    const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(k * WG_NB + 128);
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                                 : "=r"(b[k][0]), "=r"(b[k][1]), "=r"(b[k][2]), "=r"(b[k][3]), "=r"(b[k][4]), "=r"(b[k][5]), "=r"(b[k][6]), "=r"(b[k][7]),
-                                   "=r"(b[k][8]), "=r"(b[k][9]), "=r"(b[k][10]), "=r"(b[k][11]), "=r"(b[k][12]), "=r"(b[k][13]), "=r"(b[k][14]), "=r"(b[k][15])
-                                 : "r"(taddr)
-                                 : "memory");
-                }
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                bsum += __uint_as_float(b[0][0]) + __uint_as_float(b[1][0]) + __uint_as_float(b[2][0]);
+        for (int hr = 0; hr < 2; ++hr) {
+            const int e = 4 * j + 2 * hr, r = orow + 8 * hr;
+            if (col < 128) {
+                *reinterpret_cast<float2*>(stage + r * WG_SROW + col) = make_float2(total[e] * P.alpha, total[e + 1] * P.alpha);
+            } else if (col == 128 && P.dbias != nullptr && o0 + r < P.out) {
+                const float bsum = total[e];
+                if (bsum != 0.f) atomicAdd(P.dbias + o0 + r, P.bias_alpha * bsum);
             }
         }
     }
-
-    // ---- epilogue: register sums -> staging rows [output][input] (the operand buffers: every MMA has completed) -> coalesced vector
-    //      reductions into dW, one per CTA and output element
-    float* stage = reinterpret_cast<float*>(smem);
-#pragma unroll
-    for (int i = 0; i < 32; i += 4)
-        *reinterpret_cast<float4*>(stage + orow * WG_SROW + cp * 32 + i) = make_float4(sum[i] * P.alpha, sum[i + 1] * P.alpha, sum[i + 2] * P.alpha, sum[i + 3] * P.alpha);
-    if (cp == 0 && P.dbias != nullptr && o0 + orow < P.out && bsum != 0.f) atomicAdd(P.dbias + o0 + orow, P.bias_alpha * bsum);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
     if (4 * lane < P.in) {
 #pragma unroll 4
@@ -214,7 +175,6 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const WgParams P) {
             red4(P.dW + (size_t)(o0 + r) * P.lddw + 4 * lane, *reinterpret_cast<const float4*>(stage + r * WG_SROW + 4 * lane));
         }
     }
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(512) : "memory");
 }
 
 }  // namespace
@@ -232,7 +192,7 @@ static int wgrad_launch(WgParams& P, cudaStream_t s) {
         if (cudaFuncSetAttribute(k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM) != cudaSuccess) return nb_check_launch();
         attr_set = true;
     }
-    static const int n_sm = [] { int dev = 0, n = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n; }();
+    const int n_sm = nb_sm_count();
     const int out_tiles = (P.out + 127) / 128, n_sub = ((P.M + 127) / 128) * P.n_terms;
     int groups = n_sm / out_tiles;  // one CTA per SM; each sums its (term, chunk) sub-units in registers before ONE atomic flush
     groups = groups < 1 ? 1 : groups > n_sub ? n_sub : groups;

@@ -1,4 +1,4 @@
-"""B200-native drop-in for `nablaDFT.gemnet_oc.GemNetOC` (config/model/gemnet-oc.yaml): SURVEY.md section 8 a19 / f3.
+"""H100-native drop-in for `nablaDFT.gemnet_oc.GemNetOC` (config/model/gemnet-oc.yaml): SURVEY.md section 8 a19 / f3.
 
 Same constructor signature (`nablaDFT/gemnet_oc/gemnet_oc.py:171-228`), same `forward(data) -> (energy [B], forces [N, 3])` contract
 (gemnet_oc.py:1121-1251) and the same state-dict names / shapes (429 entries for the shipped config), so the yaml works with
@@ -370,7 +370,7 @@ class GemNetOC(nn.Module):
         """data.z [N], data.pos [N,3], data.batch [N] (sorted) -> (E_t [B], F_t [N,3])   (gemnet_oc.py:1121-1251)."""
         pos = data.pos
         if not pos.is_cuda:
-            raise NablaB200Error("GemNetOC runs on CUDA tensors only (sm_100a engine; there is no CPU path)")
+            raise NablaB200Error("GemNetOC runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
         if self._runner is None:
             from . import _lib
 

@@ -1,10 +1,10 @@
-"""B200-native drop-in for `nablaDFT.painn_pyg.PaiNN` (config/model/painn-oc.yaml).
+"""H100-native drop-in for `nablaDFT.painn_pyg.PaiNN` (config/model/painn-oc.yaml).
 
 Same constructor signature, same `forward(data) -> (energy, forces)` contract and the same
 state_dict names/shapes as the reference class (`nablaDFT/painn_pyg/painn.py:22-148`,
 SURVEY.md section 8b), so `config/model/painn-oc.yaml` works with
 `_target_: nabladft_b200.painn_oc.PaiNN` and reference checkpoints load with strict=True.
-The arithmetic runs in `libnabla_b200.so` (hand-written sm_100a kernels + cuBLAS SGEMM).
+The arithmetic runs in `libnabla_b200.so` (hand-written sm_90a kernels + cuBLAS SGEMM).
 
 Inference: energy + autograd-free analytic forces.  Training mode returns (energy, forces) on one autograd node
 (`training.PainnEnergyFn`): analytic parameter gradients, the `create_graph=True` force term (painn.py:142) as an exact tangent pass.

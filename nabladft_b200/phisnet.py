@@ -1,9 +1,9 @@
-"""PhiSNet Clebsch-Gordan mixing layers on the B200 engine (SURVEY.md section 8 f4) -- mirrors of
+"""PhiSNet Clebsch-Gordan mixing layers on the H100 engine (SURVEY.md section 8 f4) -- mirrors of
 `nablaDFT/phisnet/nn/modules/{clebsch_gordan,pair_mixing,self_mixing,spherical_linear}.py`: same constructor signatures, parameter names
 (`coeff_{l1}_{l2}_{L}.weight`, `mixcoeff_{l1}_{l2}_{L}`, `keepcoeff_{L}`, `mixing.*`, `linear.{L}.*`) and call contracts (features = lists
 over the order L of tensors [..., 2L+1, F]), so a reference state dict loads with strict=True and a PhiSNet built from the reference's
 `neural_network.py` can swap these modules in.  The arithmetic is in csrc/phisnet.cu (CG contractions, real CG table of the reference
-compiled in) and the tcgen05 3xTF32 GEMM (distance-dependent coefficients, per-order Linear).  Inference only; CUDA only (no CPU fallback).
+compiled in) and the wgmma 3xTF32 GEMM (distance-dependent coefficients, per-order Linear).  Inference only; CUDA only (no CPU fallback).
 """
 from typing import List
 

@@ -1,11 +1,11 @@
-"""B200-native drop-in for `nablaDFT.qhnet.QHNet` (config/model/qhnet.yaml): Hamiltonian prediction.
+"""H100-native drop-in for `nablaDFT.qhnet.QHNet` (config/model/qhnet.yaml): Hamiltonian prediction.
 
 Same constructor signature, `forward(data, keep_blocks=False)` contract and state_dict names/shapes
 as the reference class (`nablaDFT/qhnet/qhnet.py:24-342`, `layers.py`), so
 `config/model/qhnet-b200.yaml` only swaps the `_target_`.  The arithmetic runs in libnabla_b200.so:
 neighbour build, exp-Bernstein/spherical-harmonic edge basis, NormGate pieces, invariant edge
 features, the three Clebsch-Gordan tensor products (coefficients unrolled as literals), e3nn
-Linear / MLP layers on the tcgen05 3xTF32 GEMM, Expansion and the block assembly (which replaces the
+Linear / MLP layers on the wgmma 3xTF32 GEMM, Expansion and the block assembly (which replaces the
 reference's O(n^2 P) Python loop with one kernel).  PyTorch here only allocates buffers and
 sequences the calls.  Inference only (no autograd through the kernels).
 

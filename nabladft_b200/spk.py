@@ -1,4 +1,4 @@
-"""B200-native drop-ins for the schnetpack classes named by config/model/{painn,schnet}.yaml.
+"""H100-native drop-ins for the schnetpack classes named by config/model/{painn,schnet}.yaml.
 
 The reference instantiates (Hydra `_target_`, config/model/painn.yaml:5-28)
 

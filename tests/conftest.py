@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (built for H100, sm_90a; run with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

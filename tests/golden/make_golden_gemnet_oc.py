@@ -12,6 +12,7 @@ Third-party primitives the reference imports are provided as semantic shims (pub
 
     python tests/golden/make_golden_gemnet_oc.py      # writes tests/golden/gemnet_oc_f32.npz
 """
+import hashlib
 import importlib.util
 import os
 import sys
@@ -182,7 +183,8 @@ def main():
             graphs[f"{name}/{k}"] = t[k].numpy().astype(np.int32)
     q = g[8]
     for k in ("out", "trip_in_to_quad", "trip_out_to_quad", "out_agg"):
-        graphs[f"quad/{k}"] = q[k].numpy().astype(np.int32)
+        a = np.ascontiguousarray(q[k].numpy().astype(np.int32))  # 526 k entries each: stored as sha1 + length (the file stays under 1 MB)
+        graphs[f"quad/{k}/sha1"], graphs[f"quad/{k}/len"] = np.asarray(hashlib.sha1(a.tobytes()).hexdigest()), np.asarray(a.shape[0])
     for tk in ("triplet_in", "triplet_out"):
         for k in ("in", "out"):
             graphs[f"quad/{tk}/{k}"] = q[tk][k].numpy().astype(np.int32)
@@ -191,7 +193,6 @@ def main():
     print({k: v.shape for k, v in graphs.items()}, {k: v.shape for k, v in inter.items()})
     print("E", e.ravel(), "max|F|", np.abs(f).max(), "params", sum(p.numel() for p in net.parameters()))
     # a second batch (three other molecules): outputs + SHA-1 of every index array, to harden the pin without growing the file
-    import hashlib
 
     mols2 = [3, 12, 41]
     z2 = torch.from_numpy(np.concatenate([fx["z"][fx["ptr"][m]:fx["ptr"][m + 1]] for m in mols2])).long()

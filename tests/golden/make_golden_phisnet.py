@@ -94,6 +94,8 @@ def main():
             out[f"{tag}/x/{L}"] = t.numpy()
         for L, t in enumerate(ys):
             out[f"{tag}/y/{L}"] = t.detach().numpy()
+    # every layer acts row by row (pair / atom), so the stored pair rows are cut to the first 3 of the 4 generated: the file stays under 1 MB
+    out = {k: np.ascontiguousarray(v[:, :3]) if k.startswith("pair") else v for k, v in out.items()}
     np.savez_compressed(os.path.join(HERE, "phisnet_mixing.npz"), **out)
     print("wrote phisnet_cg_L4.npz (%d tensors) and phisnet_mixing.npz (%d arrays)" % (len(table), len(out)))
 

@@ -58,10 +58,10 @@ def test_reader_follows_reference_row_semantics(packed):
     assert np.array_equal(ds.energy, fx["energy"][:len(mols)].astype(np.float32))
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/tests/data/raw/test_database.db"), reason="reference checkout not present")
 def test_reader_on_the_reference_fixture_database():
+    # tests/golden/test_database.db: the reference's fixture database (tests/data/raw/test_database.db), stored unmodified
     fx = np.load(os.path.join(GOLDEN, "fixture_molecules.npz"))
-    d = read_ase_energy_db("/root/reference/tests/data/raw/test_database.db")
+    d = read_ase_energy_db(os.path.join(GOLDEN, "test_database.db"))
     assert np.array_equal(d["z"], fx["z"]) and np.array_equal(d["ptr"], fx["ptr"]) and np.array_equal(d["pos"], fx["pos"].astype(np.float32))
     assert np.array_equal(d["forces"], fx["forces"].astype(np.float32)) and np.array_equal(d["energy"], fx["energy"].astype(np.float32))
 
@@ -173,12 +173,12 @@ def test_hamiltonian_db_reader_and_packed_batches(tmp_path):
     assert float(HamiltonianLoss.packed(targets, targets)) == 0.0
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/tests/data/raw/test_hamiltonian_database.db"), reason="reference checkout not present")
 def test_hamiltonian_reader_on_the_reference_fixture_database():
     from nabladft_b200.data import read_hamiltonian_db
 
-    a = read_hamiltonian_db("/root/reference/tests/data/raw/test_hamiltonian_database.db")
-    assert len(a["energy"]) == 25 and int(a["ptr"][1]) == 38 and int(a["norb"][0]) == 396        # SURVEY.md section 8c: mol 0 = 38 atoms, 396 x 396
+    # tests/golden/hamiltonian_mol0.db: the reference's fixture database shrunk to molecule 0 (make_golden_hamiltonian_db.py)
+    a = read_hamiltonian_db(os.path.join(GOLDEN, "hamiltonian_mol0.db"))
+    assert len(a["energy"]) == 1 and int(a["ptr"][1]) == 38 and int(a["norb"][0]) == 396        # SURVEY.md section 8c: mol 0 = 38 atoms, 396 x 396
     h0 = a["H"][: 396 * 396].reshape(396, 396)
     assert np.abs(h0 - h0.T).max() < 1e-5                                                          # a Fock matrix is symmetric
     d = np.linalg.norm(a["pos"][1] - a["pos"][0])

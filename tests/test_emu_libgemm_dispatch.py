@@ -1,4 +1,4 @@
-"""The device builds of the functor engines send their dense layers to library GEMMs (the tcgen05 kernel of gemm_tc.cu, cuBLAS SGEMM for weight
+"""The device builds of the functor engines send their dense layers to library GEMMs (the wgmma kernels of gemm_tc.cu / gemm_ps.cu, cuBLAS SGEMM for weight
 gradients); host emulation normally replaces them by functor GEMMs.  With NB200_EMU_LIBGEMM=1 the emulation shim takes the SAME dispatch
 decisions as the device build and runs reference loops with the exact interface semantics of those libraries (strides, trans_b, accumulate,
 bias; the cuBLAS argument order) -- so this run checks the ARGUMENTS the engines pass on the device path.  One representative test per engine,

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on a B200 with `-m gpu`): every call goes through the C ABI
+"""GPU parity tests (run on an H100 with `-m gpu`): every call goes through the C ABI
 (libnabla_b200.so) and is compared with the CPU oracle / the golden vectors generated from
 the reference's own code.  Tolerances are the north-star ones: |dE| <= 1e-5 Ha, |dF| <= 1e-4
 Ha/A (fp32 path vs fp64 oracle), written next to each assert."""
@@ -347,7 +347,7 @@ def test_engine_edge_cases():
     (2200, 136, 96, 1, 0, False, False),
 ])
 def test_gemm_tf32x3_matches_fp64(M, N, K, trans_b, accumulate, with_bias, with_act):
-    """tcgen05 3xTF32 GEMM (node-level dense layers) == fp64 matmul to fp32-level accuracy."""
+    """wgmma 3xTF32 GEMM (node-level dense layers) == fp64 matmul to fp32-level accuracy."""
     from nabladft_b200 import _lib
 
     lib = _lib.load()
@@ -369,7 +369,7 @@ def test_gemm_tf32x3_matches_fp64(M, N, K, trans_b, accumulate, with_bias, with_
     scale = ref.abs().max().item()
     err = (C.double() - ref).abs().max().item()
     sgemm_err = ((A @ (B if trans_b else B.T) + (C0 if accumulate else 0) + (bias if with_bias else 0)).double() - ref).abs().max().item()
-    print(f"gemm {M}x{N}x{K} trans_b={trans_b}: rel err tcgen05-3xTF32 {err / scale:.2e}  torch fp32 {sgemm_err / scale:.2e}")
+    print(f"gemm {M}x{N}x{K} trans_b={trans_b}: rel err wgmma-3xTF32 {err / scale:.2e}  torch fp32 {sgemm_err / scale:.2e}")
     if not (with_act and N >= 512 and K <= 128 and M >= 1024):
         assert err < 2e-6 * scale, f"rel err {err / scale:.2e}"  # fp32 SGEMM itself: ~1e-6 at K=384
     if with_act:
@@ -387,7 +387,7 @@ def test_gemm_tf32x3_matches_fp64(M, N, K, trans_b, accumulate, with_bias, with_
     (128, 8, 16, 1, True, 0, 0),          # smallest shapes the kernel takes
 ])
 def test_linear_wgrad_matches_fp64(M, out, inn, terms, bias, scale_div, lddw_extra):
-    """tcgen05 split-K weight-gradient kernel (wgrad_tc.cu) == fp64 grad_out^T @ input / grad_out.sum(0) to fp32 accuracy, accumulated."""
+    """wgmma split-K weight-gradient kernel (wgrad_tc.cu) == fp64 grad_out^T @ input / grad_out.sum(0) to fp32 accuracy, accumulated."""
     from nabladft_b200 import _lib
 
     lib = _lib.load()
@@ -425,7 +425,7 @@ def test_linear_wgrad_matches_fp64(M, out, inn, terms, bias, scale_div, lddw_ext
 
 
 def test_engine_gemm_backends_agree():
-    """Whole-model E,F with the tcgen05 GEMMs vs the cuBLAS SGEMM path: both within tolerance of each other."""
+    """Whole-model E,F with the wgmma GEMMs vs the cuBLAS SGEMM path: both within tolerance of each other."""
     net = _oc_model(6).to(dev())
     z, pos, batch = load_fixture([30, 31, 32], torch.float32)
     d = _Data(z.to(dev()), pos.to(dev()), batch.to(dev()))

@@ -186,6 +186,8 @@ def test_gemnet_oc_graph_oracle_matches_reference_indices_exactly():
     import numpy as np
     import torch
 
+    import hashlib
+
     from oracle.gemnet_graph import build_all_indices
 
     g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gemnet_oc_f32.npz"))
@@ -198,8 +200,9 @@ def test_gemnet_oc_graph_oracle_matches_reference_indices_exactly():
     for name in ("trip_e2e", "trip_a2e", "trip_e2a"):
         for k in ("in", "out", "out_agg"):
             assert np.array_equal(o[name][k].numpy(), g[f"{name}/{k}"]), (name, k)
-    for k in ("out", "trip_in_to_quad", "trip_out_to_quad", "out_agg"):
-        assert np.array_equal(o["quad"][k].numpy(), g[f"quad/{k}"]), k
+    for k in ("out", "trip_in_to_quad", "trip_out_to_quad", "out_agg"):  # stored as sha1 of the int32 array + its length
+        a = np.ascontiguousarray(o["quad"][k].numpy().astype(np.int32))
+        assert a.shape[0] == int(g[f"quad/{k}/len"]) and hashlib.sha1(a.tobytes()).hexdigest() == str(g[f"quad/{k}/sha1"]), k
     for tk in ("triplet_in", "triplet_out"):
         for k in ("in", "out"):
             assert np.array_equal(o["quad"][tk][k].numpy(), g[f"quad/{tk}/{k}"]), (tk, k)

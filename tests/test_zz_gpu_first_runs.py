@@ -1,7 +1,7 @@
 """Device parity of the two functor engines: GemNet-OC (SURVEY.md section 8 a19, csrc/gemnet_oc.cu; training: csrc/gemnet_oc_train.inc)
 and SchNet training on energy + force losses (config/model/schnet.yaml, BASELINE configs[0]; csrc/schnet_train.cu).
 
-Written without GPU access in round 1 and first executed on a B200 at the start of round 2 (profiles/r2_gemnet_first_bench.json): all four
+Written without GPU access and first executed on a GPU afterwards: all four
 passed, so the round-1 `xfail(strict=False)` marks are gone and the tolerances are north_star's ABSOLUTE ones -- 1e-5 Ha on energies,
 1e-4 Ha/A on forces (measured: 2.4e-6 Ha / 6e-7 Ha/A for GemNet-OC against the outputs of the reference's own classes) -- and 5e-5 of a
 tensor's largest entry for parameter gradients (measured 7e-6).  Model runs stay in a SUBPROCESS with a timeout and a second run with
@@ -107,7 +107,7 @@ print("RESULT " + json.dumps(out))
 
 
 def test_gemm_tf32x3_at_gemnet_shapes():
-    """The tcgen05 GEMM at the shapes and strides this model adds (long K, weight column blocks with ldw > K, strided outputs) -- in a
+    """The wgmma GEMM at the shapes and strides this model adds (long K, weight column blocks with ldw > K, strided outputs) -- in a
     subprocess, so that a fault at a never-run shape cannot take the pytest process (and the suites before it) down."""
     p = subprocess.run([sys.executable, "-c", _GEMM_CHILD, ROOT, json.dumps(_GEMM_SHAPES)], capture_output=True, text=True, timeout=150)
     line = [ln for ln in p.stdout.splitlines() if ln.startswith("RESULT ")]
@@ -150,7 +150,7 @@ print("RESULT " + json.dumps(res))
 
 
 def _train_child(script, ok, timeout):
-    """Run a training child with the library GEMMs (tcgen05 / cuBLAS) and, if that fails, once more with NB200_GOC_GEMM=simt (the functor
+    """Run a training child with the library GEMMs (wgmma / cuBLAS) and, if that fails, once more with NB200_GOC_GEMM=simt (the functor
     GEMMs the host emulation verified) so that the failure message separates the kernels from the GEMM dispatch."""
     out = {}
     for tag, env in (("default", {}), ("simt", {"NB200_GOC_GEMM": "simt"})):

@@ -1,5 +1,5 @@
 """Experiment behind the decision recorded in nabladft_b200/training.py: a central finite difference of the analytic energy gradient as the
-force-loss gradient, against the oracle's exact double backward.  Result on a B200 (3 fixture molecules, 3 layers, fp32):
+force-loss gradient, against the oracle's exact double backward.  Result (3 fixture molecules, 3 layers, fp32):
     h 1e-3: whole-gradient rel L2 error 0.80 | 3e-3: 0.27 | 1e-2: 0.12 | 3e-2: 0.10 | 1e-1: 0.45   (worst tensor off by > 100 %)
 => rejected.  The script reimplements the difference on top of PainnEngine.run_train so that it keeps working."""
 import os, sys

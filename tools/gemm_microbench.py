@@ -1,4 +1,4 @@
-"""Time the tcgen05 3xTF32 GEMM against torch.matmul (cuBLAS SGEMM) on the shapes the engines use."""
+"""Time the wgmma 3xTF32 GEMM against torch.matmul (cuBLAS SGEMM) on the shapes the engines use."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

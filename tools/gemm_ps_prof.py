@@ -37,7 +37,7 @@ n = max(out[7], 1)
 tiles = ((N + 127) // 128) * ((K + 127) // 128)
 m_tiles = (M + 127) // 128
 print(f"[{M} x {N} x {K}]: {e0.elapsed_time(e1) / reps * 1e3:.1f} us per call (with profiling code), {n / reps:.0f} CTAs per call, ~{tiles * m_tiles / (n / reps):.1f} (N tile, K chunk) units per CTA")
-names = ["issuer total", "issuer waits X", "issuer waits TMEM buffers", "issuer waits W ring", "worker total", "worker waits accumulator + drain", "worker waits X release", "(CTAs)",
+names = ["issuer total", "issuer waits X", "issuer waits staging", "issuer waits W ring", "worker total", "worker waits accumulator + drain", "worker waits X release", "(CTAs)",
          "worker epilogue (global stores)"]
 for i, nm in enumerate(names):
     if i == 7:

@@ -2,7 +2,7 @@
 
 Each output is the reference file with ONLY the model-class `_target_`s swapped for the nabladft_b200 mirrors, so that
 `run.py --config-name ... model=<name>-b200` instantiates the same Lightning task / optimizer / scheduler / losses / metrics
-around the B200 engine (INTEGRATION.md section 1).  Everything that is not a model class keeps the reference's target.
+around the H100 engine (INTEGRATION.md section 1).  Everything that is not a model class keeps the reference's target.
 """
 import os
 import sys

@@ -32,7 +32,7 @@ for _ in range(steps):
     eng.launch(d["z"], d["pos"], d["mol_ptr"], 256)
 torch.cuda.synchronize()
 fn(out, 0)
-names = ["issuer total", "issuer waits X", "issuer waits TMEM buffers", "issuer waits W ring", "worker total", "worker waits accumulator", "worker waits X release"]
+names = ["issuer total", "issuer waits X", "issuer waits staging", "issuer waits W ring", "worker total", "worker waits accumulator", "worker waits X release"]
 for base, tag in ((0, "k_node_fwd"), (8, "k_node_bwd")):
     n = out[base + 7]
     print(f"{tag}: {n} CTA runs ({n / steps:.0f} per step)")

@@ -1,4 +1,4 @@
-"""Debug harness of the tcgen05 weight-gradient kernel: structured inputs whose products identify operand-layout mistakes."""
+"""Debug harness of the wgmma weight-gradient kernel: structured inputs whose products identify operand-layout mistakes."""
 import sys
 import torch
 sys.path.insert(0, ".")
