@@ -480,6 +480,37 @@ int nb200_phis_self_mixing(const float* x, const float* mixcoeff, const float* k
 int nb200_phis_linear(const float* x, const float* W_l, const float* bias, int32_t n_rows, int32_t c_in, int32_t c_out,
                       int32_t order, float* y, void* stream);
 
+/* PhiSNet model forward (csrc/phisnet_model.cu, neural_network.py:717-995); order 4, features [rows][25][F].  Pair rows follow the full
+ * CSR graph of nb200_neighbor_build (target-major, sources ascending = the reference's fill_idx order).
+ *   nb200_phis_swish_self_mixing  SelfMixing(4, 4) of swish(x) (swish on component 0 only; alpha = beta = NULL: no swish)
+ *   nb200_phis_linear_ex          nb200_phis_linear with accumulate (y += x . W_l): the residual add of ResidualBlock
+ *   nb200_phis_interaction        y[i] = yi[i] + sum_j PairMixing(yj[j], angular_fn1(sh)) + radial_fn(rbf) angular_fn2(sh) yj[j]_0;
+ *                                 coeff[P][70][F] = rbf . [65 mixing paths, 5 radial_fn]^T; wa*[5][F], ba*[F] = angular_fn Linear(1, F)
+ *   nb200_phis_pair_features      fii[i] = fpc[i] + sum_j radial_ii(rbf) fpn[j];  fij[e] = mix_ij(fpc[i], fpc[j]) + sum_{k != i,j}
+ *                                 radial_ij(rbf_ik) fpn[k]; coeff[P][75][F] = rbf . [65 mix_ij paths, 5 radial_ii, 5 radial_ij]^T
+ *   nb200_phis_overlap_pairs      s[e] = mix_s(x[i], (x[j]_0, angular_fn(sh)_{L>0})); coeff[P][65][F]; wa[5][F]
+ *   nb200_phis_assemble           output heads + matrix assembly: per block, only the irreps it uses, sum_f X[L][m][f] W_L[c][f] (+bias),
+ *                                 contracted with sqrt(2L+1) CG(l_i, l_j, L); writes B + B^T into per-molecule matrices M (offsets mol_off);
+ *                                 W[5][n_col][F] (nn.Linear weights), element / shell / entry tables built on the host (nabladft_b200/phisnet.py)
+ */
+int nb200_phis_swish_self_mixing(const float* x, const float* alpha, const float* beta, const float* mixcoeff, const float* keepcoeff,
+                                 int32_t n_rows, int32_t n_feat, float* y, void* stream);
+int nb200_phis_linear_ex(const float* x, const float* W_l, const float* bias, int32_t n_rows, int32_t c_in, int32_t c_out, int32_t order,
+                         int32_t accumulate, float* y, void* stream);
+int nb200_phis_interaction(const float* yi, const float* yj, const float* sh, const float* coeff, const float* wa1, const float* ba1,
+                           const float* wa2, const float* ba2, const int32_t* row_ptr, const int32_t* col, int32_t n_atoms, int32_t n_feat,
+                           float* y, void* stream);
+int nb200_phis_pair_features(const float* fpc, const float* fpn, const float* coeff, const int32_t* row_ptr, const int32_t* col,
+                             int32_t n_atoms, int32_t n_feat, float* fii, float* fij, void* stream);
+int nb200_phis_overlap_pairs(const float* x, const float* sh, const float* coeff, const float* wa, const int32_t* row_ptr,
+                             const int32_t* col, int32_t n_atoms, int32_t n_feat, float* s, void* stream);
+int nb200_phis_assemble(const float* Xd, const float* Xo, const float* Wd, const float* bd, int32_t n_col_d, const float* Wo, const float* bo,
+                        int32_t n_col_o, int32_t n_feat, const int32_t* atom_el, const int32_t* row_orb, const int32_t* row_m,
+                        const int32_t* orb_l, const int32_t* n_rows, const int32_t* ent_range, const int32_t* op_base, const int32_t* ent_col,
+                        const int32_t* ent_L, int32_t n_el, int32_t max_ent, const int32_t* tgt, const int32_t* col, const int32_t* rev,
+                        int32_t n_atoms, int32_t n_pairs, const int32_t* atom_mol, const int32_t* atom_off, const int64_t* mol_off,
+                        const int32_t* mol_norb, int32_t unit_diagonal, float* M, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

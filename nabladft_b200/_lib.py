@@ -90,6 +90,13 @@ SIGNATURES = {
     "nb200_phis_pair_mixing": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "nb200_phis_self_mixing": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "nb200_phis_linear": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
+    "nb200_phis_swish_self_mixing": (c_int32, [c_void_p] * 5 + [c_int32, c_int32, c_void_p, c_void_p]),
+    "nb200_phis_linear_ex": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
+    "nb200_phis_interaction": (c_int32, [c_void_p] * 10 + [c_int32, c_int32, c_void_p, c_void_p]),
+    "nb200_phis_pair_features": (c_int32, [c_void_p] * 5 + [c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    "nb200_phis_overlap_pairs": (c_int32, [c_void_p] * 6 + [c_int32, c_int32, c_void_p, c_void_p]),
+    "nb200_phis_assemble": (c_int32, [c_void_p] * 4 + [c_int32] + [c_void_p] * 2 + [c_int32, c_int32] + [c_void_p] * 9 + [c_int32, c_int32]
+                            + [c_void_p] * 3 + [c_int32, c_int32] + [c_void_p] * 4 + [c_int32, c_void_p, c_void_p]),
     "nb200_gemm_tf32x3": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_int32,
                                     c_int32, c_void_p, c_void_p, c_void_p]),
     "nb200_linear_wgrad": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32, c_float,

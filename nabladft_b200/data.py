@@ -295,6 +295,20 @@ def read_hamiltonian_db(path: str, include_overlap: bool = False) -> Dict[str, n
     return out
 
 
+def read_hamiltonian_max_orbitals(path: str):
+    """`max_orbitals` of a Hamiltonian database as `HamiltonianDataset.__init__` builds it (hamiltonian_dataset.py:331-335): one tuple of
+    (Z, l) per entry of the `nuclear_charges` row, the l values from the `basisset` table.  PhiSNet's output layout is defined by it."""
+    con = sqlite3.connect(f"file:{path}?mode=ro", uri=True)
+    try:
+        if not con.execute("select name from sqlite_master where type='table' and name='nuclear_charges'").fetchone():
+            return None  # older databases without the table: no PhiSNet layout
+        zs = np.frombuffer(con.execute("select Z from nuclear_charges where id=0").fetchone()[0], dtype=np.int32)
+        basis = {int(zz): np.frombuffer(b, dtype=np.int32) for zz, b in con.execute("select Z, orbitals from basisset").fetchall()}
+    finally:
+        con.close()
+    return tuple(tuple((int(zz), int(l)) for l in basis[int(zz)]) for zz in zs)
+
+
 class PackedHamiltonianDataset:
     """Z, R (bohr), H packed + offsets; `batch(indices, device)` returns what `QHNet.forward(data, keep_blocks=True)` and
     `HamiltonianLoss.packed` take: a data object (z, pos, batch, ptr) and the list of per-molecule target matrices on the device."""
@@ -303,8 +317,10 @@ class PackedHamiltonianDataset:
         self.a = arrays
 
     @classmethod
-    def from_db(cls, path: str) -> "PackedHamiltonianDataset":
-        return cls(read_hamiltonian_db(path))
+    def from_db(cls, path: str, include_overlap: bool = False) -> "PackedHamiltonianDataset":
+        ds = cls(read_hamiltonian_db(path, include_overlap=include_overlap))
+        ds.max_orbitals = read_hamiltonian_max_orbitals(path)
+        return ds
 
     def __len__(self) -> int:
         return len(self.a["energy"])
@@ -312,6 +328,26 @@ class PackedHamiltonianDataset:
     def hamiltonian(self, i: int) -> np.ndarray:
         no = int(self.a["norb"][i])
         return self.a["H"][int(self.a["h_off"][i]):int(self.a["h_off"][i + 1])].reshape(no, no)
+
+    def phisnet_batch(self, indices, device="cuda"):
+        """What `nabladft_b200.phisnet.NeuralNetwork.forward` takes, with the semantics of `HamiltonianDataset.collate_fn`
+        (hamiltonian_dataset.py:354-405): `atoms_batch` = {positions [N,3] (bohr), atomic_numbers [N] int64, orbitals (one (Z, l) tuple per
+        atom, from the basisset table), molecule_size [B] int64 (host)} on `device`, plus the packed targets: lists of the per-molecule H
+        and S matrices on `device` instead of the reference's dense block diagonals.  Needs `from_db(path, include_overlap=True)`."""
+        a, idx = self.a, np.asarray(indices, dtype=np.int64)
+        if "S" not in a:
+            raise ValueError("overlap matrices were not read: build the dataset with PackedHamiltonianDataset.from_db(path, include_overlap=True)")
+        ptr, hoff = a["ptr"], a["h_off"]
+        z = np.concatenate([a["z"][ptr[m]:ptr[m + 1]] for m in idx]).astype(np.int64)
+        pos = np.concatenate([a["pos"][ptr[m]:ptr[m + 1]] for m in idx])
+        dev = torch.device(device)
+        orb = {zz: tuple((int(zz), int(l)) for l in ls) for zz, ls in a["basis"].items()}
+        atoms_batch = {"positions": torch.from_numpy(pos).to(dev), "atomic_numbers": torch.from_numpy(z).to(dev),
+                       "orbitals": tuple(orb[int(zz)] for zz in z), "molecule_size": torch.from_numpy(ptr[idx + 1] - ptr[idx])}
+        mats = {}
+        for key in ("H", "S"):
+            mats[key] = [torch.from_numpy(a[key][hoff[m]:hoff[m + 1]].reshape(int(a["norb"][m]), int(a["norb"][m]))).to(dev) for m in idx]
+        return atoms_batch, mats["H"], mats["S"]
 
     def batch(self, indices, device="cuda"):
         a, idx = self.a, np.asarray(indices, dtype=np.int64)
