@@ -8,8 +8,8 @@
 // with no host synchronisation anywhere (edge count and error flags stay on the device).
 //
 // Node-level dense layers ([N,128]x[128,384] etc.) run on the wgmma 3xTF32 GEMM of gemm_tc.cu (fp32-accurate: the reference never
-// uses reduced precision, SURVEY.md section 0.9); cuBLAS SGEMM stays selectable for A/B runs (nb200_engine_set_gemm_backend) and carries
-// the weight-gradient GEMMs of the training step (reduction over the atom rows: a plain library GEMM).
+// uses reduced precision, SURVEY.md section 0.9); cuBLAS SGEMM stays selectable (nb200_engine_set_gemm_backend).  The weight gradients of
+// the training step run on the wgmma split-K kernel of wgrad_tc.cu.
 // `run_painn` is the one orchestration for inference, the energy-seeded parameter gradients (painn_train.cu) and the force-loss tangent
 // pass (painn_tangent.cu).
 #include <new>
@@ -110,8 +110,8 @@ struct Workspace {
     float *q, *act, *ro_pre, *eps;
     // backward
     float *gq, *gmu_a, *gmu_b, *gy, *gVW, *gt, *gn, *g_ro, *egrad;
-    // training only: layer inputs that the in-place forward overwrites, scaled-gradient / activation scratch, per-edge filter gradients
-    float *q_in[kMaxLayers], *q_mid[kMaxLayers], *mu_mid[kMaxLayers], *gs, *act_t, *gW, *seed_atom;
+    // training only: layer inputs that the in-place forward overwrites, activation scratch, per-edge filter gradients
+    float *q_in[kMaxLayers], *q_mid[kMaxLayers], *mu_mid[kMaxLayers], *act_t, *gW, *seed_atom;
     // force-loss tangent pass (painn_tangent.cu): t_X = directional derivative of X along the position-space direction v
     float *t_geom, *t_h1[kMaxLayers], *t_xh[kMaxLayers], *t_VW[kMaxLayers], *t_nrm[kMaxLayers], *t_g1[kMaxLayers], *t_y[kMaxLayers];
     float *t_q_in[kMaxLayers], *t_q_mid[kMaxLayers], *t_mu_mid[kMaxLayers], *t_mu[kMaxLayers + 1];
@@ -163,7 +163,6 @@ Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool for
     }
     if (train) {
         for (int l = 0; l < L; ++l) { w.q_in[l] = c.take<float>(N * F); w.q_mid[l] = c.take<float>(N * F); w.mu_mid[l] = c.take<float>(N * 3 * F); }
-        w.gs = c.take<float>(N * 6 * F);
         w.act_t = c.take<float>(N * F);
         w.gW = c.take<float>(E * 3 * F);
         w.seed_atom = c.take<float>(N);
@@ -218,23 +217,11 @@ extern "C" int64_t nb200_painn_workspace_bytes(const nb200_painn_weights* w, int
 
 namespace {
 
-// dW[out,in] (lddw) (+)= gY[M,out]^T (ldgy) . X[M,in] (ldx): weight gradient of a Linear layer, reduction over the M rows (cuBLAS SGEMM)
-int linear_wgrad(nb200_engine* e, cudaStream_t s, int M, int out, int in, const float* gY, int ldgy, const float* X, int ldx, float* dW, int lddw,
-                 float alpha = 1.0f, float beta = 0.0f) {
-    Scope sc(e, s, CAT_GEMM, 0);
-    return cublasSgemm(e->blas, CUBLAS_OP_N, CUBLAS_OP_T, in, out, M, &alpha, X, ldx, gY, ldgy, &beta, dW, lddw) == CUBLAS_STATUS_SUCCESS ? NB200_OK
-                                                                                                                                      : NB200_ECUDA;
-}
-
-// weight-gradient backend: wgmma split-K (wgrad_tc.cu) unless NB200_WGRAD=cublas
-bool wgrad_tc_on() {
-    static const bool on = [] { const char* e = getenv("NB200_WGRAD"); return !(e && e[0] == 'c'); }();
-    return on;
-}
-
+// The Linear weight gradients are written in 16-byte rows by the wgmma split-K kernel (wgrad_tc.cu): their arrays must be 16-byte aligned.
 bool grads_ok(const nb200_painn_weights* g) {
+    auto al = [](const float* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
     return g && g->emb && g->w_rbf && g->b_rbf && g->A1 && g->c1 && g->A2 && g->c2 && g->U && g->B1 && g->d1 && g->B2 && g->d2 && g->R1 && g->e1 &&
-           g->R2 && g->e2;
+           g->R2 && g->e2 && al(g->A1) && al(g->A2) && al(g->U) && al(g->B1) && al(g->B2) && al(g->R1);
 }
 
 // Inference (E + analytic F) with the fused node kernels of painn_fused.cu: per layer ONE message kernel and ONE node kernel per direction.
@@ -333,11 +320,8 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
     const size_t wl_stride = (size_t)e_cap * 3 * F;
     const int bf16 = train ? eng->edge_bf16 : 0;  // bf16 rows use the first half of their fp32-sized blocks: all offsets below stay in floats
     // training, like inference, stores ONE filter row (W and dW/dd, two arrays here) per undirected pair: edge e reads row min(e, rev[e]).  Half the filter
-    // kernel's work and writes; the second reader of a row mostly finds it in L2.  NB200_TRAIN_HALF_ROWS=0: one row per directed edge (round-2a layout).
-    static const bool half_env = [] { const char* e = getenv("NB200_TRAIN_HALF_ROWS"); return !(e && e[0] == '0'); }();
-    const bool half_train = train && half_env;
-    const int32_t* t_rev = half_train ? ws.rev : nullptr;
-    const int32_t* wg_scr = half_train ? ws.sort_scr2 : ws.sort_scr;
+    // kernel's work and writes; the second reader of a row mostly finds it in L2.
+    const int32_t* t_rev = train ? ws.rev : nullptr;
     if (phase != 2) {
     // ---- graph + radial filters (painn.py:104-108 / spk PairwiseDistances + filter_net)
     { Scope sc(eng, s, CAT_NBR, 3);
@@ -348,14 +332,14 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
     const bool half_rows = eng->node_backend == 1 && !train;
     { Scope sc(eng, s, CAT_FILTER, 4);
     NB_TRY(nb_painn_filter_ex(ws.geom, status, e_cap, w->w_rbf, w->b_rbf, L, K, F, w->radial_mode, w->cutoff, w->rbf_offsets, w->rbf_coeff,
-                              w->rbf_xscale, ws.W, ws.dW, ws.sort_scr, (half_rows || half_train) ? ws.rev : nullptr, half_rows && want_f ? 1 : 0, s, bf16)); }
-    if (half_train) {  // the filter weight gradients still walk every directed edge (slot e holds the gradient of the opposite edge's row): their own sort
+                              w->rbf_xscale, ws.W, ws.dW, ws.sort_scr, (half_rows || train) ? ws.rev : nullptr, half_rows && want_f ? 1 : 0, s, bf16)); }
+    if (train) {  // the filter weight gradients still walk every directed edge (slot e holds the gradient of the opposite edge's row): their own sort
         const float dx = (w->cutoff * w->rbf_xscale) / (float)(K - 1);
         Scope sc(eng, s, CAT_FILTER, 3);
         NB_TRY(nb_bin_sort(ws.geom, status, w->rbf_xscale, 1.0f / dx, K, ws.sort_scr2, s, nullptr));
     }
     if (eng->node_backend == 1 && !train) return run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s);
-    if (phase == 1) return run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s, false, bf16, half_train);
+    if (phase == 1) return run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s, false, bf16, true);
     // ---- embedding (painn.py:110-111)
     { Scope sc(eng, s, CAT_EMBED, 1); NB_TRY(nb_embed(z, w->emb, w->z_offset, w->n_elem, N, ws.q, ws.mu[0], status, s)); }
 
@@ -429,14 +413,12 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
     { Scope sc(eng, s, CAT_READOUT, 1); NB_TRY(nb_readout_bwd(ws.ro_pre, w->R2, N, F / 2, ws.g_ro, s)); }
     NB_TRY(linear_bwd(eng, s, N, F / 2, F, ws.g_ro, F / 2, w->R1, F, ws.gq, F, false));
     // energy-seed weight gradients: dW += (c o g)^T x and dbias += colsum(c o g), c = the per-atom seed (`rs_div` rows of g per atom: 3 for the
-    // (atom, xyz) rows of U).  One wgmma split-K launch (wgrad_tc.cu: the row scale is applied while loading g); NB200_WGRAD=cublas keeps the
-    // round-1 sequence (scale kernel + cuBLAS SGEMM + column-sum kernel).
+    // (atom, xyz) rows of U).  One wgmma split-K launch (wgrad_tc.cu: the row scale is applied while loading g).
     // Weight-gradient launches are LEAVES of the step: they read buffers of the backward chain and only add into `grads`.  They run on a
     // second stream of the engine, next to the chain (whose 76-CTA GEMMs and latency-bound phases leave SMs idle): fork = the side stream
     // waits for the chain's current point, and the chain waits for a leaf only right before it overwrites that leaf's inputs (`need`).  The
-    // side stream is in order, so one event per input group is enough.  NB200_TRAIN_SIDE=0 keeps everything on the caller's stream.
-    static const bool side_env = [] { const char* e = getenv("NB200_TRAIN_SIDE"); return !(e && e[0] == '0'); }();
-    bool use_side = train && phase != 1 && side_env && wgrad_tc_on();
+    // side stream is in order, so one event per input group is enough.
+    bool use_side = train && phase != 1;
     if (use_side && !eng->side && cudaStreamCreateWithFlags(&eng->side, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); use_side = false; }
     const cudaStream_t ls = use_side ? eng->side : s;
     size_t ev_next = 0;
@@ -469,22 +451,15 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
             if (cudaEventCreateWithFlags(&e, cudaEventDisableTiming) == cudaSuccess) { cudaEventRecord(e, eng->side); cudaStreamWaitEvent(s, e, 0); cudaEventDestroy(e); }
         }
     } join{eng, s, use_side};
-    // with a force seed the energy-seed term rides in the tangent call of the same Linear (one 3-term launch, wgrad_tc.cu::nb_wgrad_tc3)
-    const bool tan_for_merge = train && v_dir != nullptr;
-    auto merged = [&](int M, int out, int in, const float* g, int ldg, const float* x, int ldx, const float* dW, int lddw) {
-        return tan_for_merge && wgrad_tc_on() && nb_wgrad_tc_ok(M, out, in, g, ldg, x, ldx, dW, lddw);
-    };
+    // Every PaiNN shape fits the kernel (n_feat == NB_F; workspace and gradient arrays 16-byte aligned, see grads_ok).
+    // With a force seed the energy-seed term rides in the tangent call of the same Linear (one 3-term launch, wgrad_tc.cu::nb_wgrad_tc3).
     auto wg_primal = [&](int M, int out, int in, const float* g, int ldg, const float* x, int ldx, float* dW, int lddw, float* dbias, int rs_div) -> int {
-        if (merged(M, out, in, g, ldg, x, ldx, dW, lddw)) return NB200_OK;
-        if (wgrad_tc_on() && nb_wgrad_tc_ok(M, out, in, g, ldg, x, ldx, dW, lddw)) {
-            fork();
-            const int rc = nb_wgrad_tc(M, out, in, g, x, nullptr, nullptr, ldg, ldx, dW, lddw, 1.0f, dbias, 1.0f, 0, ws.seed_atom, rs_div, ls);
-            leaf_done();
-            return rc;
-        }
-        NB_TRY(nb_scale_rows(g, ws.seed_atom, rs_div, M, out, ws.gs, s));
-        NB_TRY(linear_wgrad(eng, s, M, out, in, ws.gs, ldg, x, ldx, dW, lddw, 1.0f, 1.0f));
-        return dbias ? nb_colsum(ws.gs, M, out, dbias, s, 1.0f, 1) : NB200_OK;
+        if (tan) return NB200_OK;
+        if (!nb_wgrad_tc_ok(M, out, in, g, ldg, x, ldx, dW, lddw)) return NB200_EUNSUPPORTED;
+        fork();
+        const int rc = nb_wgrad_tc(M, out, in, g, x, nullptr, nullptr, ldg, ldx, dW, lddw, 1.0f, dbias, 1.0f, 0, ws.seed_atom, rs_div, ls);
+        leaf_done();
+        return rc;
     };
     if (train) {
         Scope sc(eng, s, CAT_NODE, 8);
@@ -503,23 +478,14 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         NB_TRY(wg_primal(N, F / 2, F, ws.g_ro, F / 2, ws.q, F, const_cast<float*>(grads->R1), F, const_cast<float*>(grads->e1), 1));
     }
     // tangent weight gradients enter with sign -1:  d/dtheta sum_i v_i.F_i = -(v.d/dR) dE_tot/dtheta   (seed 1, not the energy seed)
+    // One launch: (c o g)^T x - tg^T x - g^T tx and the bias sums.
     auto wgrad_tan = [&](int M, int out, int in, const float* g, const float* tg, int ldg, const float* x, const float* tx, int ldx, float* dW,
                          int lddw, float* dbias = nullptr, int rs_div = 1) -> int {
-        if (merged(M, out, in, g, ldg, x, ldx, dW, lddw)) {  // (c o g)^T x - tg^T x - g^T tx and the bias sums, one launch
-            fork();
-            const int rc = nb_wgrad_tc3(M, out, in, g, tg, ldg, x, tx, ldx, dW, lddw, dbias, ws.seed_atom, rs_div, ls);
-            leaf_done();
-            return rc;
-        }
-        if (wgrad_tc_on() && nb_wgrad_tc_ok(M, out, in, tg, ldg, x, ldx, dW, lddw) && nb_wgrad_tc_ok(M, out, in, g, ldg, tx, ldx, dW, lddw)) {
-            fork();
-            const int rc = nb_wgrad_tc(M, out, in, tg, x, g, tx, ldg, ldx, dW, lddw, -1.0f, dbias, -1.0f, 0, nullptr, 1, ls);  // one launch: tg^T x + g^T tx, colsum(tg)
-            leaf_done();
-            return rc;
-        }
-        NB_TRY(linear_wgrad(eng, s, M, out, in, tg, ldg, x, ldx, dW, lddw, -1.0f, 1.0f));
-        NB_TRY(linear_wgrad(eng, s, M, out, in, g, ldg, tx, ldx, dW, lddw, -1.0f, 1.0f));
-        return dbias ? nb_colsum(tg, M, out, dbias, s, -1.0f, 1) : NB200_OK;
+        if (!nb_wgrad_tc_ok(M, out, in, g, ldg, x, ldx, dW, lddw)) return NB200_EUNSUPPORTED;
+        fork();
+        const int rc = nb_wgrad_tc3(M, out, in, g, tg, ldg, x, tx, ldx, dW, lddw, dbias, ws.seed_atom, rs_div, ls);
+        leaf_done();
+        return rc;
     };
     if (tan) {
         Scope sc(eng, s, CAT_NODE, 4);
@@ -606,7 +572,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
             NB_TRY(nb_msg_bwd_tan(ws.xh[l], ws.t_xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.t_mu[l], ws.W + l * wl_stride, ws.dW + l * wl_stride,
                                   ws.geom, ws.t_geom, ws.row_ptr, ws.col, N, ws.gq, ws.t_gq, cur, t_cur, ws.t_gy, t_other, ws.t_gW, ws.gWd, s, bf16, t_rev));
             tag = &d_F; fork();
-            NB_TRY(nb_filter_wgrad_tan(ws.geom, ws.t_geom, status, wg_scr, w->rbf_offsets, K, w->radial_mode, w->cutoff, w->rbf_coeff, w->rbf_xscale,
+            NB_TRY(nb_filter_wgrad_tan(ws.geom, ws.t_geom, status, ws.sort_scr2, w->rbf_offsets, K, w->radial_mode, w->cutoff, w->rbf_coeff, w->rbf_xscale,
                                        ws.t_gW, ws.gWd, -1.0f, const_cast<float*>(grads->w_rbf) + (size_t)l * K * 3 * F,
                                        const_cast<float*>(grads->b_rbf) + (size_t)l * 3 * F, ls, e_cap, bf16));
             leaf_done();
@@ -616,7 +582,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         if (train) {  // filter weights of this layer, then dA2, dc2
             Scope sc(eng, s, CAT_NODE, 4);
             tag = &d_F; fork();
-            NB_TRY(nb_filter_wgrad(ws.geom, status, wg_scr, w->rbf_offsets, K, w->radial_mode, w->cutoff, w->rbf_coeff, w->rbf_xscale, ws.gW,
+            NB_TRY(nb_filter_wgrad(ws.geom, status, ws.sort_scr2, w->rbf_offsets, K, w->radial_mode, w->cutoff, w->rbf_coeff, w->rbf_xscale, ws.gW,
                                    const_cast<float*>(grads->w_rbf) + (size_t)l * K * 3 * F, const_cast<float*>(grads->b_rbf) + (size_t)l * 3 * F, ls, e_cap, bf16));
             leaf_done();
             tag = &d_A2;

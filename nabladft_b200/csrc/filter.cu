@@ -17,14 +17,11 @@
 // FMA-bound (256 FFMA per edge-thread = 192 SM-cycles per edge and layer).
 //
 // Algorithmic HBM bytes: E*16 (geom) read + L*E*3F*4*(1 or 2) written  (cfg 2: 1.97 GB / 3.9 GB).
-#include <cstdlib>
-
 #include "common.cuh"
 
 #define FLT_THREADS 96   // 3F/4 float4 channel groups for F = 128
 #define FLT_CHUNK 32     // edges staged per phase
 #define FLT_SPLIT 32     // CTAs per (bin, layer)
-#define FLT_WSPLIT 48    // CTAs per bin in the weight-gradient kernels (one layer per launch; partial sums end in atomics)
 #define SORT_THREADS 256
 #define SORT_ITEMS 4
 
@@ -213,148 +210,17 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter(const float* __restrict_
     }
 }
 
-// Training: gradient of the filter weights of ONE layer from the per-edge filter gradients gW[e][3F] (written by the message backward),
-// over the same bin-sorted edge order: d w[k][c] += s1(d_e) phi_k(d_e) gW[e][c] for the 16 centres of the bin's band, d b[c] += s2(d_e) gW[e][c].
-__global__ void __launch_bounds__(FLT_THREADS) k_filter_wgrad(const float* __restrict__ geom, const int32_t* __restrict__ status,
-                                                             const int32_t* __restrict__ scr, const float* __restrict__ offsets, int n_rbf,
-                                                             int radial_mode, float cutoff, float coeff, float xscale,
-                                                             const float* __restrict__ gW, float* __restrict__ g_w, float* __restrict__ g_b) {
-    __shared__ __align__(16) float sphi[FLT_CHUNK][NB_BAND + 4];
-    __shared__ int32_t sedge[FLT_CHUNK];
-    if (status[1] != 0) return;
-    const int bin = blockIdx.x, split = blockIdx.y;
-    const int b0 = scr[SCR_START + bin], b1 = scr[SCR_START + bin + 1];
-    const int cnt = b1 - b0;
-    if (cnt == 0) return;
-    const int per = (cnt + FLT_WSPLIT - 1) / FLT_WSPLIT;
-    const int lo = b0 + split * per, hi = min(lo + per, b1);
-    if (lo >= hi) return;
-    const int k0 = min(max(bin - (NB_BAND / 2 - 1), 0), n_rbf - NB_BAND);
-    const int c4 = threadIdx.x * 4;
-    const int nf3 = 3 * NB_F;
-    float4 acc[NB_BAND];
-#pragma unroll
-    for (int kk = 0; kk < NB_BAND; ++kk) acc[kk] = f4(0.f);
-    float4 accb = f4(0.f);
-    for (int base = lo; base < hi; base += FLT_CHUNK) {
-        const int nchunk = min(FLT_CHUNK, hi - base);
-        if (threadIdx.x < nchunk) {
-            const int e = scr[SCR_PERM + base + threadIdx.x];
-            const float d = geom[4 * (size_t)e + 3];
-            const EdgeRad r = radial_scalars(d, radial_mode, cutoff);
-            const float x = d * xscale;
-            float* row = sphi[threadIdx.x];
-#pragma unroll
-            for (int kk = 0; kk < NB_BAND; ++kk) {
-                const float t = x - __ldg(offsets + k0 + kk);
-                row[kk] = r.s1 * expf(coeff * (t * t));
-            }
-            row[NB_BAND] = r.s2;
-            sedge[threadIdx.x] = e;
-        }
-        __syncthreads();
-        // 8 gradient rows in flight per thread (r1 loaded one row per iteration: one L2 / HBM round trip per edge, 19 % of the HBM rate)
-        for (int t0 = 0; t0 < nchunk; t0 += 8) {
-            float4 g[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) g[u] = (t0 + u < nchunk) ? ldg4_stream(gW + (size_t)sedge[t0 + u] * nf3 + c4) : f4(0.f);
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                if (t0 + u < nchunk) {
-                    const float* row = sphi[t0 + u];
-#pragma unroll
-                    for (int kk = 0; kk < NB_BAND; ++kk) fma4s(acc[kk], g[u], row[kk]);
-                    fma4s(accb, g[u], row[NB_BAND]);
-                }
-            }
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int kk = 0; kk < NB_BAND; ++kk) {
-        float* dst = g_w + (size_t)(k0 + kk) * nf3 + c4;
-        atomicAdd(dst, acc[kk].x); atomicAdd(dst + 1, acc[kk].y); atomicAdd(dst + 2, acc[kk].z); atomicAdd(dst + 3, acc[kk].w);
-    }
-    atomicAdd(g_b + c4, accb.x); atomicAdd(g_b + c4 + 1, accb.y); atomicAdd(g_b + c4 + 2, accb.z); atomicAdd(g_b + c4 + 3, accb.w);
-}
-
-// Tangent of k_filter_wgrad along a position-space direction (painn_tangent.cu): with dd_e the tangent of the edge length,
-//   d w^[k][c] = sum_e  gW^[e][c] s1 phi_k  +  (gW[e][c] dd_e) (s1' phi_k + s1 phi_k'),      d b^[c] = sum_e gW^ s2 + (gW dd) s2'
-// t_gW = gW^ and gWd = gW dd are written by k_msg_bwd_tan.  `sign` (-1 for the force-loss term) scales what is added to g_w / g_b.
-__global__ void __launch_bounds__(FLT_THREADS) k_filter_wgrad_tan(const float* __restrict__ geom, const int32_t* __restrict__ status,
-                                                                 const int32_t* __restrict__ scr, const float* __restrict__ offsets, int n_rbf,
-                                                                 int radial_mode, float cutoff, float coeff, float xscale,
-                                                                 const float* __restrict__ t_gW, const float* __restrict__ gWd, float sign,
-                                                                 float* __restrict__ g_w, float* __restrict__ g_b) {
-    __shared__ __align__(16) float sphi[FLT_CHUNK][2 * NB_BAND + 4];
-    __shared__ int32_t sedge[FLT_CHUNK];
-    if (status[1] != 0) return;
-    const int bin = blockIdx.x, split = blockIdx.y;
-    const int b0 = scr[SCR_START + bin], b1 = scr[SCR_START + bin + 1];
-    const int cnt = b1 - b0;
-    if (cnt == 0) return;
-    const int per = (cnt + FLT_WSPLIT - 1) / FLT_WSPLIT;
-    const int lo = b0 + split * per, hi = min(lo + per, b1);
-    if (lo >= hi) return;
-    const int k0 = min(max(bin - (NB_BAND / 2 - 1), 0), n_rbf - NB_BAND);
-    const int c4 = threadIdx.x * 4;
-    const int nf3 = 3 * NB_F;
-    float4 acc[NB_BAND];
-#pragma unroll
-    for (int kk = 0; kk < NB_BAND; ++kk) acc[kk] = f4(0.f);
-    float4 accb = f4(0.f);
-    for (int base = lo; base < hi; base += FLT_CHUNK) {
-        const int nchunk = min(FLT_CHUNK, hi - base);
-        if (threadIdx.x < nchunk) {
-            const int e = scr[SCR_PERM + base + threadIdx.x];
-            const float d = geom[4 * (size_t)e + 3];
-            const EdgeRad r = radial_scalars(d, radial_mode, cutoff);
-            const float x = d * xscale;
-            float* row = sphi[threadIdx.x];
-#pragma unroll
-            for (int kk = 0; kk < NB_BAND; ++kk) {
-                const float t = x - __ldg(offsets + k0 + kk);
-                const float p = expf(coeff * (t * t));
-                row[kk] = r.s1 * p;                                                    // s1 phi_k
-                row[NB_BAND + kk] = r.ds1 * p + r.s1 * p * (2.0f * coeff * xscale) * t;  // d/dd (s1 phi_k)
-            }
-            row[2 * NB_BAND] = r.s2; row[2 * NB_BAND + 1] = r.ds2;
-            sedge[threadIdx.x] = e;
-        }
-        __syncthreads();
-        for (int t0 = 0; t0 < nchunk; t0 += 4) {  // 2 x 4 gradient rows in flight per thread
-            float4 gh[4], gd[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const size_t off = (size_t)sedge[min(t0 + u, nchunk - 1)] * nf3 + c4;
-                gh[u] = ldg4_stream(t_gW + off); gd[u] = ldg4_stream(gWd + off);
-            }
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                if (t0 + u < nchunk) {
-                    const float* row = sphi[t0 + u];
-#pragma unroll
-                    for (int kk = 0; kk < NB_BAND; ++kk) { fma4s(acc[kk], gh[u], row[kk]); fma4s(acc[kk], gd[u], row[NB_BAND + kk]); }
-                    fma4s(accb, gh[u], row[2 * NB_BAND]); fma4s(accb, gd[u], row[2 * NB_BAND + 1]);
-                }
-            }
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int kk = 0; kk < NB_BAND; ++kk) {
-        float* dst = g_w + (size_t)(k0 + kk) * nf3 + c4;
-        atomicAdd(dst, sign * acc[kk].x); atomicAdd(dst + 1, sign * acc[kk].y); atomicAdd(dst + 2, sign * acc[kk].z); atomicAdd(dst + 3, sign * acc[kk].w);
-    }
-    atomicAdd(g_b + c4, sign * accb.x); atomicAdd(g_b + c4 + 1, sign * accb.y); atomicAdd(g_b + c4 + 2, sign * accb.z); atomicAdd(g_b + c4 + 3, sign * accb.w);
-}
-
-
-// r2: edge-balanced version of the two weight-gradient kernels above.  The (bin, 48 splits) grid ended every one of its 4800 three-warp CTAs
-// in 68 x 96 float atomics -- 31 M atomics per launch, which (not the gradient rows) set the time per layer.  Here a CTA owns
-// ~FW_TARGET consecutive edges of ONE bin in the sorted order (bins get CTAs in proportion to their edge count: no idle CTAs for the
-// empty short-distance bins, no long tail for the crowded ones), its FW_GROUPS warp groups stream disjoint quarters of them with FW_ROWS
-// gradient rows in flight per thread, the groups' band sums are combined through shared memory and flushed ONCE: ~12 x fewer atomics.
+// Training: gradient of the filter weights of ONE layer from the per-edge filter gradients, over the same bin-sorted edge order as k_filter.
+//   TAN = false: gA = gW[e][3F] (written by the message backward); for the 16 centres of the bin's band
+//     d w[k][c] += s1(d_e) phi_k(d_e) gW[e][c],   d b[c] += s2(d_e) gW[e][c]
+//   TAN = true: tangent along a position-space direction (painn_tangent.cu), with dd_e the tangent of the edge length; gA = gW^ and
+//   gB = gW dd are written by k_msg_bwd_tan:
+//     d w^[k][c] = sum_e gW^[e][c] s1 phi_k + (gW[e][c] dd_e) (s1' phi_k + s1 phi_k'),   d b^[c] = sum_e gW^ s2 + (gW dd) s2'
+//   `sign` (-1 for the force-loss term) scales what is added to g_w / g_b.
+// Edge-balanced, because the band-sum atomics (not the gradient rows) set the time per layer when every CTA of a fixed (bin, split) grid
+// flushes its own sums: a CTA owns ~FW_TARGET consecutive edges of ONE bin in the sorted order (bins get CTAs in proportion to their edge
+// count: no idle CTAs for the empty short-distance bins, no long tail for the crowded ones), its FW_GROUPS warp groups stream disjoint
+// quarters of them with D gradient rows in flight per thread, the groups' band sums are combined through shared memory and flushed ONCE.
 #define FW_GROUPS 4
 #define FW_TARGET 768
 #define FW_RING_BYTES 98304
@@ -489,42 +355,26 @@ static int fw_launch(const float* geom, const int32_t* status, const int32_t* sc
     return nb_check_launch();
 }
 
-static bool fw_balanced() {
-    static const bool on = [] { const char* e = getenv("NB200_FWGRAD"); return !(e && e[0] == 'o'); }();  // NB200_FWGRAD=old: the (bin, 48 splits) kernels
-    return on;
-}
-
 int nb_filter_wgrad_tan(const float* geom, const float* t_geom, const int32_t* status, const int32_t* sort_scratch, const float* rbf_offsets, int n_rbf,
                         int radial_mode, float cutoff, float rbf_coeff, float rbf_xscale, const float* t_gW, const float* gWd, float sign, float* g_w,
                         float* g_b, cudaStream_t s, int e_cap, int bf16) {
     (void)t_geom;  // dd_e is already folded into gWd by the message-backward tangent kernel
-    if ((fw_balanced() || bf16) && e_cap > 0) {
-        if (bf16)
-            return fw_launch<true, nb_bf16>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale,
-                                            reinterpret_cast<const nb_bf16*>(t_gW), reinterpret_cast<const nb_bf16*>(gWd), sign, g_w, g_b, e_cap, s);
-        return fw_launch<true, float>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale, t_gW, gWd, sign, g_w, g_b, e_cap, s);
-    }
-    if (bf16) return NB200_EUNSUPPORTED;
-    dim3 grid(n_rbf, FLT_WSPLIT, 1);
-    k_filter_wgrad_tan<<<grid, FLT_THREADS, 0, s>>>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale, t_gW, gWd,
-                                                   sign, g_w, g_b);
-    return nb_check_launch();
+    if (e_cap <= 0) return NB200_OK;
+    if (bf16)
+        return fw_launch<true, nb_bf16>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale,
+                                        reinterpret_cast<const nb_bf16*>(t_gW), reinterpret_cast<const nb_bf16*>(gWd), sign, g_w, g_b, e_cap, s);
+    return fw_launch<true, float>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale, t_gW, gWd, sign, g_w, g_b, e_cap, s);
 }
 
 // g_w [K][3F] and g_b [3F] of this layer must be zeroed by the caller; `sort_scratch` is the one the forward filter call left behind
 int nb_filter_wgrad(const float* geom, const int32_t* status, const int32_t* sort_scratch, const float* rbf_offsets, int n_rbf, int radial_mode,
                     float cutoff, float rbf_coeff, float rbf_xscale, const float* gW, float* g_w, float* g_b, cudaStream_t s, int e_cap, int bf16) {
-    if ((fw_balanced() || bf16) && e_cap > 0) {
-        if (bf16)
-            return fw_launch<false, nb_bf16>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale,
-                                             reinterpret_cast<const nb_bf16*>(gW), nullptr, 1.0f, g_w, g_b, e_cap, s);
-        return fw_launch<false, float>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale, gW,
-                                       static_cast<const float*>(nullptr), 1.0f, g_w, g_b, e_cap, s);
-    }
-    if (bf16) return NB200_EUNSUPPORTED;
-    dim3 grid(n_rbf, FLT_WSPLIT, 1);
-    k_filter_wgrad<<<grid, FLT_THREADS, 0, s>>>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale, gW, g_w, g_b);
-    return nb_check_launch();
+    if (e_cap <= 0) return NB200_OK;
+    if (bf16)
+        return fw_launch<false, nb_bf16>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale,
+                                         reinterpret_cast<const nb_bf16*>(gW), nullptr, 1.0f, g_w, g_b, e_cap, s);
+    return fw_launch<false, float>(geom, status, sort_scratch, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff, rbf_xscale, gW,
+                                   static_cast<const float*>(nullptr), 1.0f, g_w, g_b, e_cap, s);
 }
 
 // counting sort of the edges by distance bin: scratch = [cursor | bin_start | perm] (common.cuh SCR_*)
@@ -552,8 +402,7 @@ int nb_painn_filter_ex(const float* geom, const int32_t* status, int32_t e_strid
     const float dx = (cutoff * rbf_xscale) / (float)(n_rbf - 1);
     if (!(rbf_coeff < 0.f) || rbf_coeff * (7.0f * dx) * (7.0f * dx) > -23.0f) return NB200_EUNSUPPORTED;
     if (int rc = nb_bin_sort(geom, status, rbf_xscale, 1.0f / dx, n_rbf, sort_scratch, s, rev)) return rc;
-    static const int split = [] { const char* e = getenv("NB200_FLT_SPLIT"); return e ? atoi(e) : FLT_SPLIT; }();  // CTAs per (bin, layer)
-    dim3 grid(n_rbf, split, n_layers);
+    dim3 grid(n_rbf, FLT_SPLIT, n_layers);
     const int row_stride = interleave ? 6 * NB_F : 3 * NB_F;
     const size_t layer_stride = (size_t)e_stride * row_stride;
     if (bf16)

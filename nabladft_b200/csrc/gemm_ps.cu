@@ -163,8 +163,7 @@ static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const floa
     if (M == 0) return NB200_OK;
     const int n_nt = (N + 127) / 128, KC = (K + 127) / 128;
 #ifndef NB_GEMM_PS_2G
-    static const bool two_groups = [] { const char* e = getenv("NB200_GEMM_2G"); return !(e && e[0] == '0'); }();  // NB200_GEMM_2G=0: one worker group everywhere
-    if (KC > 1 && two_groups) return nb_gemm_ps_impl_2g(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, ws, ws_bytes, s, epi, epi_alpha);
+    if (KC > 1) return nb_gemm_ps_impl_2g(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, ws, ws_bytes, s, epi, epi_alpha);
 #endif
     const size_t need = nb_gemm_ps_ws_bytes(N, K);
     if (!ws) {
@@ -189,8 +188,7 @@ static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const floa
     P.C = C; P.ldc = ldc; P.accumulate = accumulate; P.bias = bias; P.act = act; P.act_kind = act_kind;
     P.spt = KC == 1 ? (K + KSTAGE - 1) / KSTAGE : STAGES_PER_TILE;
     P.epi = epi; P.epi_alpha = epi_alpha;
-    static const int xs_on = [] { const char* e = getenv("NB200_GEMM_XSPLIT"); return (e && e[0] == '0') ? 0 : 1; }();
-    P.xsplit = (KC > 1) ? xs_on : 0;
+    P.xsplit = KC > 1 ? 1 : 0;
     const int m_tiles = (M + NT - 1) / NT;
     int ny = 1;
     while (m_tiles * ny < nb_sm_count() && ny < n_nt) ++ny;  // few row slabs: split the N walk (the activation slab is re-staged per CTA)

@@ -17,8 +17,6 @@
 //   optional second output  act[M,N] = silu(C)   (C then holds the pre-activation)
 // k_gemm_tf32x3: tile 128 x 64 x 32, 512 threads = four warpgroups (each a 64 x 32 quarter of the tile), double-buffered stages with
 // register prefetch.  Tall problems go to the pre-split-weight kernel of gemm_ps.cu.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -209,10 +207,8 @@ int nb_gemm_tf32x3_ex(int M, int N, int K, const float* A, int lda, const float*
     if (!A || !B || !C || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
     if (K % G_BK || N % 4 || lda % 4 || ldb % 4 || ldc % 4) return NB200_EUNSUPPORTED;
     if (M == 0) return NB200_OK;
-    // tall problems: weights pre-split once into shared-memory tile images and streamed (gemm_ps.cu); NB200_GEMM_VARIANT=tile keeps every
-    // shape on the tile kernel below, =ps forces the pre-split kernel
-    static const int variant = [] { const char* e = getenv("NB200_GEMM_VARIANT"); return !e ? 0 : (e[0] == 't') ? 1 : (e[0] == 'p') ? 3 : 0; }();
-    if (variant == 3 || (variant == 0 && nb_gemm_ps_wanted(M, N, K)))
+    // tall problems: weights pre-split once into shared-memory tile images and streamed (gemm_ps.cu)
+    if (nb_gemm_ps_wanted(M, N, K))
         return nb_gemm_ps(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, nullptr, 0, s);
     return launch(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, 0, 1, 0, 0, 0, s);
 }
@@ -224,8 +220,7 @@ int nb_gemm_tf32x3_lm(int M, int N, int K, const float* A, int lda, const float*
     if (K % G_BK || N % 4 || lda % 4 || ldc % 4) return NB200_EUNSUPPORTED;
     if (M == 0) return NB200_OK;
     // tall inputs (per-pair features of QHNet / PhiSNet: 1e5 rows x 25 slices): pre-split weights, one launch over (row slab, slice)
-    static const bool ps_off = [] { const char* e = getenv("NB200_GEMM_VARIANT"); return e && e[0] == 't'; }();
-    if (!ps_off && nb_gemm_ps_lm_wanted(M, N, K)) return nb_gemm_ps_lm(M, N, K, A, lda, W_l, w_l_stride, C, ldc, accumulate, bias, n_lm, s);
+    if (nb_gemm_ps_lm_wanted(M, N, K)) return nb_gemm_ps_lm(M, N, K, A, lda, W_l, w_l_stride, C, ldc, accumulate, bias, n_lm, s);
     return launch(M, N, K, A, lda, W_l, N, 1, C, ldc, accumulate, bias, nullptr, NB_ACT_SILU, 1, n_lm, K, w_l_stride, N, s);
 }
 

@@ -122,8 +122,7 @@ struct Ctx {
         (void)M; (void)N; (void)K; (void)A; (void)C;
         return false;
 #else
-        static const bool off = [] { const char* v = getenv("NB200_GOC_TAILS"); return v && v[0] == 's'; }();  // =separate: A/B runs
-        return !off && A != C && M <= 0x7fffffff && goc_tc_ok(N, K, K, K, N) && nb_gemm_ps_wanted((int)M, N, K);
+        return A != C && M <= 0x7fffffff && goc_tc_ok(N, K, K, K, N) && nb_gemm_ps_wanted((int)M, N, K);
 #endif
     }
     int dense_act(int64_t M, int N, int K, const float* A, int lda, const float* W, float* C) const {
@@ -320,8 +319,6 @@ int trip_edge_aggregate(nb200_engine* eng, cudaStream_t s, const Graph& o, const
 #ifdef NB_EMU
     return pfor(eng, s, CAT_MSG_FWD, E * TI, TripEdgeK{o, in, x, R, ldr, O});
 #else
-    static const bool functor = [] { const char* v = getenv("NB200_GOC_TRIP"); return v && v[0] == 'f'; }();  // =functor: the round-1 kernel (A/B runs)
-    if (functor) return pfor(eng, s, CAT_MSG_FWD, E * TI, TripEdgeK{o, in, x, R, ldr, O});
     if (E <= 0) return NB200_OK;
     Scope sc(eng, s, CAT_MSG_FWD, 1);
     const int64_t want = (E + TW_WARPS - 1) / TW_WARPS;
@@ -334,8 +331,6 @@ int quad_aggregate(nb200_engine* eng, cudaStream_t s, const Graph& mn, const Gra
 #ifdef NB_EMU
     return pfor(eng, s, CAT_MSG_FWD, E * QI, QuadK{mn, q, q_tin, xt, R, ldr, O});
 #else
-    static const bool functor = [] { const char* v = getenv("NB200_GOC_QUAD"); return v && v[0] == 'f'; }();  // =functor: the round-1 kernel (A/B runs)
-    if (functor) return pfor(eng, s, CAT_MSG_FWD, E * QI, QuadK{mn, q, q_tin, xt, R, ldr, O});
     if (E <= 0) return NB200_OK;
     Scope sc(eng, s, CAT_MSG_FWD, 1);
     const int64_t want = (E + QW_WARPS - 1) / QW_WARPS;

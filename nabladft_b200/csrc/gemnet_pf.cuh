@@ -110,9 +110,9 @@ inline int goc_tc_gemm_ex(nb200_engine* e, cudaStream_t s, int M, int N, int K, 
     Scope sc(e, s, CAT_GEMM, 1);
     return nb_gemm_tf32x3_ex(M, N, K, A, lda, W, ldw, trans_w, C, ldc, accumulate, bias, nullptr, NB_ACT_SILU, s);
 }
-// dW[out, in] (lddw) += alpha * gY[M, out]^T (ldgy) . X[M, in] (ldx): weight gradient of a Linear layer as ONE cuBLAS SGEMM (fp32, no TF32), the
-// call pattern of engine.cu::linear_wgrad that the PaiNN training step runs on the device.  false = not available (NB200_GOC_GEMM=simt, no
-// handle): the caller falls back to its row-chunked functor reduction (which is also what host emulation runs).
+// dW[out, in] (lddw) += alpha * gY[M, out]^T (ldgy) . X[M, in] (ldx): weight gradient of a Linear layer as ONE cuBLAS SGEMM (fp32, no TF32).
+// false = not available (NB200_GOC_GEMM=simt, no handle): the caller falls back to its row-chunked functor reduction (which is also what host
+// emulation runs).
 inline bool goc_wgrad(nb200_engine* e, cudaStream_t s, int64_t M, int out, int in, const float* gY, int ldgy, const float* X, int ldx, float* dW, int lddw,
                       float alpha, int* rc) {
     static const bool simt = [] { const char* v = getenv("NB200_GOC_GEMM"); return v && v[0] == 's'; }();

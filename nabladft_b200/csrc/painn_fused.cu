@@ -593,19 +593,13 @@ int nb_fused_prep(const nb200_painn_weights* w, void* wtiles, cudaStream_t s) {
     return nb_check_launch();
 }
 
-// NB200_NF_XSPLIT=1: hand the activation operands over in two K halves (tc_pipe.cuh).  Measured neutral for these kernels (122.4 k vs 122.8 k
-// molecules/s, A/B run: most of their operands are written by the previous GEMM's epilogue, which the hand-over cannot
-// start earlier), so the whole-operand protocol stays the default here; the pre-split-weight GEMM uses it for K > 128.
-static int nf_xsplit() {
-    static const int on = [] { const char* e = getenv("NB200_NF_XSPLIT"); return (e && e[0] == '1') ? 1 : 0; }();
-    return on;
-}
-
 int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s) {
     static bool attr = false;
     if (!attr) { if (set_smem(k_node_fwd) != NB200_OK) return NB200_ECUDA; attr = true; }
     FwdParams P{};
-    P.xsplit = nf_xsplit();
+    // Whole-operand hand-over: the two-K-halves protocol of tc_pipe.cuh (xsplit, used by the pre-split-weight GEMM for K > 128) measured neutral
+    // here (122.4 k vs 122.8 k molecules/s): most operands of these kernels are written by the previous GEMM's epilogue, which it cannot start earlier.
+    P.xsplit = 0;
     P.n_atoms = a.n_atoms; P.do_upd = a.layer_upd >= 0; P.do_mlp = a.layer_mlp >= 0; P.do_ro = a.readout;
     P.wt = static_cast<const unsigned char*>(a.wtiles);
     P.tile_upd = a.layer_upd * TILES_PER_LAYER; P.tile_mlp = a.layer_mlp * TILES_PER_LAYER; P.tile_ro = a.n_layers * TILES_PER_LAYER;
@@ -621,7 +615,7 @@ int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s) {
     static bool attr = false;
     if (!attr) { if (set_smem(k_node_bwd) != NB200_OK) return NB200_ECUDA; attr = true; }
     BwdParams P{};
-    P.xsplit = nf_xsplit();
+    P.xsplit = 0;  // as in nb_fused_node_fwd
     P.n_atoms = a.n_atoms; P.do_mlp = a.layer_mlp >= 0; P.do_ro = a.readout; P.do_upd = a.layer_upd >= 0;
     P.wt = static_cast<const unsigned char*>(a.wtiles);
     P.tile_mlp = a.layer_mlp * TILES_PER_LAYER; P.tile_ro = a.n_layers * TILES_PER_LAYER + 1; P.tile_upd = a.layer_upd * TILES_PER_LAYER;

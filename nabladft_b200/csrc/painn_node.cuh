@@ -18,13 +18,12 @@ int nb_poison_on_error(const int32_t* status, float* energy, int n_mol, float* f
 
 // training helpers (painn_train.cu, filter.cu, painn_msg.cu)
 int nb_seed_atom(const float* seed_mol, const int32_t* mol_ptr, int n_mol, float* seed_atom, cudaStream_t s);
-int nb_scale_rows(const float* g, const float* seed_atom, int rows_per_atom, int64_t n_rows, int width, float* out, cudaStream_t s);
 int nb_act_only(const float* pre, const float* seed_atom, int64_t n_rows, int width, int kind, float* act, cudaStream_t s);
 int nb_colsum(const float* x, int64_t n_rows, int width, float* out, cudaStream_t s, float alpha = 1.0f, int accumulate = 0);
 int nb_emb_grad(const float* gq, const float* seed_atom, const int32_t* z, int z_offset, int n_elem, int n_atoms, float* g_emb, cudaStream_t s,
                 float sign = 1.0f);
 int nb_filter_wgrad(const float* geom, const int32_t* status, const int32_t* sort_scratch, const float* rbf_offsets, int n_rbf, int radial_mode,
-                    float cutoff, float rbf_coeff, float rbf_xscale, const float* gW, float* g_w, float* g_b, cudaStream_t s, int e_cap = 0, int bf16 = 0);
+                    float cutoff, float rbf_coeff, float rbf_xscale, const float* gW, float* g_w, float* g_b, cudaStream_t s, int e_cap, int bf16);
 int nb_painn_msg_bwd_train(const float* xh, const float* xh_bias, const float* mu, const float* W, const float* dW, const float* geom,
                            const int32_t* row_ptr, const int32_t* col, int32_t n_atoms, const float* g_q, const float* g_mu, float* g_xh,
                            float* g_mu_in, float* egrad, float* gW, const float* seed_atom, cudaStream_t stream, int bf16 = 0, const int32_t* rev = nullptr);
@@ -49,7 +48,7 @@ int nb_msg_bwd_tan(const float* xh, const float* t_xh, const float* xh_bias, con
                    cudaStream_t s, int bf16 = 0, const int32_t* rev = nullptr);
 int nb_filter_wgrad_tan(const float* geom, const float* t_geom, const int32_t* status, const int32_t* sort_scratch, const float* rbf_offsets, int n_rbf,
                         int radial_mode, float cutoff, float rbf_coeff, float rbf_xscale, const float* t_gW, const float* gWd, float sign, float* g_w,
-                        float* g_b, cudaStream_t s, int e_cap = 0, int bf16 = 0);
+                        float* g_b, cudaStream_t s, int e_cap, int bf16);
 
 // fused per-layer node kernels (painn_fused.cu): wgmma chain of the update / message-MLP / readout Linear layers with their elementwise glue
 struct NbFusedFwd {

@@ -4,28 +4,17 @@
 // schnetpack AtomisticTask).  The engine's analytic backward (engine.cu) already holds dE/d(activation) for every layer with
 // dE/dE_m = 1; because molecules do not interact, the gradient of sum_m c_m E_m w.r.t. a weight is the same sum over atoms /
 // edges with each term scaled by c of its molecule.  The kernels here form those scaled sums:
-//   k_scale_rows      gs[r,:] = c[atom(r)] * g[r,:]            (operand of the weight-gradient GEMM  dW = gs^T . X, cuBLAS)
 //   k_colsum          bias gradients
 //   k_act_only        act = silu(pre) (the forward keeps pre-activations only)
-//   k_filter_wgrad    d/d w_rbf[l][k][c] = sum_e s1(d_e) phi_k(d_e) gW[e][c],  d/d b_rbf[l][c] = sum_e s2(d_e) gW[e][c]
-//                     over the same distance-bin-sorted edge order as the forward filter kernel (filter.cu): the 16-centre band of a
-//                     bin is accumulated in registers, one atomic add per (band row, channel) per CTA at the end
 //   k_emb_grad        scatter of c_i * dE/dq0_i into the embedding rows
+// The Linear weight gradients (c o g)^T X are wgmma split-K launches with the row scale c applied on load (wgrad_tc.cu); the filter
+// weight gradients run over the distance-bin-sorted edge order of the forward filter kernel (filter.cu, k_filter_wgrad_bal).
 #include "common.cuh"
 #include "painn_node.cuh"
 
 namespace {
 
 constexpr int TR_THREADS = 256;
-
-__global__ void __launch_bounds__(TR_THREADS) k_scale_rows(const float* __restrict__ g, const float* __restrict__ seed_atom, int rows_per_atom,
-                                                          int64_t n4, int width4, float* __restrict__ out) {
-    const int64_t t = (int64_t)blockIdx.x * TR_THREADS + threadIdx.x;
-    if (t >= n4) return;
-    const int64_t row = t / width4;
-    const float c = __ldg(seed_atom + row / rows_per_atom);
-    st4(out + 4 * t, ldg4(g + 4 * t) * c);
-}
 
 __global__ void __launch_bounds__(TR_THREADS) k_act_only(const float* __restrict__ pre, const float* __restrict__ seed_atom, int64_t n4, int width4,
                                                         int kind, float* __restrict__ act) {
@@ -82,11 +71,6 @@ static inline int tr_grid(int64_t n) { return (int)((n + TR_THREADS - 1) / TR_TH
 
 int nb_seed_atom(const float* seed_mol, const int32_t* mol_ptr, int n_mol, float* seed_atom, cudaStream_t s) {
     k_seed_atom<<<n_mol, TR_THREADS, 0, s>>>(seed_mol, mol_ptr, n_mol, seed_atom);
-    return nb_check_launch();
-}
-int nb_scale_rows(const float* g, const float* seed_atom, int rows_per_atom, int64_t n_rows, int width, float* out, cudaStream_t s) {
-    const int64_t n4 = n_rows * width / 4;
-    k_scale_rows<<<tr_grid(n4), TR_THREADS, 0, s>>>(g, seed_atom, rows_per_atom, n4, width / 4, out);
     return nb_check_launch();
 }
 int nb_act_only(const float* pre, const float* seed_atom, int64_t n_rows, int width, int kind, float* act, cudaStream_t s) {

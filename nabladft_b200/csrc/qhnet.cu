@@ -153,64 +153,6 @@ __global__ void __launch_bounds__(QH_C) k_qh_tp_conv(const float* __restrict__ x
     for (int k = 0; k < QH_LM; ++k) ot[k * QH_C] = o[k] + ((add_self && !LAYER0) ? __ldg(x + ((size_t)t * QH_LM + k) * QH_C + u) : 0.f);
 }
 
-// r2b experiment (NOT the default, see nb200_qh_tp_conv): layers >= 1 with the edge's two weight rows (2 x 21 504 B) bulk-copied into a two-stage shared-memory ring, one edge ahead of the
-// arithmetic (thread 0 issues, an mbarrier per stage completes); the x[col e] gather is issued before the wait.  2 CTAs per SM.
-constexpr int QH_TCS_STAGE = 2 * QH_CONV_WEIGHTS;                                  // floats per stage: [w1 row | w2 row]
-constexpr int QH_TCS_BYTES = 2 * QH_TCS_STAGE * (int)sizeof(float) + 16;
-__device__ __forceinline__ void qh_mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n.reg .pred P1;\nLAB_WAIT:\nmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n@P1 bra DONE;\nbra LAB_WAIT;\nDONE:\n}\n" ::"r"(bar), "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void qh_bulk_row(float* dst, const float* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src),
-                 "r"(bytes), "r"(bar)
-                 : "memory");
-}
-__global__ void __launch_bounds__(QH_C) k_qh_tp_conv_s(const float* __restrict__ x, const float* __restrict__ sh, const float* __restrict__ w1,
-                                                      const float* __restrict__ w2, const int32_t* __restrict__ row_ptr,
-                                                      const int32_t* __restrict__ col, int add_self, float* __restrict__ out) {
-    extern __shared__ __align__(128) unsigned char tcs_smem[];
-    float* ring = reinterpret_cast<float*>(tcs_smem);
-    const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(tcs_smem + 2 * QH_TCS_STAGE * sizeof(float));
-    const int t = blockIdx.x, u = threadIdx.x;
-    const int e0 = row_ptr[t], e1 = row_ptr[t + 1];
-    constexpr uint32_t ROW_BYTES = QH_CONV_WEIGHTS * sizeof(float);
-    auto issue = [&](int e, int st) {  // thread 0 only
-        const uint32_t bar = bar0 + 8 * st;
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(2 * ROW_BYTES) : "memory");
-        qh_bulk_row(ring + (size_t)st * QH_TCS_STAGE, w1 + (size_t)e * QH_CONV_WEIGHTS, ROW_BYTES, bar);
-        qh_bulk_row(ring + (size_t)st * QH_TCS_STAGE + QH_CONV_WEIGHTS, w2 + (size_t)e * QH_CONV_WEIGHTS, ROW_BYTES, bar);
-    };
-    if (u == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0) : "memory");
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        if (e0 < e1) issue(e0, 0);
-    }
-    float o[QH_LM];
-#pragma unroll
-    for (int k = 0; k < QH_LM; ++k) o[k] = 0.f;
-    __syncthreads();  // barriers initialised
-    for (int e = e0; e < e1; ++e) {
-        const int st = (e - e0) & 1;
-        if (u == 0 && e + 1 < e1) issue(e + 1, st ^ 1);  // stage st ^ 1 was released by the __syncthreads at the end of the previous iteration
-        const int c = col[e];
-        float a[QH_LM], b[QH_LM];
-#pragma unroll
-        for (int k = 0; k < QH_LM; ++k) b[k] = __ldg(sh + (size_t)e * QH_LM + k);
-#pragma unroll
-        for (int k = 0; k < QH_LM; ++k) a[k] = __ldg(x + ((size_t)c * QH_LM + k) * QH_C + u);
-        qh_mbar_wait(bar0 + 8 * st, (uint32_t)(((e - e0) >> 1) & 1));
-        const float* sw = ring + (size_t)st * QH_TCS_STAGE + u;
-        qh_tp_conv<true>(a, b, sw, sw + QH_CONV_WEIGHTS, QH_C, o);
-        __syncthreads();  // every thread has read stage st
-    }
-    float* ot = out + (size_t)t * QH_LM * QH_C + u;
-#pragma unroll
-    for (int k = 0; k < QH_LM; ++k) ot[k * QH_C] = o[k] + (add_self ? __ldg(x + ((size_t)t * QH_LM + k) * QH_C + u) : 0.f);
-}
-
 // ---- a14: PairNetLayer tensor product (layers.py:481-485): pair p = (src = row owner t, dst = col c)
 //   out[p] = TP_uuu(x[src], x[dst], w1_p * w2_p)
 __global__ void __launch_bounds__(QH_C) k_qh_tp_pair(const float* __restrict__ x, const float* __restrict__ w1, const float* __restrict__ w2,
@@ -227,52 +169,6 @@ __global__ void __launch_bounds__(QH_C) k_qh_tp_pair(const float* __restrict__ x
         o[k] = 0.f;
     }
     qh_tp_uuu2(a, b, w1 + (size_t)p * QH_UUU_WEIGHTS + u, w2 + (size_t)p * QH_UUU_WEIGHTS + u, QH_C, o);
-    float* op = out + (size_t)p * QH_LM * QH_C + u;
-#pragma unroll
-    for (int k = 0; k < QH_LM; ++k) op[k * QH_C] = o[k];
-}
-
-// r2b experiment (NOT the default, see nb200_qh_tp_pair): the same product with the pair's two weight rows (2 x 33 280 B) fetched by TWO bulk copies
-// into shared memory while the threads gather x[src], x[dst]: k_qh_tp_pair streams them with 4-byte loads per thread and path and reached 45 % of the
-// HBM rate; three CTAs per SM keep ~200 KB of rows in flight.
-constexpr int QH_TPS_BYTES = 2 * QH_UUU_WEIGHTS * (int)sizeof(float) + 16;
-__global__ void __launch_bounds__(QH_C) k_qh_tp_pair_s(const float* __restrict__ x, const float* __restrict__ w1, const float* __restrict__ w2,
-                                                      const int32_t* __restrict__ tgt, const int32_t* __restrict__ col,
-                                                      const int32_t* __restrict__ status, float* __restrict__ out) {
-    extern __shared__ __align__(128) unsigned char tps_smem[];
-    float* sw1 = reinterpret_cast<float*>(tps_smem);
-    float* sw2 = sw1 + QH_UUU_WEIGHTS;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(tps_smem + 2 * QH_UUU_WEIGHTS * sizeof(float));
-    const int p = blockIdx.x, u = threadIdx.x;
-    if (status[1] != 0 || p >= status[0]) return;
-    if (u == 0) {
-        const uint32_t b = (uint32_t)__cvta_generic_to_shared(bar);
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(b) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(b), "r"(2u * QH_UUU_WEIGHTS * (uint32_t)sizeof(float)) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"((uint32_t)__cvta_generic_to_shared(sw1)),
-                     "l"(w1 + (size_t)p * QH_UUU_WEIGHTS), "r"((uint32_t)(QH_UUU_WEIGHTS * sizeof(float))), "r"(b)
-                     : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"((uint32_t)__cvta_generic_to_shared(sw2)),
-                     "l"(w2 + (size_t)p * QH_UUU_WEIGHTS), "r"((uint32_t)(QH_UUU_WEIGHTS * sizeof(float))), "r"(b)
-                     : "memory");
-    }
-    const int t = tgt[p], c = col[p];
-    float a[QH_LM], b[QH_LM], o[QH_LM];
-#pragma unroll
-    for (int k = 0; k < QH_LM; ++k) {
-        a[k] = __ldg(x + ((size_t)t * QH_LM + k) * QH_C + u);
-        b[k] = __ldg(x + ((size_t)c * QH_LM + k) * QH_C + u);
-        o[k] = 0.f;
-    }
-    __syncthreads();  // the barrier is initialised
-    {
-        const uint32_t bb = (uint32_t)__cvta_generic_to_shared(bar);
-        asm volatile(
-            "{\n.reg .pred P1;\nLAB_WAIT:\nmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n@P1 bra DONE;\nbra LAB_WAIT;\nDONE:\n}\n" ::"r"(bb), "r"(0u)
-            : "memory");
-    }
-    qh_tp_uuu2<true>(a, b, sw1 + u, sw2 + u, QH_C, o);
     float* op = out + (size_t)p * QH_LM * QH_C + u;
 #pragma unroll
     for (int k = 0; k < QH_LM; ++k) op[k * QH_C] = o[k];
@@ -303,10 +199,7 @@ struct ExpIns { int lin, l1, l2, woff, boff; };
 __constant__ ExpIns c_exp_ins[19];
 __constant__ float c_exp_cg[19 * 5 * 5 * 9];  // [ins][i][j][k], zero padded, already divided by mul_in = 32
 
-// STAGED (r2b experiment, NOT the default, see nb200_qh_expand): the row's 8320 path weights (33 280 B) arrive by ONE bulk copy per warp into shared memory (2 warps per CTA, 2 CTAs per SM, so a
-// CTA's copy overlaps its neighbour's arithmetic) instead of 19 x 32 dependent 100-byte loads per row: the streaming form ran at ~45 % of the
-// HBM rate.
-template <bool STAGED, int WARPS>
+template <int WARPS>
 __global__ void __launch_bounds__(32 * WARPS) k_qh_expand(const float* __restrict__ x, const float* __restrict__ W, const float* __restrict__ Bw,
                                                   int bw_stride, int n_rows, float* __restrict__ blocks) {
     // v1 had lane = input channel w and warp-reduced every (u,v,k): 5 k shuffles per row and 4-byte loads strided by
@@ -315,36 +208,16 @@ __global__ void __launch_bounds__(32 * WARPS) k_qh_expand(const float* __restric
     // read once), x[w][k] is a shared-memory broadcast, no shuffles, and each lane owns its (u,v) sub-block of the tile.
     __shared__ float sblk[WARPS][32 * 32];
     __shared__ float sx[WARPS][QH_LM * QH_B];
-    extern __shared__ __align__(128) unsigned char exp_smem[];  // STAGED: [WARPS][8320] floats, then WARPS mbarriers
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int r = blockIdx.x * WARPS + warp;
     if (r >= n_rows) return;
     float* blk = sblk[warp];
     float* xs = sx[warp];
     const float* Wr = W + (size_t)r * 8320;
-    if (STAGED) {
-        float* sw = reinterpret_cast<float*>(exp_smem) + (size_t)warp * 8320;
-        const uint32_t bar = (uint32_t)__cvta_generic_to_shared(exp_smem + (size_t)WARPS * 8320 * sizeof(float) + 8 * warp);
-        if (lane == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar) : "memory");
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(8320u * 4u) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"((uint32_t)__cvta_generic_to_shared(sw)),
-                         "l"(Wr), "r"(8320u * 4u), "r"(bar)
-                         : "memory");
-        }
-        Wr = sw;
-    }
     for (int t = lane; t < 1024; t += 32) blk[t] = 0.f;
     for (int t = lane; t < QH_LM * QH_B; t += 32) xs[t] = __ldg(x + (size_t)r * QH_LM * QH_B + t);  // [lm][w]
     const float* Br = Bw + (size_t)r * bw_stride;
     __syncwarp();
-    if (STAGED) {
-        const uint32_t bar = (uint32_t)__cvta_generic_to_shared(exp_smem + (size_t)WARPS * 8320 * sizeof(float) + 8 * warp);
-        asm volatile(
-            "{\n.reg .pred P1;\nLAB_WAIT:\nmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n@P1 bra DONE;\nbra LAB_WAIT;\nDONE:\n}\n" ::"r"(bar), "r"(0u)
-            : "memory");
-    }
     for (int ins = 0; ins < 19; ++ins) {
         const ExpIns I = c_exp_ins[ins];
         const int n1 = (I.l1 == 0) ? 5 : (I.l1 == 1) ? 4 : 3, n2 = (I.l2 == 0) ? 5 : (I.l2 == 1) ? 4 : 3;
@@ -358,7 +231,7 @@ __global__ void __launch_bounds__(32 * WARPS) k_qh_expand(const float* __restric
             const float* xk = xs + I.lin * I.lin * QH_B;
 #pragma unroll 4
             for (int w = 0; w < QH_B; ++w) {
-                const float wv = STAGED ? wp[w * nuv] : __ldg(wp + w * nuv);
+                const float wv = __ldg(wp + w * nuv);
 #pragma unroll
                 for (int k = 0; k < 9; ++k)
                     if (k < dk) rk[k] = fmaf(wv, xk[k * QH_B + w], rk[k]);
@@ -479,20 +352,7 @@ extern "C" int nb200_qh_tp_conv(const float* x, const float* sh, const float* w1
     if (!x || !sh || !w1 || !w2 || !row_ptr || !col || !out || n_atoms < 0) return NB200_EINVAL;
     if (n_atoms == 0) return NB200_OK;
     if (layer0) k_qh_tp_conv<true><<<n_atoms, QH_C, 0, (cudaStream_t)stream>>>(x, sh, w1, w2, row_ptr, col, add_self, out);
-    else {
-        // the staged variant was not faster than the streaming kernel on the previous target GPU; the streaming kernel stays the default (not re-measured on H100)
-        static const bool plain = [] { const char* e = getenv("NB200_QH_TP_CONV"); return !(e && e[0] == 's'); }();
-        if (plain || ((reinterpret_cast<uintptr_t>(w1) | reinterpret_cast<uintptr_t>(w2)) & 15)) {
-            k_qh_tp_conv<false><<<n_atoms, QH_C, 0, (cudaStream_t)stream>>>(x, sh, w1, w2, row_ptr, col, add_self, out);
-            return nb_check_launch();
-        }
-        static bool attr = false;
-        if (!attr) {
-            if (cudaFuncSetAttribute(k_qh_tp_conv_s, cudaFuncAttributeMaxDynamicSharedMemorySize, QH_TCS_BYTES) != cudaSuccess) return nb_check_launch();
-            attr = true;
-        }
-        k_qh_tp_conv_s<<<n_atoms, QH_C, QH_TCS_BYTES, (cudaStream_t)stream>>>(x, sh, w1, w2, row_ptr, col, add_self, out);
-    }
+    else k_qh_tp_conv<false><<<n_atoms, QH_C, 0, (cudaStream_t)stream>>>(x, sh, w1, w2, row_ptr, col, add_self, out);
     return nb_check_launch();
 }
 
@@ -500,21 +360,7 @@ extern "C" int nb200_qh_tp_pair(const float* x, const float* w1, const float* w2
                                 int32_t p_cap, float* out, void* stream) {
     if (!x || !w1 || !w2 || !tgt || !col || !status || !out || p_cap < 0) return NB200_EINVAL;
     if (p_cap == 0) return NB200_OK;
-    // The staged kernel's 66.5 KB of shared memory leave 3 CTAs = 12 warps per SM (streaming form: 20), and what the copy engine saves in load latency
-    // the lower occupancy loses on the gathers and the FMA chains of the 2052-term product (no gain on the previous target GPU; not re-measured on H100).
-    // NB200_QH_TP_PAIR=staged selects it.
-    static const bool plain = [] { const char* e = getenv("NB200_QH_TP_PAIR"); return !(e && e[0] == 's'); }();
-    const bool aligned = ((reinterpret_cast<uintptr_t>(w1) | reinterpret_cast<uintptr_t>(w2)) & 15) == 0;   // bulk copies need 16-byte aligned rows
-    if (plain || !aligned) {
-        k_qh_tp_pair<<<p_cap, QH_C, 0, (cudaStream_t)stream>>>(x, w1, w2, tgt, col, status, out);
-        return nb_check_launch();
-    }
-    static bool attr = false;
-    if (!attr) {
-        if (cudaFuncSetAttribute(k_qh_tp_pair_s, cudaFuncAttributeMaxDynamicSharedMemorySize, QH_TPS_BYTES) != cudaSuccess) return nb_check_launch();
-        attr = true;
-    }
-    k_qh_tp_pair_s<<<p_cap, QH_C, QH_TPS_BYTES, (cudaStream_t)stream>>>(x, w1, w2, tgt, col, status, out);
+    k_qh_tp_pair<<<p_cap, QH_C, 0, (cudaStream_t)stream>>>(x, w1, w2, tgt, col, status, out);
     return nb_check_launch();
 }
 
@@ -550,20 +396,7 @@ extern "C" int nb200_qh_expand_setup(const int32_t* ins_host, const float* cg_ho
 extern "C" int nb200_qh_expand(const float* x, const float* W, const float* Bw, int32_t bw_stride, int32_t n_rows, float* blocks, void* stream) {
     if (!x || !W || !Bw || !blocks || n_rows < 0 || bw_stride < 50) return NB200_EINVAL;
     if (n_rows == 0) return NB200_OK;
-    // The staged kernel runs 4 warps per SM instead of 28, and the 19 x 32 serial steps of a row need occupancy more than they need the copy engine
-    // (it was slower on the previous target GPU; not re-measured on H100).  NB200_QH_EXPAND=staged selects it.
-    static const bool plain = [] { const char* e = getenv("NB200_QH_EXPAND"); return !(e && e[0] == 's'); }();
-    if (plain || (reinterpret_cast<uintptr_t>(W) & 15)) {
-        k_qh_expand<false, 4><<<(n_rows + 3) / 4, 128, 0, (cudaStream_t)stream>>>(x, W, Bw, bw_stride, n_rows, blocks);
-        return nb_check_launch();
-    }
-    constexpr int EW = 2, ESMEM = EW * 8320 * (int)sizeof(float) + 8 * EW;
-    static bool attr = false;
-    if (!attr) {
-        if (cudaFuncSetAttribute(k_qh_expand<true, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, ESMEM) != cudaSuccess) return nb_check_launch();
-        attr = true;
-    }
-    k_qh_expand<true, EW><<<(n_rows + EW - 1) / EW, 32 * EW, ESMEM, (cudaStream_t)stream>>>(x, W, Bw, bw_stride, n_rows, blocks);
+    k_qh_expand<4><<<(n_rows + 3) / 4, 128, 0, (cudaStream_t)stream>>>(x, W, Bw, bw_stride, n_rows, blocks);
     return nb_check_launch();
 }
 

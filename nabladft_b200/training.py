@@ -21,11 +21,7 @@ from typing import Dict, List
 
 import torch
 
-import os
-
 from .engine import PainnEngine
-
-_KEEP_FORWARD = os.environ.get("NB200_TRAIN_KEEP", "1") != "0"
 
 
 class PainnEnergyFn(torch.autograd.Function):
@@ -36,11 +32,8 @@ class PainnEnergyFn(torch.autograd.Function):
         wkey = object()
         engine.set_weights(wkey, tensors, scalars)
         # training-mode forward: its activations stay in the engine's workspace for the backward call (no forward recompute); no host sync
-        # after the first (capacity-sizing) batch, status check deferred.  NB200_TRAIN_KEEP=0 keeps the one-call gradient path for A/B runs.
-        if _KEEP_FORWARD:
-            energy, forces, ctx.token = engine.run_train_forward(z, pos, mol_ptr, n_mol)
-        else:
-            (energy, forces), ctx.token = engine.run_async(z, pos, mol_ptr, n_mol), 0
+        # after the first (capacity-sizing) batch, status check deferred.
+        energy, forces, ctx.token = engine.run_train_forward(z, pos, mol_ptr, n_mol)
         ctx.wkey = wkey
         ctx.engine, ctx.names, ctx.n_mol = engine, names, n_mol
         ctx.tensors, ctx.scalars = tensors, scalars
@@ -59,7 +52,7 @@ class PainnEnergyFn(torch.autograd.Function):
         fseed = g_forces.to(torch.float32).contiguous() if g_forces is not None else None
         if eng.kept(ctx.token) and eng._wkey is ctx.wkey:  # the workspace still holds this forward: gradients from the kept activations
             grads = eng.run_train_backward(ctx.token, z, mol_ptr, seed, fseed)
-        else:  # another forward ran on this engine since (or NB200_TRAIN_KEEP=0): one call that recomputes the forward
+        else:  # another forward ran on this engine since: one call that recomputes the forward
             eng._wkey = None
             eng.set_weights(object(), ctx.tensors, ctx.scalars)
             _, _, grads = eng.run_train(z, pos, mol_ptr, ctx.n_mol, seed, fseed)

@@ -298,6 +298,10 @@ def test_two_call_training_c_abi_argument_checks():
     # backward without gradient buffers
     assert lib.nb200_painn_train_backward(h, byref(w), _lib.ptr(zz), _lib.ptr(mp), n_mol, n_atoms, e_cap, _lib.ptr(ws), ws.numel(), 1, _lib.ptr(seed),
                                           None, None, _lib.ptr(st), _lib.current_stream()) == EINVAL
+    # a weight-gradient array that is not 16-byte aligned (the weight-gradient kernel writes 16-byte rows)
+    gw.A1 = grads["A1"].data_ptr() + 4
+    assert lib.nb200_painn_train_backward(h, byref(w), _lib.ptr(zz), _lib.ptr(mp), n_mol, n_atoms, e_cap, _lib.ptr(ws), ws.numel(), wfs, _lib.ptr(seed),
+                                          None, byref(gw), _lib.ptr(st), _lib.current_stream()) == EINVAL
     assert lib.nb200_engine_set_edge_storage(h, 2) == EINVAL
     with pytest.raises(ValueError):
         eng.set_edge_storage("fp8")
