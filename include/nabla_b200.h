@@ -286,9 +286,10 @@ int nb200_schnet_energy_grads(nb200_engine* eng, const nb200_schnet_weights* w, 
  * -------------------------------------------------------------------------------------- */
 int nb200_qh_expand_rows(const int32_t* row_ptr, int32_t n_atoms, int32_t* tgt, void* stream);
 /* a12: ExponentialBernsteinRadialBasisFunctions (layers.py:86-120) + o3.spherical_harmonics l<=4 of
- * sign * edge direction (qhnet.py:264-271).  rbf [E][n_rbf] and/or sh [E][25] may be NULL. */
-int nb200_qh_edge_basis(const float* geom, const int32_t* status, int32_t e_cap, float alpha, float cutoff,
-                        float sign, const float* logc, int32_t n_rbf, float* rbf, float* sh, void* stream);
+ * sign * edge direction (qhnet.py:264-271).  rbf [E][n_rbf] and/or sh [E][25] may be NULL.  alpha and
+ * logc [n_rbf] (log binomial coefficients) are double: the basis exponent is summed in double. */
+int nb200_qh_edge_basis(const float* geom, const int32_t* status, int32_t e_cap, double alpha, float cutoff,
+                        float sign, const double* logc, int32_t n_rbf, float* rbf, float* sh, void* stream);
 /* NormGate pieces (layers.py:123-147): f0 [R][640] = [scalars, norms l=1..4]; y = [gates0, x_l * gates_l] */
 int nb200_qh_norm_feats(const float* x, int32_t n_rows, float* f0, void* stream);
 int nb200_qh_gate(const float* x, const float* gates, int32_t n_rows, float* y, void* stream);

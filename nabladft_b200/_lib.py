@@ -102,7 +102,7 @@ SIGNATURES = {
     "nb200_linear_wgrad": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32, c_float,
                                      c_void_p, c_float, c_void_p, c_int32, c_void_p]),
     "nb200_qh_expand_rows": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
-    "nb200_qh_edge_basis": (c_int32, [c_void_p, c_void_p, c_int32, c_float, c_float, c_float, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
+    "nb200_qh_edge_basis": (c_int32, [c_void_p, c_void_p, c_int32, c_double, c_float, c_float, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
     "nb200_qh_norm_feats": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
     "nb200_qh_gate": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
     "nb200_qh_invariants": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),

@@ -32,20 +32,27 @@ __global__ void k_expand_rows(const int32_t* __restrict__ row_ptr, int n_atoms, 
 // ---- a12: exponential-Bernstein radial basis (layers.py:86-120) + real spherical harmonics l <= 4
 // (qhnet.py:266-271: o3.spherical_harmonics(sh, edge_vec[:, [1,2,0]], normalize=True, 'component') ==
 //  the standard z-polar real SH of edge_vec/|edge_vec| times sqrt(4 pi); oracle/e3.py::spherical_harmonics)
-__global__ void __launch_bounds__(128) k_qh_edge_basis(const float* __restrict__ geom, const int32_t* __restrict__ status, float alpha,
-                                                      float cutoff, float sign, const float* __restrict__ logc, int n_rbf,
+// The exponent logc_k + (K-1-k) x + k log(1 - e^x) sums terms of up to ~85 (logc at K = 128) that cancel to <= 0, so x, the log, logc and
+// the sum are double; only the rounded exponent goes through expf.  In fp32 the basis was off by up to ~1e-5 of each row's largest value.
+// The cutoff function's argument -d^2 / (c^2 - d^2) reaches -100 and beyond near the cutoff, where its fp32 rounding alone puts ~1e-5 on
+// the whole row, so it is evaluated in double once per edge as well.
+__global__ void __launch_bounds__(128) k_qh_edge_basis(const float* __restrict__ geom, const int32_t* __restrict__ status, double alpha,
+                                                      float cutoff, float sign, const double* __restrict__ logc, int n_rbf,
                                                       float* __restrict__ rbf, float* __restrict__ sh) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (status[1] != 0 || e >= status[0]) return;
     const float4 g = ldg4(geom + 4 * (size_t)e);
     const float d = g.w;
     if (rbf) {
-        const float x = -alpha * d;
-        const float lt = logf(-expm1f(x));
+        const double x = -alpha * (double)d;
+        const double lt = log(-expm1(x));
         float fc = 0.f;
-        if (d < cutoff) fc = expf(-(d * d) / ((cutoff - d) * (cutoff + d)));
+        if (d < cutoff) {
+            const double dd = d, c = cutoff;
+            fc = (float)exp(-(dd * dd) / ((c - dd) * (c + dd)));
+        }
         for (int k = 0; k < n_rbf; ++k)
-            rbf[(size_t)e * n_rbf + k] = fc * expf(__ldg(logc + k) + (float)(n_rbf - 1 - k) * x + (float)k * lt);
+            rbf[(size_t)e * n_rbf + k] = fc * expf((float)(__ldg(logc + k) + (double)(n_rbf - 1 - k) * x + (double)k * lt));
     }
     if (sh) {
         const float x = sign * g.x, y = sign * g.y, z = sign * g.z;
@@ -317,8 +324,8 @@ extern "C" int nb200_qh_expand_rows(const int32_t* row_ptr, int32_t n_atoms, int
     return nb_check_launch();
 }
 
-extern "C" int nb200_qh_edge_basis(const float* geom, const int32_t* status, int32_t e_cap, float alpha, float cutoff, float sign,
-                                   const float* logc, int32_t n_rbf, float* rbf, float* sh, void* stream) {
+extern "C" int nb200_qh_edge_basis(const float* geom, const int32_t* status, int32_t e_cap, double alpha, float cutoff, float sign,
+                                   const double* logc, int32_t n_rbf, float* rbf, float* sh, void* stream) {
     if (!geom || !status || e_cap < 0 || (rbf && !logc)) return NB200_EINVAL;
     if (e_cap == 0) return NB200_OK;
     k_qh_edge_basis<<<(e_cap + 127) / 128, 128, 0, (cudaStream_t)stream>>>(geom, status, alpha, cutoff, sign, logc, n_rbf, rbf, sh);

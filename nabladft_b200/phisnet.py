@@ -457,7 +457,7 @@ class NeuralNetwork(nn.Module):
         e = self.embedding.embedding
         w["emb"] = c(e.element_embedding.double() + e.electron_config.double() @ e.config_linear.weight.double().t())
         w["alpha"] = float(torch.nn.functional.softplus(self.radial_basis_functions._alpha.double()))
-        w["logc"] = c(self.radial_basis_functions.logc)
+        w["logc"] = self.radial_basis_functions.logc.detach().to(dev, torch.float64).contiguous()  # the edge basis sums its exponent in double
         w["mods"] = []
         for mb in self.module:
             it = mb.interaction

@@ -255,7 +255,8 @@ class QHNet(nn.Module):
                 b2 = torch.cat([b2, b2.new_zeros(pad_out - b2.shape[0])])
             return c(seq[0].weight), c(seq[0].bias), c(w2), c(b2)
 
-        w = {"emb": c(self.node_embedding.weight), "logc": c(self.distance_expansion.logc)}
+        # the model's float32 logc, widened: the edge basis takes it in double
+        w = {"emb": c(self.node_embedding.weight), "logc": self.distance_expansion.logc.detach().to(dev, torch.float64).contiguous()}
         w["alpha"] = float(torch.nn.functional.softplus(self.distance_expansion._alpha))
         w["conv"] = []
         for i, layer in enumerate(self.e3_gnn_layer):
