@@ -192,6 +192,8 @@ class QHNet(nn.Module):
         self.hs, self.hbs, self.max_radius, self.num_gnn_layers, self.radius_embed_dim = 128, 32, max_radius, num_gnn_layers, 32
         self.order, self.start_layer = sh_lmax, 2
         self.pair_chunk = int(os.environ.get("NB200_QH_PAIR_CHUNK", 16384))  # atom pairs whose path weights [chunk, 8320] exist at a time
+        if self.pair_chunk < 1:
+            raise ValueError(f"NB200_QH_PAIR_CHUNK must be a positive number of atom pairs, got {self.pair_chunk}")
         self.node_embedding = nn.Embedding(num_nodes, self.hs)
         self.distance_expansion = _ExpBernstein(radius_embed_dim, max_radius)
         self.orbital_mask, counts = self._get_mask(orbitals)
@@ -212,7 +214,7 @@ class QHNet(nn.Module):
         self.fc_ij = nn.ModuleDict({"hamiltonian": mk(2 * hs, n_path)})
         self.fc_ij_bias = nn.ModuleDict({"hamiltonian": mk(2 * hs, n_bias)})
         self.output_ii, self.output_ij = _E3Linear(hs, self.hbs), _E3Linear(hs, self.hbs)
-        self._cache_key, self._w, self._tables_dev = None, None, None
+        self._cache_key, self._w, self._tables_dev, self._z_ok = None, None, None, {}
 
     # qhnet.py:323-342
     @staticmethod
@@ -387,10 +389,32 @@ class QHNet(nn.Module):
         with torch.no_grad():
             return self._forward(data, keep_blocks, packed)
 
+    def _unsupported(self, z):
+        """Mask of the atoms whose Z has no embedding row or no orbital-table entry, computed where z lives without a host read.  The
+        kernels index both tables by Z unchecked, and an element without orbitals would silently vanish from H."""
+        ok = self._z_ok.get(str(z.device))
+        if ok is None:  # built once per device: True for every Z with both an embedding row and orbitals
+            ok = torch.zeros(self.node_embedding.num_embeddings, dtype=torch.bool)
+            ok[[k for k in self.orbital_mask if k < ok.numel()]] = True
+            ok = self._z_ok.setdefault(str(z.device), ok.to(z.device))
+        zl = z.reshape(-1).long()
+        return ~(ok[zl.clamp(0, ok.numel() - 1)] & (zl >= 0) & (zl < ok.numel()))
+
+    def _refuse(self, z, bad):
+        raise ValueError(f"atomic numbers {torch.unique(z.reshape(-1)[bad]).tolist()} are not supported: the orbital table has "
+                         f"{sorted(self.orbital_mask)} and the embedding has num_nodes = {self.node_embedding.num_embeddings}")
+
     def _forward(self, data, keep_blocks, packed):
+        if self.pair_chunk < 1:
+            raise ValueError(f"pair_chunk must be a positive number of atom pairs, got {self.pair_chunk}")
         pos = data.pos
         if not pos.is_cuda:
+            z = getattr(data, "z", None)
+            bad = None if z is None else self._unsupported(z)
+            if bad is not None and bool(bad.any()):  # the same refusal as on the device, before the CUDA-only error
+                self._refuse(z, bad)
             raise NablaB200Error("nabladft_b200.qhnet.QHNet runs on CUDA only (no CPU fallback)")
+        bad = self._unsupported(data.z)
         dev = pos.device
         w = self._export(dev)
         o = self._ops(dev)
@@ -403,7 +427,10 @@ class QHNet(nn.Module):
         mol_ptr = data.ptr.to(torch.int32).contiguous()
         n_mol, N = mol_ptr.numel() - 1, z.shape[0]
         n_per = (mol_ptr[1:] - mol_ptr[:-1]).to(torch.int64)
-        P = int((n_per * (n_per - 1)).sum().item())  # ordered pairs: known from the batch structure (one host read)
+        # ordered pairs, known from the batch structure, and the unsupported-element count: one host read, before any kernel launch
+        P, n_bad = torch.stack([(n_per * (n_per - 1)).sum(), bad.sum()]).tolist()
+        if n_bad:
+            self._refuse(z, bad)
         gf = self._graph(o, pos, mol_ptr, n_mol, 10000.0, max(P, 1))
         gc = self._graph(o, pos, mol_ptr, n_mol, self.max_radius, max(P, 1))  # E <= P
         st = gc["status"].cpu()

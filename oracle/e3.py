@@ -314,7 +314,7 @@ class Linear(nn.Module):
             n = self.irreps_out[o].mul
             outs[o] = outs[o] + self.bias[boff:boff + n][None, :, None]
             boff += n
-        return torch.cat([t.reshape(B, -1) for t in outs], dim=-1)
+        return torch.cat([t.reshape(B, mo.dim) for t, mo in zip(outs, self.irreps_out)], dim=-1)  # B may be 0 (no pairs)
 
 
 class Norm(nn.Module):
@@ -340,7 +340,7 @@ class ElementwiseTensorProduct(nn.Module):
         B = x.shape[0]
         out, off = [], 0
         for s, m in zip(self.irreps.slices(), self.irreps):
-            out.append((x[:, s].reshape(B, m.mul, m.ir.dim) * scalars[:, off:off + m.mul, None]).reshape(B, -1))
+            out.append((x[:, s].reshape(B, m.mul, m.ir.dim) * scalars[:, off:off + m.mul, None]).reshape(B, m.dim))
             off += m.mul
         return torch.cat(out, dim=-1)
 

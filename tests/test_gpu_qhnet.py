@@ -68,48 +68,6 @@ def _small(n=14):
     return torch.from_numpy(g["a.z"])[:n], torch.from_numpy(g["a.pos"])[:n], torch.from_numpy(g["a.batch"])[:n]
 
 
-def test_qh_linear_normgate_and_tensor_products(models):
-    from nabladft_b200 import _lib
-    from oracle import e3
-
-    ora, net = models
-    lib = _lib.load()
-    w = net._export(torch.device(DEV))
-    o = net._ops(torch.device(DEV))
-    g = torch.Generator().manual_seed(0)
-    R = 37
-    x64 = torch.randn(R, 3200, generator=g, dtype=torch.float64)
-    x = to_cm(x64.float()).to(DEV)
-    conv = ora.e3_gnn_layer[1].conv
-    # o3.Linear
-    y = o.linear(x, w["conv"][1]["linear_node"])
-    ref = conv.linear_node(x64)
-    assert (from_cm(y.cpu()).double() - ref).abs().max() < 2e-5 * ref.abs().max()
-    # NormGate
-    y = o.norm_gate(x, w["conv"][1]["norm_gate"])
-    ref = conv.norm_gate(x64)
-    assert (from_cm(y.cpu()).double() - ref).abs().max() < 2e-5 * ref.abs().max()
-    # self tensor product (uuu, internal weights) + residual
-    xr64 = torch.randn(R, 3200, generator=g, dtype=torch.float64)
-    sl = ora.e3_gnn_node_layer[0]
-    t = o.E(R, 25, 128)
-    _lib.check(lib.nb200_qh_tp_self(_lib.ptr(x), _lib.ptr(to_cm(xr64.float()).to(DEV)), _lib.ptr(w["self"][0]["tp"]), _lib.ptr(x), R, _lib.ptr(t),
-                                    _lib.current_stream()), "tp_self")
-    ref = sl.tp(x64, xr64) + x64
-    assert (from_cm(t.cpu()).double() - ref).abs().max() < 2e-5 * ref.abs().max()
-    # expansion
-    ex = ora.expand_ii["hamiltonian"]
-    xb64 = torch.randn(R, 800, generator=g, dtype=torch.float64)
-    W64, B64 = torch.randn(R, 8320, generator=g, dtype=torch.float64), torch.randn(R, 50, generator=g, dtype=torch.float64)
-    net(_Data(*[t_.to(DEV) for t_ in _small(4)]))  # uploads the expansion tables
-    blk = o.E(R, 32, 32)
-    Bpad = torch.cat([B64.float(), torch.zeros(R, 2)], dim=1).contiguous().to(DEV)
-    _lib.check(lib.nb200_qh_expand(_lib.ptr(to_cm(xb64.float(), 32).to(DEV)), _lib.ptr(W64.float().contiguous().to(DEV)), _lib.ptr(Bpad), 52, R, _lib.ptr(blk),
-                                   _lib.current_stream()), "expand")
-    ref = ex(xb64, W64, B64)
-    assert (blk.cpu().double() - ref).abs().max() < 2e-5 * ref.abs().max()
-
-
 def test_qh_linear_tall_rows_pre_split_path(models):
     """o3.Linear over >= 2048 rows takes the pre-split-weight kernel batched over the 25 (l,m) slices (gemm_ps.cu::nb_gemm_ps_lm):
     per-pair features of config 4 (1e5 rows).  Checked against the float64 product with the exported per-order weights, 128 -> 128
