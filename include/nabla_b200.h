@@ -227,6 +227,17 @@ int nb200_painn_train_backward(nb200_engine* eng, const nb200_painn_weights* w,
                                void* workspace, int64_t workspace_bytes, int32_t with_force_seed,
                                const float* energy_seed, const float* force_seed,
                                const nb200_painn_weights* grads, int32_t* status, void* stream);
+/* Hessian-vector products of the PaiNN energy (both radial flavours): for each of n_dir position-space directions v[d] ([N,3], Angstrom)
+ *     hv[d] = H v[d] = -(dF/dR) v[d]       (H = d2 E / dR dR in Ha/A^2, so hv is in Ha/A)
+ * exact (forward-over-reverse tangent pass, no finite step), fp32 arithmetic and storage.  The primal forward runs once per call, the
+ * directions one after another; energy[B] and forces[N,3] (NULL => not written) are those of nb200_painn_energy_forces.  Molecules do not
+ * interact: one direction may displace an atom of every molecule at once.  `workspace` >= nb200_painn_hvp_workspace_bytes(w, b, n, e_cap,
+ * n_dir) (independent of n_dir >= 1).  Status and capacity conventions as nb200_painn_energy_forces; on a device error flag energy, forces
+ * and hv are NaN.  NB200_EINVAL (nothing launched) for a null required pointer, n_dir < 1 or a short workspace. */
+int64_t nb200_painn_hvp_workspace_bytes(const nb200_painn_weights* w, int32_t b_cap, int32_t n_cap, int32_t e_cap, int32_t n_dir);
+int nb200_painn_hvp(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
+                    int32_t n_mol, int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes,
+                    int32_t n_dir, const float* v, float* energy, float* forces, float* hv, int32_t* status, void* stream);
 
 /* ----------------------------------------------------------------------------------------
  * SchNet energy + forces (config/model/schnet.yaml: schnetpack.representation.SchNet inside

@@ -135,6 +135,9 @@ SIGNATURES = {
                                              c_void_p, c_int64, c_int32, c_void_p, c_void_p, POINTER(PainnWeights), c_void_p, c_void_p]),
     "nb200_painn_energy_forces": (c_int32, [c_void_p, POINTER(PainnWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32,
                                             c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_painn_hvp_workspace_bytes": (c_int64, [POINTER(PainnWeights), c_int32, c_int32, c_int32, c_int32]),
+    "nb200_painn_hvp": (c_int32, [c_void_p, POINTER(PainnWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,
+                                  c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 
     "nb200_gemnet_oc_graph_bytes": (c_int64, [c_int32, c_int32]),
     "nb200_gemnet_oc_graph_count": (c_int32, [POINTER(GemNetOCWeights), c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,

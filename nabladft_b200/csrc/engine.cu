@@ -13,6 +13,7 @@
 // `run_painn` is the one orchestration for inference, the energy-seeded parameter gradients (painn_train.cu) and the force-loss tangent
 // pass (painn_tangent.cu).
 #include <new>
+#include <utility>
 
 #include "engine_common.cuh"
 
@@ -116,6 +117,8 @@ struct Workspace {
     float *t_geom, *t_h1[kMaxLayers], *t_xh[kMaxLayers], *t_VW[kMaxLayers], *t_nrm[kMaxLayers], *t_g1[kMaxLayers], *t_y[kMaxLayers];
     float *t_q_in[kMaxLayers], *t_q_mid[kMaxLayers], *t_mu_mid[kMaxLayers], *t_mu[kMaxLayers + 1];
     float *t_q, *t_act, *t_ro, *t_gq, *t_gmu_a, *t_gmu_b, *t_gy, *t_gVW, *t_gt, *t_gn, *t_g_ro, *t_gW, *gWd;
+    // Hessian-vector product (run_painn_hvp): d2W/dd2 rows [L][E][3F] next to W, dW; tangent of the per-edge geometric gradient
+    float *d2W, *t_egrad;
     // fused node path (painn_fused.cu): per-layer inputs / post-message states instead of in-place q, mu; prepared weight tiles
     float *fq_in[kMaxLayers + 1], *fq_mid[kMaxLayers], *fmu_mid[kMaxLayers], *fdot[kMaxLayers], *gq_b, *fgn, *fgdot;
     void* wtiles;
@@ -123,7 +126,9 @@ struct Workspace {
     int64_t bytes;
 };
 
-Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool forces, bool train = false, bool tangent = false) {
+// `hvp` (with forces and tangent, without train): the Hessian-vector product's workspace -- the tangent arrays minus those only the weight
+// gradients read (t_q_in, t_q_mid, t_mu_mid, t_gW, gWd), plus d2W and t_egrad
+Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool forces, bool train = false, bool tangent = false, bool hvp = false) {
     (void)B;
     Workspace w{};
     Carver c(p);
@@ -173,7 +178,7 @@ Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool for
         for (int l = 0; l < L; ++l) {
             w.t_h1[l] = c.take<float>(N * F); w.t_xh[l] = c.take<float>(N * 3 * F); w.t_VW[l] = c.take<float>(N * 6 * F);
             w.t_nrm[l] = c.take<float>(N * F); w.t_g1[l] = c.take<float>(N * F); w.t_y[l] = c.take<float>(N * 3 * F);
-            w.t_q_in[l] = c.take<float>(N * F); w.t_q_mid[l] = c.take<float>(N * F); w.t_mu_mid[l] = c.take<float>(N * 3 * F);
+            if (!hvp) { w.t_q_in[l] = c.take<float>(N * F); w.t_q_mid[l] = c.take<float>(N * F); w.t_mu_mid[l] = c.take<float>(N * 3 * F); }
         }
         for (int l = 0; l <= L; ++l) w.t_mu[l] = c.take<float>(N * 3 * F);
         w.t_q = c.take<float>(N * F); w.t_act = c.take<float>(N * F); w.t_ro = c.take<float>(N * (F / 2));
@@ -189,7 +194,11 @@ Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool for
         w.gt = c.take<float>(N * F); w.t_gt = c.take<float>(N * F);
         w.gn = c.take<float>(N * F); w.t_gn = c.take<float>(N * F);
         w.t_g_ro = c.take<float>(N * (F / 2));
-        w.t_gW = c.take<float>(E * 3 * F); w.gWd = c.take<float>(E * 3 * F);
+        if (!hvp) { w.t_gW = c.take<float>(E * 3 * F); w.gWd = c.take<float>(E * 3 * F); }
+    }
+    if (hvp) {
+        w.d2W = c.take<float>((int64_t)L * E * 3 * F);
+        w.t_egrad = c.take<float>(4 * E);
     }
     for (int l = 0; l <= L; ++l) w.fq_in[l] = c.take<float>(N * F);
     for (int l = 0; l < L; ++l) { w.fq_mid[l] = c.take<float>(N * F); w.fmu_mid[l] = c.take<float>(N * 3 * F); w.fdot[l] = c.take<float>(N * F); }
@@ -667,4 +676,129 @@ extern "C" int nb200_painn_energy_forces_grads(nb200_engine* eng, const nb200_pa
     if (!grads) return NB200_EINVAL;
     return run_painn(eng, w, z, pos, mol_ptr, n_mol, n_atoms, e_cap, workspace, workspace_bytes, energy, forces, status, stream, energy_seed, grads,
                      force_seed);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Hessian-vector products H v = -dF/dR . v (DESIGN.md section 3.13): the primal forward (fused node kernels, activations kept, as the first
+// call of the two-call training step) runs once; then, per direction, the tangent forward of painn_tangent.cu and the stacked
+// [primal ; tangent] backward of the training step without any weight gradient, the message backward tangent also producing the tangent
+// of the per-edge geometric gradient (t_egrad), and the tangent of the force assembly.  The workspace holds ONE direction's tangent
+// arrays whatever n_dir is.
+namespace {
+
+int run_painn_hvp(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr, int32_t n_mol,
+                  int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes, int32_t n_dir, const float* v, float* energy, float* forces,
+                  float* hv, int32_t* status, void* stream) {
+    if (!eng || !weights_ok(w) || !z || !pos || !mol_ptr || !workspace || !v || !energy || !hv || !status || n_dir < 1) return NB200_EINVAL;
+    if (w->n_feat != NB_F || w->n_layers <= 0 || w->n_layers > kMaxLayers) return NB200_EUNSUPPORTED;
+    if (n_mol <= 0 || n_atoms <= 0 || e_cap <= 0) return NB200_EINVAL;
+    const int L = w->n_layers, F = NB_F, K = w->n_rbf, N = n_atoms;
+    Workspace ws = carve(workspace, L, F, n_mol, N, e_cap, true, false, true, true);
+    if (ws.bytes > workspace_bytes) return NB200_EINVAL;
+    cudaStream_t s = (cudaStream_t)stream;
+    cublasHandle_t h = eng->blas;
+    NB_BLAS(cublasSetStream(h, s) == CUBLAS_STATUS_SUCCESS);
+    NB_BLAS(cublasSetWorkspace(h, ws.blas_ws, kBlasWs) == CUBLAS_STATUS_SUCCESS);
+    const size_t wl = (size_t)e_cap * 3 * F;
+    { Scope sc(eng, s, CAT_NBR, 3);
+    NB_TRY(nb200_neighbor_build(pos, mol_ptr, n_mol, N, w->cutoff, w->max_neighbors, e_cap, ws.row_ptr, ws.col, ws.rev, ws.geom, ws.deg, status, s)); }
+    // W, dW/dd and d2W/dd2: one row per undirected pair, three arrays
+    { Scope sc(eng, s, CAT_FILTER, 4);
+    NB_TRY(nb_painn_filter_d2(ws.geom, status, e_cap, w->w_rbf, w->b_rbf, L, K, w->radial_mode, w->cutoff, w->rbf_offsets, w->rbf_coeff, w->rbf_xscale, ws.W,
+                              ws.dW, ws.d2W, ws.sort_scr, ws.rev, s)); }
+    // energies (and forces) with every activation the tangent pass reads kept: layer inputs / post-message states in fq_in, fmu_mid
+    NB_TRY(run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s, false, 0, true));
+
+    for (int32_t dir = 0; dir < n_dir; ++dir) {
+        // ---- tangent forward along v_dir (painn_tangent.cu; the same sequence as the force-loss term of the training step).  With timing on,
+        // its CAT_MSG_FWD scope brackets the whole tangent forward, GEMMs included (bench_hessian.py splits forward / backward with it).
+        {
+            Scope sc(eng, s, CAT_MSG_FWD, 1 + 6 * L);
+            NB_TRY(nb_geom_tan(ws.geom, ws.row_ptr, ws.col, v + (size_t)dir * 3 * N, N, ws.t_geom, s));
+            if (cudaMemsetAsync(ws.t_q, 0, (size_t)N * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();  // embedding: no tangent
+            if (cudaMemsetAsync(ws.t_mu[0], 0, (size_t)N * 3 * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();
+            for (int l = 0; l < L; ++l) {
+                const float* A1 = w->A1 + (size_t)l * F * F;
+                const float* A2 = w->A2 + (size_t)l * 3 * F * F;
+                const float* U = w->U + (size_t)l * 2 * F * F;
+                const float* B1 = w->B1 + (size_t)l * F * 2 * F;
+                const float* B2 = w->B2 + (size_t)l * 3 * F * F;
+                NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, A1, F, ws.t_h1[l], F, false, nullptr, nullptr));
+                NB_TRY(nb_mul_dact(ws.h1pre[l], ws.t_h1[l], (int64_t)N * F, ws.t_act, s));
+                NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, A2, F, ws.t_xh[l], 3 * F, false, nullptr, nullptr));
+                NB_TRY(nb_msg_fwd_tan(ws.xh[l], ws.t_xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.t_mu[l], ws.W + l * wl, ws.dW + l * wl, ws.geom,
+                                      ws.t_geom, ws.row_ptr, ws.col, N, ws.t_q, ws.t_mu[l + 1], s, 0, ws.rev));
+                NB_TRY(linear_fwd(eng, s, 3 * N, 2 * F, F, ws.t_mu[l + 1], F, U, F, ws.t_VW[l], 2 * F, false, nullptr, nullptr));
+                NB_TRY(nb_upd_norm_tan(ws.VW[l], ws.t_VW[l], ws.nrm[l], N, ws.t_nrm[l], s));
+                NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, B1, 2 * F, ws.t_g1[l], F, false, nullptr, nullptr));
+                NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_nrm[l], F, B1 + F, 2 * F, ws.t_g1[l], F, true, nullptr, nullptr));
+                NB_TRY(nb_mul_dact(ws.g1pre[l], ws.t_g1[l], (int64_t)N * F, ws.t_act, s));
+                NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, B2, F, ws.t_y[l], 3 * F, false, nullptr, nullptr));
+                NB_TRY(nb_upd_combine_tan(ws.t_q, ws.t_mu[l + 1], ws.VW[l], ws.t_VW[l], ws.y[l], ws.t_y[l], N, s));
+            }
+            NB_TRY(linear_fwd(eng, s, N, F / 2, F, ws.t_q, F, w->R1, F, ws.t_ro, F / 2, false, nullptr, nullptr));
+        }
+        // ---- backward, primal and tangent: every Linear backward on the stacked rows [g ; g^] (carve: adjacent pairs)
+        if (cudaMemsetAsync(ws.egrad, 0, (size_t)e_cap * 4 * sizeof(float), s) != cudaSuccess ||
+            cudaMemsetAsync(ws.t_egrad, 0, (size_t)e_cap * 4 * sizeof(float), s) != cudaSuccess ||
+            cudaMemsetAsync(ws.gmu_a, 0, (size_t)N * 3 * F * sizeof(float), s) != cudaSuccess ||
+            cudaMemsetAsync(ws.t_gmu_a, 0, (size_t)N * 3 * F * sizeof(float), s) != cudaSuccess)
+            return nb_check_launch();
+        { Scope sc(eng, s, CAT_READOUT, 2);
+          NB_TRY(nb_readout_bwd(ws.ro_pre, w->R2, N, F / 2, ws.g_ro, s));
+          NB_TRY(nb_readout_bwd_tan(ws.ro_pre, ws.t_ro, w->R2, N, F / 2, ws.t_g_ro, ws.t_act, s)); }
+        NB_TRY(linear_bwd(eng, s, N, F / 2, F, ws.g_ro, F / 2, w->R1, F, ws.gq, F, false));
+        NB_TRY(linear_bwd(eng, s, N, F / 2, F, ws.t_g_ro, F / 2, w->R1, F, ws.t_gq, F, false));
+        float *cur = ws.gmu_a, *other = ws.gmu_b, *t_cur = ws.t_gmu_a, *t_other = ws.t_gmu_b;
+        for (int l = L - 1; l >= 0; --l) {
+            const float* A1 = w->A1 + (size_t)l * F * F;
+            const float* A2 = w->A2 + (size_t)l * 3 * F * F;
+            const float* U = w->U + (size_t)l * 2 * F * F;
+            const float* B1 = w->B1 + (size_t)l * F * 2 * F;
+            const float* B2 = w->B2 + (size_t)l * 3 * F * F;
+            { Scope sc(eng, s, CAT_NODE, 2);
+              NB_TRY(nb_upd_combine_bwd(ws.gq, cur, ws.y[l], ws.VW[l], N, ws.gy, ws.gVW, s));
+              NB_TRY(nb_upd_combine_bwd_tan(ws.gq, ws.t_gq, cur, t_cur, ws.y[l], ws.t_y[l], ws.VW[l], ws.t_VW[l], N, ws.t_gy, ws.t_gVW, s)); }
+            NB_TRY(linear_bwd(eng, s, 2 * N, 3 * F, F, ws.gy, 3 * F, B2, F, ws.gt, F, false));
+            { Scope sc(eng, s, CAT_NODE, 2);
+              NB_TRY(nb_act_bwd_tan(ws.t_gt, ws.gt, ws.g1pre[l], ws.t_g1[l], (int64_t)N * F, s));  // needs gt BEFORE the primal act_bwd
+              NB_TRY(nb_act_bwd(ws.gt, ws.g1pre[l], (int64_t)N * F, NB_ACT_SILU, s)); }
+            NB_TRY(linear_bwd(eng, s, 2 * N, F, F, ws.gt, F, B1, 2 * F, ws.gq, F, true));
+            NB_TRY(linear_bwd(eng, s, 2 * N, F, F, ws.gt, F, B1 + F, 2 * F, ws.gn, F, false));
+            { Scope sc(eng, s, CAT_NODE, 2);
+              NB_TRY(nb_upd_norm_bwd_tan(ws.gn, ws.t_gn, ws.VW[l], ws.t_VW[l], ws.nrm[l], ws.t_nrm[l], N, ws.t_gVW, s));
+              NB_TRY(nb_upd_norm_bwd(ws.gn, ws.VW[l], ws.nrm[l], N, ws.gVW, s)); }
+            NB_TRY(linear_bwd(eng, s, 2 * 3 * N, 2 * F, F, ws.gVW, 2 * F, U, F, cur, F, true));  // (cur, t_cur) adjacent
+            // message backward of EVERY layer (egrad and its tangent collect contributions from all of them)
+            { Scope sc(eng, s, CAT_MSG_BWD, 2);
+              NB_TRY(nb_painn_msg_bwd_ex(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.W + l * wl, ws.dW + l * wl, 3 * F, ws.rev, ws.geom, ws.row_ptr, ws.col,
+                                         N, ws.gq, cur, ws.gy, other, ws.egrad, s, 0));
+              NB_TRY(nb_msg_bwd_hvp(ws.xh[l], ws.t_xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.t_mu[l], ws.W + l * wl, ws.dW + l * wl, ws.d2W + l * wl,
+                                    ws.geom, ws.t_geom, ws.row_ptr, ws.col, ws.rev, N, ws.gq, ws.t_gq, cur, t_cur, ws.t_gy, t_other, ws.t_egrad, s)); }
+            std::swap(cur, other); std::swap(t_cur, t_other);
+            if (l == 0) break;  // the embedding does not depend on positions
+            NB_TRY(linear_bwd(eng, s, 2 * N, 3 * F, F, ws.gy, 3 * F, A2, F, ws.gt, F, false));
+            { Scope sc(eng, s, CAT_NODE, 2);
+              NB_TRY(nb_act_bwd_tan(ws.t_gt, ws.gt, ws.h1pre[l], ws.t_h1[l], (int64_t)N * F, s));
+              NB_TRY(nb_act_bwd(ws.gt, ws.h1pre[l], (int64_t)N * F, NB_ACT_SILU, s)); }
+            NB_TRY(linear_bwd(eng, s, 2 * N, F, F, ws.gt, F, A1, F, ws.gq, F, true));
+        }
+        { Scope sc(eng, s, CAT_FORCE, 1);
+          NB_TRY(nb_edge_forces_hvp(ws.egrad, ws.t_egrad, ws.geom, ws.t_geom, ws.row_ptr, ws.rev, N, hv + (size_t)dir * 3 * N, s)); }
+    }
+    { Scope sc(eng, s, CAT_FORCE, 1); NB_TRY(nb_poison_on_error(status, energy, 0, hv, (int64_t)n_dir * 3 * N, s)); }
+    return NB200_OK;
+}
+
+}  // namespace
+
+extern "C" int64_t nb200_painn_hvp_workspace_bytes(const nb200_painn_weights* w, int32_t b_cap, int32_t n_cap, int32_t e_cap, int32_t n_dir) {
+    if (!w || w->n_layers <= 0 || w->n_layers > kMaxLayers || w->n_feat != NB_F || b_cap < 0 || n_cap < 0 || e_cap < 0 || n_dir < 1) return NB200_EINVAL;
+    return carve(nullptr, w->n_layers, w->n_feat, b_cap, n_cap, e_cap, true, false, true, true).bytes;
+}
+
+extern "C" int nb200_painn_hvp(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
+                               int32_t n_mol, int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes, int32_t n_dir, const float* v,
+                               float* energy, float* forces, float* hv, int32_t* status, void* stream) {
+    return run_painn_hvp(eng, w, z, pos, mol_ptr, n_mol, n_atoms, e_cap, workspace, workspace_bytes, n_dir, v, energy, forces, hv, status, stream);
 }

@@ -127,16 +127,32 @@ __device__ __forceinline__ EdgeRad radial_scalars(float d, int mode, float cutof
     return r;
 }
 
+// second derivatives (d2s1, d2s2) of the scalars above, for the Hessian-vector product (painn_tangent.cu k_msg_bwd_hvp)
+__device__ __forceinline__ float2 radial_d2(float d, int mode, float cutoff) {
+    if (mode == NB200_RADIAL_SPK) {
+        const float a = 3.14159265358979323846f / cutoff;
+        const float d2 = d < cutoff ? -0.5f * a * a * cosf(d * a) : 0.f;
+        return make_float2(d2, d2);
+    }
+    const float x = d * (1.0f / cutoff);
+    const float x3 = x * x * x;
+    return make_float2(x < 1.0f ? x3 * (-420.0f + x * (1050.0f - 630.0f * x)) * (1.0f / (cutoff * cutoff)) : 0.f, 0.f);
+}
+
 // WT = storage type of the rows (float, or nb_bf16: bf16 storage of the training path).  Layer l's rows start at the FLOAT offset
 // l * layer_stride of `W` / `dW` whatever WT is (the engine carves fp32-sized arrays; bf16 rows use the first half of a layer's block).
-template <bool WITH_DW, class WT>
+// WITH_D2W (fp32, separate arrays; needs WITH_DW): also d2W/dd2 into `d2W`, same layout -- the Hessian-vector product reads it.
+template <bool WITH_DW, class WT, bool WITH_D2W = false>
 __global__ void __launch_bounds__(FLT_THREADS) k_filter(const float* __restrict__ geom, const int32_t* __restrict__ status,
                                                        const int32_t* __restrict__ scr, const float* __restrict__ w_rbf,
                                                        const float* __restrict__ b_rbf, const float* __restrict__ offsets,
                                                        int n_rbf, int radial_mode, float cutoff, float coeff, float xscale,
-                                                       size_t layer_stride, int row_stride, float* __restrict__ W, float* __restrict__ dW) {
+                                                       size_t layer_stride, int row_stride, float* __restrict__ W, float* __restrict__ dW,
+                                                       float* __restrict__ d2W = nullptr) {
     // rows of `row_stride` floats: 3F (W and dW/dd in two arrays) or 6F (ONE 3 KB record [W | dW/dd] per edge, dW = W + 3F)
-    __shared__ __align__(16) float sphi[FLT_CHUNK][2 * NB_BAND + 4];
+    // staged row: [phi | phi' | s1 s1' s2 s2'] (+ [phi'' | s1'' s2'' 0 0] with WITH_D2W)
+    constexpr int NROW = WITH_D2W ? 3 * NB_BAND + 8 : 2 * NB_BAND + 4;
+    __shared__ __align__(16) float sphi[FLT_CHUNK][NROW];
     __shared__ int32_t sedge[FLT_CHUNK];
     if (status[1] != 0) return;
     const int bin = blockIdx.x, split = blockIdx.y, layer = blockIdx.z;
@@ -173,9 +189,14 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter(const float* __restrict_
                 const float p = expf(coeff * (t * t));  // torch.exp(coeff * pow(x - offset, 2))
                 row[kk] = p;
                 row[NB_BAND + kk] = p * (2.0f * coeff * xscale) * t;  // d phi / d d
+                if (WITH_D2W) row[2 * NB_BAND + 4 + kk] = p * (2.0f * coeff * xscale * xscale) * (1.0f + 2.0f * coeff * (t * t));  // d2 phi / d d2
             }
             row[2 * NB_BAND + 0] = r.s1; row[2 * NB_BAND + 1] = r.ds1;
             row[2 * NB_BAND + 2] = r.s2; row[2 * NB_BAND + 3] = r.ds2;
+            if (WITH_D2W) {
+                const float2 r2 = radial_d2(d, radial_mode, cutoff);
+                row[3 * NB_BAND + 4] = r2.x; row[3 * NB_BAND + 5] = r2.y; row[3 * NB_BAND + 6] = 0.f; row[3 * NB_BAND + 7] = 0.f;
+            }
             sedge[threadIdx.x] = e;
         }
         __syncthreads();
@@ -204,6 +225,21 @@ __global__ void __launch_bounds__(FLT_THREADS) k_filter(const float* __restrict_
                 fma4s(dw, acc0, sc.y);
                 fma4s(dw, acc1, sc.x);
                 stw4(dWl + off, dw);
+            }
+            if (WITH_D2W) {  // d2W = s1'' acc0 + 2 s1' acc1 + s1 acc2 + s2'' b
+                float4 acc2 = f4(0.f);
+#pragma unroll
+                for (int q4 = 0; q4 < NB_BAND / 4; ++q4) {
+                    const float4 p = row4[(2 * NB_BAND + 4) / 4 + q4];
+                    fma4s(acc2, wreg[4 * q4 + 0], p.x); fma4s(acc2, wreg[4 * q4 + 1], p.y);
+                    fma4s(acc2, wreg[4 * q4 + 2], p.z); fma4s(acc2, wreg[4 * q4 + 3], p.w);
+                }
+                const float4 s2 = row4[(3 * NB_BAND + 4) / 4];
+                float4 d2w = bias * s2.y;
+                fma4s(d2w, acc0, s2.x);
+                fma4s(d2w, acc1, 2.0f * sc.y);
+                fma4s(d2w, acc2, sc.x);
+                st4(d2W + (size_t)layer * layer_stride + off, d2w);
             }
         }
         __syncthreads();
@@ -414,6 +450,23 @@ int nb_painn_filter_ex(const float* geom, const int32_t* status, int32_t e_strid
     else
         k_filter<false, float><<<grid, FLT_THREADS, 0, s>>>(geom, status, sort_scratch, w_rbf, b_rbf, rbf_offsets, n_rbf, radial_mode, cutoff,
                                                           rbf_coeff, rbf_xscale, layer_stride, row_stride, W, dW);
+    return nb_check_launch();
+}
+
+// Hessian-vector product: W, dW/dd and d2W/dd2 in three fp32 arrays [L][e_stride][3F], one row per undirected pair (rev required)
+int nb_painn_filter_d2(const float* geom, const int32_t* status, int32_t e_stride, const float* w_rbf, const float* b_rbf, int32_t n_layers,
+                       int32_t n_rbf, int32_t radial_mode, float cutoff, const float* rbf_offsets, float rbf_coeff, float rbf_xscale, float* W,
+                       float* dW, float* d2W, int32_t* sort_scratch, const int32_t* rev, cudaStream_t s) {
+    if (!geom || !status || !w_rbf || !b_rbf || !rbf_offsets || !W || !dW || !d2W || !sort_scratch || !rev) return NB200_EINVAL;
+    if (n_rbf < NB_BAND || n_rbf > NB_NBINS_MAX) return NB200_EUNSUPPORTED;
+    if (radial_mode != NB200_RADIAL_SPK && radial_mode != NB200_RADIAL_OC) return NB200_EUNSUPPORTED;
+    if (n_layers <= 0 || e_stride < 0) return NB200_EINVAL;
+    const float dx = (cutoff * rbf_xscale) / (float)(n_rbf - 1);
+    if (!(rbf_coeff < 0.f) || rbf_coeff * (7.0f * dx) * (7.0f * dx) > -23.0f) return NB200_EUNSUPPORTED;
+    if (int rc = nb_bin_sort(geom, status, rbf_xscale, 1.0f / dx, n_rbf, sort_scratch, s, rev)) return rc;
+    dim3 grid(n_rbf, FLT_SPLIT, n_layers);
+    k_filter<true, float, true><<<grid, FLT_THREADS, 0, s>>>(geom, status, sort_scratch, w_rbf, b_rbf, rbf_offsets, n_rbf, radial_mode, cutoff, rbf_coeff,
+                                                             rbf_xscale, (size_t)e_stride * 3 * NB_F, 3 * NB_F, W, dW, d2W);
     return nb_check_launch();
 }
 

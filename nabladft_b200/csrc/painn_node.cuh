@@ -50,6 +50,17 @@ int nb_filter_wgrad_tan(const float* geom, const float* t_geom, const int32_t* s
                         int radial_mode, float cutoff, float rbf_coeff, float rbf_xscale, const float* t_gW, const float* gWd, float sign, float* g_w,
                         float* g_b, cudaStream_t s, int e_cap, int bf16);
 
+// Hessian-vector product (filter.cu, painn_tangent.cu)
+int nb_painn_filter_d2(const float* geom, const int32_t* status, int32_t e_stride, const float* w_rbf, const float* b_rbf, int32_t n_layers,
+                       int32_t n_rbf, int32_t radial_mode, float cutoff, const float* rbf_offsets, float rbf_coeff, float rbf_xscale, float* W,
+                       float* dW, float* d2W, int32_t* sort_scratch, const int32_t* rev, cudaStream_t s);
+int nb_msg_bwd_hvp(const float* xh, const float* t_xh, const float* xh_bias, const float* mu, const float* t_mu, const float* W, const float* dW,
+                   const float* d2W, const float* geom, const float* t_geom, const int32_t* row_ptr, const int32_t* col, const int32_t* rev, int n_atoms,
+                   const float* g_q, const float* t_g_q, const float* g_mu, const float* t_g_mu, float* t_g_xh, float* t_g_mu_in, float* t_egrad,
+                   cudaStream_t s);
+int nb_edge_forces_hvp(const float* egrad, const float* t_egrad, const float* geom, const float* t_geom, const int32_t* row_ptr, const int32_t* rev,
+                       int n_atoms, float* hv, cudaStream_t s);
+
 // fused per-layer node kernels (painn_fused.cu): wgmma chain of the update / message-MLP / readout Linear layers with their elementwise glue
 struct NbFusedFwd {
     int n_atoms, n_layers;

@@ -211,7 +211,11 @@ __global__ void __launch_bounds__(TN_THREADS) k_upd_norm_bwd_tan(const float* __
 // message backward tangent (by source atom j, slot e carries the opposite edge; painn_msg.cu k_painn_msg_bwd).  Also writes, per slot,
 //   t_gW[e]  = tangent of the per-edge filter gradient,   gWd[e] = (unseeded filter gradient) * dd_e
 // the two operands of the filter-weight gradient tangent (k_filter_wgrad_tan).
-template <class WT>
+// HVP = true (Hessian-vector product, fp32 rows): no filter-gradient operands; instead the tangent of the per-edge geometric gradient
+// egrad[e] = (dE/du'[3], dE/dd) the primal kernel accumulates is ADDED to t_egrad[e] (one lane per slot, layers run in order: deterministic):
+//   dE/dd^    = sum_ch d2W dd fW + dW fW^          (fW = the per-edge filter gradient above, d2W = d2W/dd2 of the row)
+//   dE/du'^[x] = sum_ch (Wb b)^ gmu_i[x] + (Wb b) gmu_i^[x]
+template <class WT, bool HVP = false>
 __global__ void __launch_bounds__(TN_THREADS) k_msg_bwd_tan(const float* __restrict__ xh, const float* __restrict__ t_xh, const float* __restrict__ xh_bias,
                                                            const float* __restrict__ mu, const float* __restrict__ t_mu,
                                                            const WT* __restrict__ W, const WT* __restrict__ dW,
@@ -220,7 +224,8 @@ __global__ void __launch_bounds__(TN_THREADS) k_msg_bwd_tan(const float* __restr
                                                            const float* __restrict__ g_q, const float* __restrict__ t_g_q,
                                                            const float* __restrict__ g_mu, const float* __restrict__ t_g_mu,
                                                            float* __restrict__ t_g_xh, float* __restrict__ t_g_mu_in, WT* __restrict__ t_gW,
-                                                           WT* __restrict__ gWd, const int32_t* __restrict__ rev) {
+                                                           WT* __restrict__ gWd, const int32_t* __restrict__ rev, const float* __restrict__ d2W = nullptr,
+                                                           float* __restrict__ t_egrad = nullptr) {
     const int t = blockIdx.x * TN_THREADS + threadIdx.x;
     const int j = t >> 5, c = (t & 31) * 4;
     if (j >= n_atoms) return;
@@ -265,16 +270,70 @@ __global__ void __launch_bounds__(TN_THREADS) k_msg_bwd_tan(const float* __restr
         float4 fa_h = a_h * gq; fma4(fa_h, a, gq_h);
         float4 fb_h = b_h * tb; fma4(fb_h, b, tb_h);
         float4 fc_h = c_h * tc; fma4(fc_h, cc, tc_h);
-        WT* o = t_gW + (size_t)e * 3 * NB_F + c;
-        stw4(o, fa_h); stw4(o + NB_F, fb_h); stw4(o + 2 * NB_F, fc_h);
-        WT* o2 = gWd + (size_t)e * 3 * NB_F + c;
-        stw4(o2, fa * tg.w); stw4(o2 + NB_F, fb * tg.w); stw4(o2 + 2 * NB_F, fc * tg.w);
+        if (!HVP) {
+            WT* o = t_gW + (size_t)e * 3 * NB_F + c;
+            stw4(o, fa_h); stw4(o + NB_F, fb_h); stw4(o + 2 * NB_F, fc_h);
+            WT* o2 = gWd + (size_t)e * 3 * NB_F + c;
+            stw4(o2, fa * tg.w); stw4(o2 + NB_F, fb * tg.w); stw4(o2 + 2 * NB_F, fc * tg.w);
+        } else {
+            const float* d2 = d2W + wr * 3 * NB_F + c;
+            float4 sd = ldg4(d2) * fa; fma4(sd, ldg4(d2 + NB_F), fb); fma4(sd, ldg4(d2 + 2 * NB_F), fc);
+            sd = sd * tg.w;
+            fma4(sd, ldw4(dw), fa_h); fma4(sd, ldw4(dw + NB_F), fb_h); fma4(sd, ldw4(dw + 2 * NB_F), fc_h);
+            const float4 pb = wb * b;
+            float4 pb_h = wb_h * b; fma4(pb_h, wb, b_h);
+            float4 u0 = pb_h * h0; fma4(u0, pb, h0_h);
+            float4 u1 = pb_h * h1; fma4(u1, pb, h1_h);
+            float4 u2 = pb_h * h2; fma4(u2, pb, h2_h);
+            float r0 = hsum4(u0), r1 = hsum4(u1), r2 = hsum4(u2), r3 = hsum4(sd);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                r0 += __shfl_xor_sync(0xffffffffu, r0, o); r1 += __shfl_xor_sync(0xffffffffu, r1, o);
+                r2 += __shfl_xor_sync(0xffffffffu, r2, o); r3 += __shfl_xor_sync(0xffffffffu, r3, o);
+            }
+            if ((t & 31) == 0) {
+                float* te = t_egrad + 4 * (size_t)e;
+                st4(te, *reinterpret_cast<const float4*>(te) + make_float4(r0, r1, r2, r3));
+            }
+        }
     }
     float* gx = t_g_xh + (size_t)j * 3 * NB_F + c;
     st4(gx, ga); st4(gx + NB_F, gb); st4(gx + 2 * NB_F, gc);
     const float* tgmj = t_g_mu + (size_t)j * 3 * NB_F + c;
     float* go = t_g_mu_in + (size_t)j * 3 * NB_F + c;
     st4(go, ldg4(tgmj) + gm0); st4(go + NB_F, ldg4(tgmj + NB_F) + gm1); st4(go + 2 * NB_F, ldg4(tgmj + 2 * NB_F) + gm2);
+}
+
+// Tangent of the force assembly (painn_msg.cu k_edge_forces): hv = H v = -F^.  Slot e holds eg = (gu[3], gd) of the opposite edge e',
+// u' = -u_e, with  G = P/d + gd u',  P = gu - (gu.u') u':
+//   G^ = P^/d - P d^/d^2 + gd^ u' + gd u'^,   P^ = gu^ - (gu^.u' + gu.u'^) u' - (gu.u') u'^
+// One thread per atom over its own CSR row, like the primal: no atomics, bitwise repeatable.
+__device__ __forceinline__ float3 edge_G_tan(const float4 eg, const float4 t_eg, const float4 g, const float4 t_g) {
+    const float ux = -g.x, uy = -g.y, uz = -g.z, tux = -t_g.x, tuy = -t_g.y, tuz = -t_g.z;
+    const float inv = 1.0f / g.w, t_d = t_g.w;
+    const float dot = eg.x * ux + eg.y * uy + eg.z * uz;
+    const float t_dot = t_eg.x * ux + t_eg.y * uy + t_eg.z * uz + eg.x * tux + eg.y * tuy + eg.z * tuz;
+    const float px = eg.x - dot * ux, py = eg.y - dot * uy, pz = eg.z - dot * uz;
+    const float tpx = t_eg.x - t_dot * ux - dot * tux, tpy = t_eg.y - t_dot * uy - dot * tuy, tpz = t_eg.z - t_dot * uz - dot * tuz;
+    const float s = t_d * inv * inv;
+    return make_float3(tpx * inv - px * s + t_eg.w * ux + eg.w * tux, tpy * inv - py * s + t_eg.w * uy + eg.w * tuy,
+                       tpz * inv - pz * s + t_eg.w * uz + eg.w * tuz);
+}
+
+__global__ void __launch_bounds__(TN_THREADS) k_edge_forces_hvp(const float* __restrict__ egrad, const float* __restrict__ t_egrad,
+                                                               const float* __restrict__ geom, const float* __restrict__ t_geom,
+                                                               const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ rev, int n_atoms,
+                                                               float* __restrict__ hv) {
+    const int j = blockIdx.x * TN_THREADS + threadIdx.x;
+    if (j >= n_atoms) return;
+    float hx = 0.f, hy = 0.f, hz = 0.f;
+    for (int e = row_ptr[j]; e < row_ptr[j + 1]; ++e) {
+        const int r = rev[e];
+        const float3 g1 = edge_G_tan(ldg4(egrad + 4 * (size_t)e), ldg4(t_egrad + 4 * (size_t)e), ldg4(geom + 4 * (size_t)e), ldg4(t_geom + 4 * (size_t)e));
+        const float3 g2 = edge_G_tan(ldg4(egrad + 4 * (size_t)r), ldg4(t_egrad + 4 * (size_t)r), ldg4(geom + 4 * (size_t)r), ldg4(t_geom + 4 * (size_t)r));
+        hx += g1.x - g2.x; hy += g1.y - g2.y; hz += g1.z - g2.z;
+    }
+    hv[3 * (size_t)j] = hx; hv[3 * (size_t)j + 1] = hy; hv[3 * (size_t)j + 2] = hz;
 }
 
 }  // namespace
@@ -339,5 +398,19 @@ int nb_msg_bwd_tan(const float* xh, const float* t_xh, const float* xh_bias, con
     else
         k_msg_bwd_tan<float><<<tn_grid((int64_t)n_atoms * 32), TN_THREADS, 0, s>>>(xh, t_xh, xh_bias, mu, t_mu, W, dW, geom, t_geom, row_ptr, col, n_atoms, g_q,
                                                                                   t_g_q, g_mu, t_g_mu, t_g_xh, t_g_mu_in, t_gW, gWd, rev);
+    return nb_check_launch();
+}
+int nb_msg_bwd_hvp(const float* xh, const float* t_xh, const float* xh_bias, const float* mu, const float* t_mu, const float* W, const float* dW,
+                   const float* d2W, const float* geom, const float* t_geom, const int32_t* row_ptr, const int32_t* col, const int32_t* rev, int n_atoms,
+                   const float* g_q, const float* t_g_q, const float* g_mu, const float* t_g_mu, float* t_g_xh, float* t_g_mu_in, float* t_egrad,
+                   cudaStream_t s) {
+    k_msg_bwd_tan<float, true><<<tn_grid((int64_t)n_atoms * 32), TN_THREADS, 0, s>>>(xh, t_xh, xh_bias, mu, t_mu, W, dW, geom, t_geom, row_ptr, col, n_atoms,
+                                                                                    g_q, t_g_q, g_mu, t_g_mu, t_g_xh, t_g_mu_in, nullptr, nullptr, rev, d2W,
+                                                                                    t_egrad);
+    return nb_check_launch();
+}
+int nb_edge_forces_hvp(const float* egrad, const float* t_egrad, const float* geom, const float* t_geom, const int32_t* row_ptr, const int32_t* rev,
+                       int n_atoms, float* hv, cudaStream_t s) {
+    k_edge_forces_hvp<<<tn_grid(n_atoms), TN_THREADS, 0, s>>>(egrad, t_egrad, geom, t_geom, row_ptr, rev, n_atoms, hv);
     return nb_check_launch();
 }

@@ -251,6 +251,49 @@ class PainnEngine:
         self._kept_token = 0  # the backward reuses transient buffers; a second backward of the same forward recomputes
         return grads
 
+    # ------------------------------------------------------------------ Hessian-vector products
+    def run_hvp(self, z, pos, mol_ptr, n_mol, v, with_forces: bool = True):
+        """Exact Hessian-vector products of the energy (`nb200_painn_hvp`): v [n_dir, n_atoms, 3] (or [n_atoms, 3]) fp32 CUDA, in Angstrom.
+        Returns (energy [B], forces [N, 3] or None, hv [n_dir, N, 3] = H v in Ha/A).  Synchronous like `run`: checks the device status and
+        regrows the edge capacity once."""
+        if self.kind != "painn":
+            raise NotImplementedError("Hessian-vector products are built for the PaiNN engine only")
+        if self._weights is None:
+            raise NablaB200Error("set_weights() first")
+        n_atoms, dev = z.shape[0], z.device
+        if not (z.is_cuda and z.dtype == torch.int32 and pos.dtype == torch.float32 and mol_ptr.dtype == torch.int32):
+            raise NablaB200Error("run_hvp(): need CUDA int32 z / mol_ptr and fp32 pos")
+        if v.dim() == 2:
+            v = v.unsqueeze(0)
+        if not (v.is_cuda and v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n_atoms, 3) and v.shape[0] >= 1):
+            raise NablaB200Error("run_hvp(): v must be a contiguous fp32 CUDA tensor [n_dir, n_atoms, 3] with n_dir >= 1")
+        n_dir = v.shape[0]
+        self._kept_token = 0  # this call overwrites the workspace a kept training forward lives in
+        for _ in range(2):
+            e_cap = max(self.e_cap, n_atoms * self.edges_per_atom_guess)
+            self.e_cap = e_cap
+            need = self.lib.nb200_painn_hvp_workspace_bytes(byref(self._weights), n_mol, n_atoms, e_cap, n_dir)
+            if need < 0:
+                check(int(need), "nb200_painn_hvp_workspace_bytes")
+            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
+                self._ws = None
+                self._ws = torch.empty(int(need * 1.05) + 256, dtype=torch.uint8, device=dev)
+            if self._status is None or self._status.device != dev:
+                self._status = torch.zeros(4, dtype=torch.int32, device=dev)
+            energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+            forces = torch.empty(n_atoms, 3, dtype=torch.float32, device=dev) if with_forces else None
+            hv = torch.empty(n_dir, n_atoms, 3, dtype=torch.float32, device=dev)
+            rc = self.lib.nb200_painn_hvp(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(self._ws),
+                                          self._ws.numel(), n_dir, ptr(v), ptr(energy), ptr(forces), ptr(hv), ptr(self._status), current_stream())
+            check(rc, "nb200_painn_hvp")
+            st = self._status.cpu()
+            if int(st[1]) == -4:
+                self.e_cap = int(int(st[0]) * 1.1) + 1024
+                continue
+            self.raise_on_status(st)
+            return energy, forces, hv
+        raise NablaB200Error("edge capacity regrow failed")
+
     # ------------------------------------------------------------------ asynchronous inference (the reference-facing forward())
     _MAX_PENDING = 8
 
