@@ -361,6 +361,31 @@ int nb200_lbfgs_step(void* state, int64_t state_bytes, const int32_t* mol_ptr, i
                      float* pos32_out, int32_t* unconverged_out, int32_t* n_normalizations, void* stream);
 
 /* ----------------------------------------------------------------------------------------
+ * Batched molecular dynamics (PYGAseInterface.init_md / run_md of nablaDFT/optimization/pyg_ase_interface.py): ASE 3.22
+ * VelocityVerlet and Langevin(fixcm=True) for a whole batch, one CTA per molecule, float64 positions and momenta (csrc/md.cu,
+ * oracle/md.py).  ASE units: eV, A, u, ASE time.  Noise: counter-based Philox4x32-10, key = seed, counter = (global atom index,
+ * noise step, stream, call); the layout is specified in csrc/md.cu.  The caller owns every buffer:
+ *   mass   double [n_atoms] (u);  pos, mom  double [n_atoms,3], in/out;  pos32 float [n_atoms,3] = (float)pos for the engine
+ *   forces float [n_atoms,3] and energy float [n_mol] in the engine's units; f_scale / e_scale convert them to eV/A and eV
+ * nb200_md_init_momenta: MaxwellBoltzmannDistribution(kT), then Stationary and ZeroRotation, each rescaling back to the kinetic
+ *   energy it found (preserve_temperature); noise step `noise_step`, stream 0.  A principal moment below 1e-10 of the largest counts as
+ *   zero; a molecule without kinetic energy is not rescaled.
+ * nb200_md_step: `phase` = 1 FINISH (second half-kick of the step with noise step `step`, with `forces` evaluated at `pos`) | 2 START
+ *   (first half-kick and drift of step `step + 1`; writes pos, mom, pos32).  thermostat 0: velocity Verlet; 1: Langevin at kT with
+ *   friction `gamma` (1 / ASE time).  log_slot (optional) double [n_mol][2]: Epot, Ekin after FINISH and before START; frame_pos /
+ *   frame_mom (optional) double [n_atoms,3] copies of pos / mom at the same point.  status (optional, then worst required): the
+ *   engine's int32[4] status word; worst[0] = max edges, [1] = min error code, [2] = max degree, [3] = 1 once a status reported
+ *   NB200_ECAPACITY.  While status or worst shows an error, the call leaves pos, mom and pos32 untouched (the engine's outputs are NaN).
+ * NB200_EINVAL (nothing launched) for a null required pointer, n_mol < 0, dt <= 0, kT < 0, gamma < 0, a bad phase or thermostat,
+ * or a noise step outside [0, 2^32); NB200_OK with nothing written for n_mol == 0.  Asynchronous on `stream`. */
+int nb200_md_init_momenta(const int32_t* mol_ptr, int32_t n_mol, const double* mass, const double* pos, double kT, uint64_t seed,
+                          int64_t noise_step, double* mom, void* stream);
+int nb200_md_step(const int32_t* mol_ptr, int32_t n_mol, const double* mass, int32_t phase, int32_t thermostat, double dt, double kT,
+                  double gamma, uint64_t seed, int64_t step, double f_scale, double e_scale, double* pos, double* mom, float* pos32,
+                  const float* forces, const float* energy, double* log_slot, double* frame_pos, double* frame_mom,
+                  const int32_t* status, int32_t* worst, void* stream);
+
+/* ----------------------------------------------------------------------------------------
  * GemNet-OC energy + direct coupled forces (SURVEY.md section 8 a19 / f3), config/model/gemnet-oc.yaml:
  * non-periodic, quadruplet + atom-edge + edge-atom + atom-atom interactions, `forces_coupled`, `extensive`.
  * Replaces GemNetOC.forward (nablaDFT/gemnet_oc/gemnet_oc.py:1121-1251) and everything below it: the four graphs and their

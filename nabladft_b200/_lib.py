@@ -6,7 +6,7 @@ There is NO fallback: if the shared library is missing or a call fails, we raise
 """
 import ctypes
 import os
-from ctypes import c_double, POINTER, c_float, c_int32, c_int64, c_void_p
+from ctypes import c_double, POINTER, c_float, c_int32, c_int64, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libnabla_b200.so")
@@ -120,6 +120,9 @@ SIGNATURES = {
     "nb200_lbfgs_state_bytes": (c_int64, [c_int32, c_int32, c_int32]),
     "nb200_lbfgs_step": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_double, c_double, c_double,
                                    c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_md_init_momenta": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_double, c_uint64, c_int64, c_void_p, c_void_p]),
+    "nb200_md_step": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_double, c_double, c_double, c_uint64, c_int64, c_double, c_double]
+                      + [c_void_p] * 11),
     "nb200_painn_workspace_bytes": (c_int64, [POINTER(PainnWeights), c_int32, c_int32, c_int32, c_int32]),
     "nb200_schnet_workspace_bytes": (c_int64, [POINTER(SchnetWeights), c_int32, c_int32, c_int32, c_int32]),
     "nb200_schnet_energy_forces": (c_int32, [c_void_p, POINTER(SchnetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32,
