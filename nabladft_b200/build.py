@@ -16,7 +16,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
-] + os.environ.get("NB200_NVCC_EXTRA", "").split()  # e.g. -DNF_PROF for the pipeline role timing
+] + os.environ.get("NB200_NVCC_EXTRA", "").split()
 
 
 def sources():

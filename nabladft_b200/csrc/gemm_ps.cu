@@ -46,7 +46,6 @@ struct GemmParams {
     int M, N, K, KC, n_nt, tiles_per_cta;
     int spt;                      // 32-k stages per weight tile that carry data (K <= 96: fewer than 4)
     int epi; float epi_alpha;     // NB_EPI_* (common.cuh)
-    int xsplit;                   // K > 128: activation slabs handed over in two K halves (tc_pipe.cuh)
     int lm_batch;                 // 1: blockIdx.z = (l,m) row of an equivariant feature; weights per l, bias on lm = 0 only
     long long a_boff, c_boff, w_boff;
     const float* A; int lda;
@@ -56,6 +55,8 @@ struct GemmParams {
     float* act; int act_kind;
 };
 
+// L (tc_pipe.cuh): OneGroup for K <= 128 and the lm path, TwoGroups for K > 128 (see gemm_ps_impl)
+template <class L>
 __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmParams P0) {
     extern __shared__ __align__(1024) unsigned char smem[];
     GemmParams P = P0;
@@ -68,8 +69,7 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
     const int t_begin = blockIdx.y * P.tiles_per_cta, t_end = min(t_begin + P.tiles_per_cta, P.n_nt);
     if (t_begin >= t_end) return;
     const int n_it = t_end - t_begin, KC = P.KC, n_units = n_it * KC;
-    Ctx c = setup(smem, tid, P.xsplit);
-    NF_PROF_DO(const long long tk0_ = clock64(); long long w_epi_ = 0;)
+    Ctx<L> c = setup<L>(smem, tid);
     // unit u = (N tile t_begin + u / KC, K chunk u % KC).  K <= 128: the activation slab is written once and stays; else once per unit.
     auto flags_of = [&](int u) {
         const int kc = u % KC;
@@ -77,13 +77,12 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
     };
     if (warp >= WARP_ISSUE) {
         run_issuer_t(c, n_units, flags_of, [&](int u) { return (t_begin + u / KC) * KC + u % KC; }, P.wt, P.spt);
-        NF_PROF_DO(if (warp == WARP_ISSUE && lane == 0) { atomicAdd(&g_nf_prof[0], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[1], (unsigned long long)c.w_x);
-                   atomicAdd(&g_nf_prof[2], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[3], (unsigned long long)c.w_full); })
     } else {
         const int M = P.M, m0 = blockIdx.x * NT;
-        const int fl = 32 * (warp & 3) + lane, n0 = CPT * (warp >> 2);
-        const bool isE = role_epi(warp), isL = role_load(warp);
-        const int ltid = load_tid(tid);
+        const int fl = 32 * (warp & 3) + lane, n0 = L::CPT * (warp >> 2);
+        // epilogue warps [0, NEPI), loader warps [NWORK - NLOAD, NWORK): with one group every worker warp is both
+        const bool isE = warp < L::NEPI, isL = warp >= NWORK - L::NLOAD;
+        const int ltid = tid - 32 * (NWORK - L::NLOAD);
 #pragma unroll 1
         for (int u = 0; u < n_units; ++u) {
             const int fg = flags_of(u), kc_i = u % KC;
@@ -99,7 +98,6 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
             if ((fg & U_LAST) && isE) {
                 const int n = (t_begin + u / KC) * 128 + fl;
                 drain(c, warp);
-                NF_PROF_DO(const long long te0_ = clock64();)
                 const bool n_ok = n < P.N;
                 const float b = (P.bias && n_ok) ? __ldg(P.bias + n) : 0.f;
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
@@ -127,45 +125,19 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
                         }
                     }
                 });
-                NF_PROF_DO(w_epi_ += clock64() - te0_;)
             }
         }
     }
-    NF_PROF_DO(if (tid == 0) { atomicAdd(&g_nf_prof[4], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[5], (unsigned long long)c.w_acc);
-                            atomicAdd(&g_nf_prof[6], (unsigned long long)c.w_xfree); atomicAdd(&g_nf_prof[7], 1ull); atomicAdd(&g_nf_prof[8], (unsigned long long)w_epi_); })
 }
 
 // grow-only scratch for the prepared weights, one per (thread, stream): calls on one stream are ordered, so the buffer is reused safely
 struct Scratch { void* p = nullptr; size_t bytes = 0; };
 thread_local std::map<cudaStream_t, Scratch> g_scratch;
 
-}  // namespace
-
-// This file is compiled TWICE: as itself (all 16 worker warps load operands and run epilogues, in program order) and, through gemm_ps2.cu, with
-// NF_TWO_GROUPS (8 loader warps run ahead of 8 epilogue warps, tc_pipe.cuh) -- the build used for K > 128, where the finished tile's drain + 64 KB
-// of stores otherwise delay the next activation operand.  The second build exports only
-// nb_gemm_ps_impl_2g.
-int nb_gemm_ps_impl_2g(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate, const float* bias,
-                       float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, int epi, float epi_alpha);
-#ifndef NB_GEMM_PS_2G
-size_t nb_gemm_ps_ws_bytes(int N, int K) { return (size_t)((N + 127) / 128) * ((K + 127) / 128) * WTILE_BYTES; }
-
-// worth it when the weight preparation is amortised over many row slabs
-// (K = 32: the radial-basis layers of QHNet's convolution, [E, 32] x [32, 5376] -- one stage per tile, bound by the output write)
-bool nb_gemm_ps_wanted(int M, int N, int K) { return M >= 2048 && N >= 64 && K >= 32 && K % 4 == 0; }
-#endif
-
-// `ws` (>= nb_gemm_ps_ws_bytes(N, K)) may be NULL: a per-stream grow-only scratch owned by this translation unit is used then.
-static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-                        const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, int epi, float epi_alpha) {
-    if (!A || !B || !C || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
-    if (K % 4 || lda % 4 || ldc < N) return NB200_EUNSUPPORTED;
-    if (M == 0) return NB200_OK;
-    const int n_nt = (N + 127) / 128, KC = (K + 127) / 128;
-#ifndef NB_GEMM_PS_2G
-    if (KC > 1) return nb_gemm_ps_impl_2g(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, ws, ws_bytes, s, epi, epi_alpha);
-#endif
-    const size_t need = nb_gemm_ps_ws_bytes(N, K);
+// Set-up shared by the entry points: `ws` (the prepared-weight buffer) becomes the stream's scratch, grown to `need` bytes, unless the caller
+// passed one; the dynamic shared-memory limit of k_gemm_ps<L> is raised once per process and layout.
+template <class L>
+int gemm_ps_ready(void*& ws, size_t need, cudaStream_t s) {
     if (!ws) {
         Scratch& sc = g_scratch[s];
         if (sc.bytes < need) {
@@ -174,36 +146,53 @@ static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const floa
             sc.bytes = need;
         }
         ws = sc.p;
-    } else if (ws_bytes < need) {
-        return NB200_EINVAL;
     }
     static bool attr = false;
     if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_ps, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL) != cudaSuccess) return nb_check_launch();
+        if (cudaFuncSetAttribute(k_gemm_ps<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL) != cudaSuccess) return nb_check_launch();
         attr = true;
     }
+    return NB200_OK;
+}
+
+}  // namespace
+
+size_t nb_gemm_ps_ws_bytes(int N, int K) { return (size_t)((N + 127) / 128) * ((K + 127) / 128) * WTILE_BYTES; }
+
+// worth it when the weight preparation is amortised over many row slabs
+// (K = 32: the radial-basis layers of QHNet's convolution, [E, 32] x [32, 5376] -- one stage per tile, bound by the output write)
+bool nb_gemm_ps_wanted(int M, int N, int K) { return M >= 2048 && N >= 64 && K >= 32 && K % 4 == 0; }
+
+// `ws` (>= nb_gemm_ps_ws_bytes(N, K)) may be NULL: a per-stream grow-only scratch owned by this translation unit is used then.
+static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
+                        const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, int epi, float epi_alpha) {
+    if (!A || !B || !C || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
+    if (K % 4 || lda % 4 || ldc < N) return NB200_EUNSUPPORTED;
+    if (M == 0) return NB200_OK;
+    const int n_nt = (N + 127) / 128, KC = (K + 127) / 128;
+    const size_t need = nb_gemm_ps_ws_bytes(N, K);
+    if (ws && ws_bytes < need) return NB200_EINVAL;
+    // K > 128: every (N tile, K chunk) needs a fresh activation operand.  With two worker groups, handing it over in K halves, the loaders
+    // write the next operand while the epilogue group drains the finished tile and stores it, instead of after that.
+    const bool two_groups = KC > 1;
+    const int rc = two_groups ? gemm_ps_ready<TwoGroups>(ws, need, s) : gemm_ps_ready<OneGroup>(ws, need, s);
+    if (rc != NB200_OK) return rc;
     k_prep_gemm<<<n_nt * KC * 4, 256, 0, s>>>(B, ldb, trans_b ? 1 : 0, N, K, KC, static_cast<unsigned char*>(ws));
     GemmParams P{};
     P.M = M; P.N = N; P.K = K; P.KC = KC; P.n_nt = n_nt; P.A = A; P.lda = lda; P.wt = static_cast<const unsigned char*>(ws);
     P.C = C; P.ldc = ldc; P.accumulate = accumulate; P.bias = bias; P.act = act; P.act_kind = act_kind;
     P.spt = KC == 1 ? (K + KSTAGE - 1) / KSTAGE : STAGES_PER_TILE;
     P.epi = epi; P.epi_alpha = epi_alpha;
-    P.xsplit = KC > 1 ? 1 : 0;
     const int m_tiles = (M + NT - 1) / NT;
     int ny = 1;
     while (m_tiles * ny < nb_sm_count() && ny < n_nt) ++ny;  // few row slabs: split the N walk (the activation slab is re-staged per CTA)
     P.tiles_per_cta = (n_nt + ny - 1) / ny;
     dim3 grid(m_tiles, (n_nt + P.tiles_per_cta - 1) / P.tiles_per_cta);
-    k_gemm_ps<<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
+    if (two_groups) k_gemm_ps<TwoGroups><<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
+    else k_gemm_ps<OneGroup><<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
     return nb_check_launch();
 }
 
-#ifdef NB_GEMM_PS_2G
-int nb_gemm_ps_impl_2g(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate, const float* bias,
-                       float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, int epi, float epi_alpha) {
-    return gemm_ps_impl(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, ws, ws_bytes, s, epi, epi_alpha);
-}
-#else
 int nb_gemm_ps(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
                const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s) {
     return gemm_ps_impl(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, ws, ws_bytes, s, NB_EPI_PLAIN, 1.0f);
@@ -229,38 +218,18 @@ int nb_gemm_ps_lm(int M, int N, int K, const float* A, int lda, const float* W_l
     const int n_l = n_lm > 16 ? 5 : n_lm > 9 ? 4 : n_lm > 4 ? 3 : n_lm > 1 ? 2 : 1;
     const int n_nt = (N + 127) / 128, KC = (K + 127) / 128;
     const size_t per_w = nb_gemm_ps_ws_bytes(N, K), need = per_w * n_l;
-    Scratch& sc = g_scratch[s];
-    if (sc.bytes < need) {
-        if (sc.p) cudaFree(sc.p);
-        if (cudaMalloc(&sc.p, need) != cudaSuccess) { sc = Scratch{}; return nb_check_launch(); }
-        sc.bytes = need;
-    }
-    static bool attr = false;
-    if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_ps, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL) != cudaSuccess) return nb_check_launch();
-        attr = true;
-    }
+    void* ws = nullptr;
+    const int rc = gemm_ps_ready<OneGroup>(ws, need, s);
+    if (rc != NB200_OK) return rc;
     for (int l = 0; l < n_l; ++l)
-        k_prep_gemm<<<n_nt * KC * 4, 256, 0, s>>>(W_l + (size_t)l * w_l_stride, N, 1, N, K, KC, static_cast<unsigned char*>(sc.p) + (size_t)l * per_w);
+        k_prep_gemm<<<n_nt * KC * 4, 256, 0, s>>>(W_l + (size_t)l * w_l_stride, N, 1, N, K, KC, static_cast<unsigned char*>(ws) + (size_t)l * per_w);
     GemmParams P{};
-    P.M = M; P.N = N; P.K = K; P.KC = KC; P.n_nt = n_nt; P.A = A; P.lda = lda; P.wt = static_cast<const unsigned char*>(sc.p);
+    P.M = M; P.N = N; P.K = K; P.KC = KC; P.n_nt = n_nt; P.A = A; P.lda = lda; P.wt = static_cast<const unsigned char*>(ws);
     P.C = C; P.ldc = ldc; P.accumulate = accumulate; P.bias = bias; P.act = nullptr; P.act_kind = 0;
     P.spt = KC == 1 ? (K + KSTAGE - 1) / KSTAGE : STAGES_PER_TILE;
     P.lm_batch = 1; P.a_boff = K; P.c_boff = N; P.w_boff = (long long)per_w;
     P.tiles_per_cta = n_nt;
     dim3 grid((M + NT - 1) / NT, 1, n_lm);
-    k_gemm_ps<<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
+    k_gemm_ps<OneGroup><<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
     return nb_check_launch();
 }
-
-#endif  // !NB_GEMM_PS_2G
-
-#if defined(NF_PROF) && !defined(NB_GEMM_PS_2G)
-// role timing of k_gemm_ps (tools/gemm_ps_prof.py): [0] issuer total, [1] issuer waits X, [2] issuer waits staging, [3] issuer waits W ring,
-// [4] worker thread 0 total, [5] worker waits accumulator (incl. drain), [6] worker waits X release, [7] CTAs, [8] worker epilogue (stores)
-extern "C" int nb200_debug_gemm_ps_prof(unsigned long long* out16, int reset) {
-    if (cudaMemcpyFromSymbol(out16, g_nf_prof, sizeof(unsigned long long) * 16) != cudaSuccess) return -1;
-    if (reset) { unsigned long long z[16] = {0}; cudaMemcpyToSymbol(g_nf_prof, z, sizeof(z)); }
-    return 0;
-}
-#endif

@@ -27,23 +27,6 @@ constexpr int G_BN = 64;
 constexpr int G_BK = 32;
 constexpr int G_THREADS = 512;  // 16 warps: the hi/lo split is SIMT work and wants many threads
 
-__device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// round-to-nearest split (cvt.rna.tf32.f32): |x - hi| <= 2^-12 |x| and the rounding of lo costs
-// 2^-24 |x| -- fp32-level and unbiased.  (Masking the low 13 bits instead truncates toward zero.)
-__device__ __forceinline__ float tf32_rn(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
-__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
-    hi = tf32_rn(x);
-    lo = tf32_rn(x - hi);
-}
-__device__ __forceinline__ void split4(const float4 v, float4& hi, float4& lo) {
-    split_tf32(v.x, hi.x, lo.x); split_tf32(v.y, hi.y, lo.y); split_tf32(v.z, hi.z, lo.z); split_tf32(v.w, hi.w, lo.w);
-}
-
 // element (row r, k) of a [ROWS x 32] stage tile lives at float index ((k/4)*ROWS + r)*4 + k%4
 struct Stage {
     float a_hi[G_BM * G_BK], a_lo[G_BM * G_BK], b_hi[G_BN * G_BK], b_lo[G_BN * G_BK];
@@ -131,7 +114,7 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_tf32x3(int M, int N, int 
             st4(st.b_hi + ((bkc0 + i) * G_BN + btile_row) * 4, hi);
             st4(st.b_lo + ((bkc0 + i) * G_BN + btile_row) * 4, lo);
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy smem writes -> visible to the MMA (async proxy)
+        fence_proxy_async();
         __syncthreads();
         const uint32_t ah = s_u32(st.a_hi) + mh * 64 * 16, al = s_u32(st.a_lo) + mh * 64 * 16;
         const uint32_t bh = s_u32(st.b_hi) + nh * 32 * 16, bl = s_u32(st.b_lo) + nh * 32 * 16;

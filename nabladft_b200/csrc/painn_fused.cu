@@ -103,7 +103,6 @@ __global__ void __launch_bounds__(256) k_prep_painn(nb200_painn_weights w, unsig
 
 // ================================================================================================== forward
 struct FwdParams {
-    int xsplit;  // tc_pipe.cuh: activation operands handed over in two K halves
     int n_atoms, do_upd, do_mlp, do_ro;
     const unsigned char* wt;  // prepared weight tiles
     int tile_upd, tile_mlp, tile_ro;  // first tile of the layer updated / of the layer whose message MLP runs / readout forward tile
@@ -142,63 +141,50 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
         }
         if (P.do_ro) prog_add(prog, P.tile_ro, U_NEWX | U_FIRST | U_LAST | U_XLAST);
     }
-    Ctx c = setup(smem, tid, P.xsplit);
-    NF_PROF_DO(const long long tk0_ = clock64(); c.t_last = tk0_;)
-#define NF_BASE 0
+    Ctx<OneGroup> c = setup<OneGroup>(smem, tid);  // every worker warp loads operands and runs epilogues
 
     if (warp >= WARP_ISSUE) {
         run_issuer(c, prog, P.wt);
-        NF_PROF_DO(if (warp == WARP_ISSUE && lane == 0) { atomicAdd(&g_nf_prof[0], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[1], (unsigned long long)c.w_x);
-                   atomicAdd(&g_nf_prof[2], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[3], (unsigned long long)c.w_full); })
     } else {
         const int N = P.n_atoms, A0 = blockIdx.x * NT;
         const int fl = 32 * (warp & 3) + lane;   // my feature inside a 128-row weight tile
-        const int n0 = CPT * (warp >> 2);        // my first atom column
-        const bool isE = role_epi(warp), isL = role_load(warp);  // both true for every worker warp in single-group builds
-        const int ltid = load_tid(tid);
-#define NF_LOAD(...) do { if (isL) load_x(c, ltid, __VA_ARGS__); else ++c.xg; } while (0)
+        const int n0 = OneGroup::CPT * (warp >> 2);  // my first atom column
         if (P.do_upd) {
             // ---- VW[(atom, x)] = mu_mid[(atom, x)] . U^T : V half, W half per cartesian component
 #pragma unroll 1
             for (int x = 0; x < 3; ++x) {
-                NF_LOAD([&](int r, int kc) { return A0 + r < N ? ldg4(P.mu_mid + (size_t)(A0 + r) * (3 * F) + x * F + 4 * kc) : f4(0.f); });
-                NF_MARK(0);
+                load_x(c, tid, [&](int r, int kc) { return A0 + r < N ? ldg4(P.mu_mid + (size_t)(A0 + r) * (3 * F) + x * F + 4 * kc) : f4(0.f); });
 #pragma unroll 1
-                for (int half = 0; half < 2 && isE; ++half) {
+                for (int half = 0; half < 2; ++half) {
                     drain(c, warp);
-                    NF_MARK(1);
                     epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                         float* dst = P.VW + (size_t)(A0 + n0 + 16 * cb) * (6 * F) + x * 2 * F + half * F + fl;
 #pragma unroll
                         for (int j = 0; j < 16; ++j)
                             if (A0 + n0 + 16 * cb + j < N) dst[(size_t)j * (6 * F)] = v[j];
                     });
-                    NF_MARK(21);
                 }
             }
-            NF_MARK(2);
-            if (isE) dep_signal(c, 0);  // VW of this tile is visible to the loader-mapped threads below
+            work_barrier();  // VW of this tile is visible to the threads that read it below
             // ---- g1pre = [q_mid | nrm] . B1^T + d1 as two K = 128 halves summed in the staging columns
-            NF_LOAD([&](int r, int kc) { return A0 + r < N ? ldg4(P.q_mid + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
-            NF_MARK(3);
-            if (isL) {   // while the tensor core works on q_mid: nrm = sqrt(sum_x V_x^2 + eps) and dot = sum_x V_x Wv_x, 2 atoms per round
+            load_x(c, tid, [&](int r, int kc) { return A0 + r < N ? ldg4(P.q_mid + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
+            {   // while the tensor core works on q_mid: nrm = sqrt(sum_x V_x^2 + eps) and dot = sum_x V_x Wv_x, 2 atoms per round
                 // (|V|^2 and <V,Wv> are not kept in registers across the U tiles: 64 persistent registers would spill, and with ~195 KB of
                 //  shared memory per CTA little L1 is left for local memory)
-                dep_wait(c, 0);
-                const int kc = ltid & 31, w = ltid >> 5;
+                const int kc = tid & 31, w = tid >> 5;
 #pragma unroll 1
-                for (int it0 = 0; it0 < RPT; it0 += 2) {
+                for (int it0 = 0; it0 < OneGroup::RPT; it0 += 2) {
                     float4 V[2][3], Wv[2][3];
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
-                        const int a = A0 + w + NLOAD * (it0 + b);
+                        const int a = A0 + w + OneGroup::NLOAD * (it0 + b);
                         const float* vv = P.VW + (size_t)min(a, N - 1) * (6 * F) + 4 * kc;
 #pragma unroll
                         for (int x = 0; x < 3; ++x) { V[b][x] = ld4(vv + x * 2 * F); Wv[b][x] = ld4(vv + x * 2 * F + F); }
                     }
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
-                        const int a = A0 + w + NLOAD * (it0 + b);
+                        const int a = A0 + w + OneGroup::NLOAD * (it0 + b);
                         if (a < N) {
                             float4 sq = V[b][0] * V[b][0]; fma4(sq, V[b][1], V[b][1]); fma4(sq, V[b][2], V[b][2]);
                             float4 dt = f4(0.f); fma4(dt, V[b][0], Wv[b][0]); fma4(dt, V[b][1], Wv[b][1]); fma4(dt, V[b][2], Wv[b][2]);
@@ -208,17 +194,11 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                     }
                 }
             }
-            NF_MARK(4);
-            if (isL) dep_signal(c, 1);  // nrm (read back by the same threads) and dot (read by the y2 epilogue threads) are visible
-            NF_LOAD([&](int r, int kc) { return A0 + r < N ? ld4(P.nrm + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
-            NF_MARK(5);
-            if (isE) drain(c, warp);      // q_mid half: stays in the staging columns
-            NF_MARK(6);
-            NF_MARK(7);
-            if (!isE) ++c.xg;             // the activation operand written by the epilogue group below
-            else {
+            work_barrier();  // nrm (read back by the same threads) and dot (read by the y2 epilogue threads) are visible
+            load_x(c, tid, [&](int r, int kc) { return A0 + r < N ? ld4(P.nrm + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
+            drain(c, warp);  // q_mid half: stays in the staging columns
+            {
                 drain(c, warp, 1);   // + nrm half
-                NF_MARK(8);
                 const float b = __ldg(P.d1 + fl);
                 const XPut xp(c, fl);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {   // operand first: the tensor core restarts before anything is stored
@@ -233,14 +213,12 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                         if (A0 + n0 + 16 * cb + j < N) g[(size_t)j * F] = v[j] + b;
                 });
             }
-            NF_MARK(9);
             // ---- y = silu(g1pre) . B2^T + d2, tiles in the order (gate y1, scalar y0, dot-scale y2)
-            if (isE) {   // y1: mu_next = mu_mid + y1 * Wv   (runs while the tensor core works on the y0 / y2 tiles)
+            {   // y1: mu_next = mu_mid + y1 * Wv   (runs while the tensor core works on the y0 / y2 tiles)
                 drain(c, warp);
-                NF_MARK(10);
                 const float b = __ldg(P.d2 + F + fl);
 #pragma unroll 1
-                for (int cb = 0; cb < CPT / 8; ++cb) {  // 8 atoms per round: 48 loads in flight per thread
+                for (int cb = 0; cb < OneGroup::CPT / 8; ++cb) {  // 8 atoms per round: 48 loads in flight per thread
                     float v16[16];
                     stage_ld16(c, warp, cb >> 1, v16);
                     float tw[8][3], tm[8][3];
@@ -265,10 +243,8 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                     }
                 }
             }
-            NF_MARK(11);
-            if (isE) {   // y0: stored, and q_next <- q_mid + y0 (completed by the y2 tile)
+            {   // y0: stored, and q_next <- q_mid + y0 (completed by the y2 tile)
                 drain(c, warp);
-                NF_MARK(12);
                 const float b = __ldg(P.d2 + fl);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                     float t[16];
@@ -285,12 +261,8 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                     }
                 });
             }
-            NF_MARK(13);
-            if (!isE) ++c.xg;
-            else {   // y2: q_next = (q_mid + y0) + y2 * <V, Wv>; it is the next operand (message MLP of the next layer / readout)
-                dep_wait(c, 1);
+            {   // y2: q_next = (q_mid + y0) + y2 * <V, Wv>; it is the next operand (message MLP of the next layer / readout)
                 drain(c, warp);
-                NF_MARK(14);
                 const float b = __ldg(P.d2 + 2 * F + fl);
                 const XPut xp(c, fl);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
@@ -320,14 +292,11 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 });
             }
         } else {
-            NF_LOAD([&](int r, int kc) { return A0 + r < N ? ldg4(P.q_mlp_in + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
+            load_x(c, tid, [&](int r, int kc) { return A0 + r < N ? ldg4(P.q_mlp_in + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
         }
-        NF_MARK(15);
-        if (P.do_mlp && !isE) ++c.xg;
-        if (P.do_mlp && isE) {
+        if (P.do_mlp) {
             {   // h1pre = q . A1^T + c1 ; silu -> operand (first), then the saved pre-activation
                 drain(c, warp);
-                NF_MARK(16);
                 const float b = __ldg(P.c1 + fl);
                 const XPut xp(c, fl);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
@@ -341,11 +310,9 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                         if (A0 + n0 + 16 * cb + j < N) P.h1pre[(size_t)(A0 + n0 + 16 * cb + j) * F + fl] = v[j] + b;
                 });
             }
-            NF_MARK(17);
 #pragma unroll 1
             for (int ct = 0; ct < 3; ++ct) {  // xh = act . A2^T  (bias c2 is added inside the message kernel)
                 drain(c, warp);
-                NF_MARK(18);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                     float* dst = P.xh + (size_t)(A0 + n0 + 16 * cb) * (3 * F) + ct * F + fl;
 #pragma unroll
@@ -354,8 +321,7 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 });
             }
         }
-        NF_MARK(19);
-        if (P.do_ro && isE) {
+        if (P.do_ro) {
             drain(c, warp);
             epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                 if (fl < F / 2) {
@@ -366,17 +332,11 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 }
             });
         }
-#undef NF_LOAD
     }
-    NF_MARK(20);
-#undef NF_BASE
-    NF_PROF_DO(if (tid == 0) { atomicAdd(&g_nf_prof[4], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[5], (unsigned long long)c.w_acc);
-                            atomicAdd(&g_nf_prof[6], (unsigned long long)c.w_xfree); atomicAdd(&g_nf_prof[7], 1ull); })
 }
 
 // ================================================================================================== backward
 struct BwdParams {
-    int xsplit;
     int n_atoms, do_mlp, do_ro, do_upd;
     const unsigned char* wt;
     int tile_mlp, tile_ro, tile_upd;  // layer whose message MLP is differentiated / readout transposed tile / layer whose update is differentiated
@@ -414,47 +374,38 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
             }
         }
     }
-    Ctx c = setup(smem, tid, P.xsplit);
-    NF_PROF_DO(const long long tk0_ = clock64();)
+    Ctx<OneGroup> c = setup<OneGroup>(smem, tid);  // every worker warp loads operands and runs epilogues
 
     if (warp >= WARP_ISSUE) {
         run_issuer(c, prog, P.wt);
-        NF_PROF_DO(if (warp == WARP_ISSUE && lane == 0) { atomicAdd(&g_nf_prof[8], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[9], (unsigned long long)c.w_x);
-                   atomicAdd(&g_nf_prof[10], (unsigned long long)c.w_buf); atomicAdd(&g_nf_prof[11], (unsigned long long)c.w_full); })
     } else {
         const int N = P.n_atoms, A0 = blockIdx.x * NT;
         const int fl = 32 * (warp & 3) + lane;
-        const int n0 = CPT * (warp >> 2);
-        const bool isE = role_epi(warp), isL = role_load(warp);
-        const int ltid = load_tid(tid);
-#define NF_LOAD(...) do { if (isL) load_x(c, ltid, __VA_ARGS__); else ++c.xg; } while (0)
+        const int n0 = OneGroup::CPT * (warp >> 2);
         if (P.do_mlp) {
             // ---- gt = g_xh . A2 (K = 384) ; gt *= silu'(h1pre) ; gq_b = gq_a + gt . A1
 #pragma unroll 1
             for (int ck = 0; ck < 3; ++ck)
-                NF_LOAD([&](int r, int kc) { return A0 + r < N ? ldg4(P.g_xh + (size_t)(A0 + r) * (3 * F) + ck * F + 4 * kc) : f4(0.f); });
-            if (!isE) ++c.xg;
-            else {
-                drain(c, warp);
-                const XPut xp(c, fl);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float t[16];
+                load_x(c, tid, [&](int r, int kc) { return A0 + r < N ? ldg4(P.g_xh + (size_t)(A0 + r) * (3 * F) + ck * F + 4 * kc) : f4(0.f); });
+            drain(c, warp);
+            const XPut xp(c, fl);
+            epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
+                float t[16];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) t[j] = __ldg(P.h1pre + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
+                for (int j = 0; j < 16; ++j) t[j] = __ldg(P.h1pre + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, A0 + n0 + 16 * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
-                });
-                xp.done(c);
-            }
+                for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, A0 + n0 + 16 * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
+            });
+            xp.done(c);
         } else if (P.do_ro) {
             // ---- gq_b = g_ro . R1 with g_ro[k] = R2[k] silu'(ro_pre[k]), k < F/2 (zero-padded to K = 128)
-            NF_LOAD([&](int r, int kc) {
+            load_x(c, tid, [&](int r, int kc) {
                 if (A0 + r >= N || kc >= F / 8) return f4(0.f);
                 const float4 p = ldg4(P.ro_pre + (size_t)(A0 + r) * (F / 2) + 4 * kc), w2 = ldg4(P.R2 + 4 * kc);
                 return make_float4(w2.x * dsiluf_(p.x), w2.y * dsiluf_(p.y), w2.z * dsiluf_(p.z), w2.w * dsiluf_(p.w));
             });
         }
-        if ((P.do_mlp || P.do_ro) && isE) {  // gq_b = dE/dq_in of the layer above; gdot = gq_b * y2 is what the combine backward needs three times
+        if (P.do_mlp || P.do_ro) {  // gq_b = dE/dq_in of the layer above; gdot = gq_b * y2 is what the combine backward needs three times
             drain(c, warp);
             epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                 float t[16], ty[16];
@@ -476,11 +427,10 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
             });
         }
         if (P.do_upd) {
-            if (isE) dep_signal(c, 0);  // gq_b, gdot visible to the loader-mapped threads
-            if (isL) dep_wait(c, 0);
+            work_barrier();  // gq_b, gdot visible to the threads that load them below
             // ---- gt = gy . B2 (K = 384) with gy = (gq, sum_x cur_x Wv_x, gq <V, Wv>) formed on the fly (combine backward)
-            NF_LOAD([&](int r, int kc) { return A0 + r < N ? ld4(P.gq_b + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
-            NF_LOAD([&](int r, int kc) {
+            load_x(c, tid, [&](int r, int kc) { return A0 + r < N ? ld4(P.gq_b + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f); });
+            load_x(c, tid, [&](int r, int kc) {
                 if (A0 + r >= N) return f4(0.f);
                 const float* vw = P.VW + (size_t)(A0 + r) * (6 * F) + F + 4 * kc;
                 const float* gm = P.cur + (size_t)(A0 + r) * (3 * F) + 4 * kc;
@@ -489,23 +439,20 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
                 for (int x = 0; x < 3; ++x) fma4(sacc, ld4(gm + x * F), ldg4(vw + x * 2 * F));
                 return sacc;
             });
-            NF_LOAD([&](int r, int kc) {
+            load_x(c, tid, [&](int r, int kc) {
                 return A0 + r < N ? ld4(P.gq_b + (size_t)(A0 + r) * F + 4 * kc) * ldg4(P.dot + (size_t)(A0 + r) * F + 4 * kc) : f4(0.f);
             });
-            if (!isE) ++c.xg;
-            else {
-                drain(c, warp);
-                const XPut xp(c, fl);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float t[16];
+            drain(c, warp);
+            const XPut xp(c, fl);
+            epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
+                float t[16];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) t[j] = __ldg(P.g1pre + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
+                for (int j = 0; j < 16; ++j) t[j] = __ldg(P.g1pre + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, A0 + n0 + 16 * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
-                });
-                xp.done(c);
-            }
-            if (isE) {   // gq_a = gq_b + gt . B1[:, :F]   (dE/dq_mid of this layer: what the message backward reads)
+                for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, A0 + n0 + 16 * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
+            });
+            xp.done(c);
+            {   // gq_a = gq_b + gt . B1[:, :F]   (dE/dq_mid of this layer: what the message backward reads)
                 drain(c, warp);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                     float t[16];
@@ -516,7 +463,7 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
                         if (A0 + n0 + 16 * cb + j < N) P.gq_a[(size_t)(A0 + n0 + 16 * cb + j) * F + fl] = t[j] + v[j];
                 });
             }
-            if (isE) {   // gn = gt . B1[:, F:], stored as s = gn / nrm (norm backward: gV_x += s V_x)
+            {   // gn = gt . B1[:, F:], stored as s = gn / nrm (norm backward: gV_x += s V_x)
                 drain(c, warp);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                     float t[16];
@@ -527,26 +474,24 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
                         if (A0 + n0 + 16 * cb + j < N) P.gn[(size_t)(A0 + n0 + 16 * cb + j) * F + fl] = v[j] / t[j];
                 });
             }
-            if (isE) dep_signal(c, 1);  // s visible
-            if (isL) dep_wait(c, 1);
+            work_barrier();  // s visible
             // ---- cur_x += gVW_x . U (K = 256: V chunk then Wv chunk), gVW formed on the fly (combine + norm backward)
 #pragma unroll 1
             for (int x = 0; x < 3; ++x) {
-                NF_LOAD([&](int r, int kc) {  // gV = gdot * Wv + s * V
+                load_x(c, tid, [&](int r, int kc) {  // gV = gdot * Wv + s * V
                     if (A0 + r >= N) return f4(0.f);
                     const size_t a = (size_t)(A0 + r);
                     float4 o = ld4(P.gdot + a * F + 4 * kc) * ldg4(P.VW + a * (6 * F) + x * 2 * F + F + 4 * kc);
                     fma4(o, ld4(P.gn + a * F + 4 * kc), ldg4(P.VW + a * (6 * F) + x * 2 * F + 4 * kc));
                     return o;
                 });
-                NF_LOAD([&](int r, int kc) {  // gWv = cur_x * y1 + gdot * V
+                load_x(c, tid, [&](int r, int kc) {  // gWv = cur_x * y1 + gdot * V
                     if (A0 + r >= N) return f4(0.f);
                     const size_t a = (size_t)(A0 + r);
                     float4 o = ld4(P.cur + a * (3 * F) + x * F + 4 * kc) * ldg4(P.y + a * (3 * F) + F + 4 * kc);
                     fma4(o, ld4(P.gdot + a * F + 4 * kc), ldg4(P.VW + a * (6 * F) + x * 2 * F + 4 * kc));
                     return o;
                 });
-                if (isE) {
                 drain(c, warp);
                 epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
                     float t[16];
@@ -556,13 +501,9 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
                     for (int j = 0; j < 16; ++j)
                         if (A0 + n0 + 16 * cb + j < N) P.cur[(size_t)(A0 + n0 + 16 * cb + j) * (3 * F) + x * F + fl] = t[j] + v[j];
                 });
-                }
             }
         }
-#undef NF_LOAD
     }
-    NF_PROF_DO(if (tid == 0) { atomicAdd(&g_nf_prof[12], (unsigned long long)(clock64() - tk0_)); atomicAdd(&g_nf_prof[13], (unsigned long long)c.w_acc);
-                            atomicAdd(&g_nf_prof[14], (unsigned long long)c.w_xfree); atomicAdd(&g_nf_prof[15], 1ull); })
 }
 
 template <class K>
@@ -571,19 +512,6 @@ int set_smem(K kernel) {
 }
 
 }  // namespace
-
-#ifdef NF_PROF
-extern "C" int nb200_debug_nf_prof(unsigned long long* out16, int reset) {
-    if (cudaMemcpyFromSymbol(out16, g_nf_prof, sizeof(unsigned long long) * 16) != cudaSuccess) return -1;
-    if (reset) { unsigned long long z[16] = {0}; cudaMemcpyToSymbol(g_nf_prof, z, sizeof(z)); }
-    return 0;
-}
-extern "C" int nb200_debug_nf_phase(unsigned long long* out64, int reset) {
-    if (cudaMemcpyFromSymbol(out64, g_nf_phase, sizeof(unsigned long long) * 64) != cudaSuccess) return -1;
-    if (reset) { unsigned long long z[64] = {0}; cudaMemcpyToSymbol(g_nf_phase, z, sizeof(z)); }
-    return 0;
-}
-#endif
 
 int64_t nb_fused_wtile_bytes(int n_layers) { return (int64_t)(n_layers * TILES_PER_LAYER + 2) * WTILE_BYTES; }
 
@@ -597,9 +525,8 @@ int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s) {
     static bool attr = false;
     if (!attr) { if (set_smem(k_node_fwd) != NB200_OK) return NB200_ECUDA; attr = true; }
     FwdParams P{};
-    // Whole-operand hand-over: the two-K-halves protocol of tc_pipe.cuh (xsplit, used by the pre-split-weight GEMM for K > 128) measured neutral
-    // here (122.4 k vs 122.8 k molecules/s): most operands of these kernels are written by the previous GEMM's epilogue, which it cannot start earlier.
-    P.xsplit = 0;
+    // One worker group, whole-operand hand-over: the K-halves hand-over of tc_pipe.cuh's two-group layout gains nothing here, because most
+    // operands of these kernels are written by the previous GEMM's epilogue, which cannot start earlier.
     P.n_atoms = a.n_atoms; P.do_upd = a.layer_upd >= 0; P.do_mlp = a.layer_mlp >= 0; P.do_ro = a.readout;
     P.wt = static_cast<const unsigned char*>(a.wtiles);
     P.tile_upd = a.layer_upd * TILES_PER_LAYER; P.tile_mlp = a.layer_mlp * TILES_PER_LAYER; P.tile_ro = a.n_layers * TILES_PER_LAYER;
@@ -615,7 +542,6 @@ int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s) {
     static bool attr = false;
     if (!attr) { if (set_smem(k_node_bwd) != NB200_OK) return NB200_ECUDA; attr = true; }
     BwdParams P{};
-    P.xsplit = 0;  // as in nb_fused_node_fwd
     P.n_atoms = a.n_atoms; P.do_mlp = a.layer_mlp >= 0; P.do_ro = a.readout; P.do_upd = a.layer_upd >= 0;
     P.wt = static_cast<const unsigned char*>(a.wtiles);
     P.tile_mlp = a.layer_mlp * TILES_PER_LAYER; P.tile_ro = a.n_layers * TILES_PER_LAYER + 1; P.tile_upd = a.layer_upd * TILES_PER_LAYER;

@@ -15,6 +15,7 @@
 //   forward : N*10F*4 + E*(3F*4 + 20)           = 5120 N + 1556 E
 //   backward: N*16F*4 + E*(6F*4 + 32)           = 8192 N + 3104 E
 #include "common.cuh"
+#include "wgmma.cuh"
 
 // One warp per CTA (16 CTAs per SM): a CTA's shared memory and registers return to the SM as soon as ITS atom is done.  With 8 warps per
 // CTA the slot was held until the slowest of 8 atoms (degrees 15..40) finished.
@@ -46,32 +47,6 @@ __device__ __forceinline__ float4 lds4(const float* p) { return *reinterpret_cas
 #define FWD_WROW (3 * NB_F)
 #define FWD_GROW (6 * NB_F)
 #define FWD_WARP_FLOATS (FWD_WS * FWD_WROW + FWD_GS * FWD_GROW)
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(float* dst, const float* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src),
-                 "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        "@P1 bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
 
 __device__ __forceinline__ void fwd_gather_issue(float* dst, const float* xrow, const float* mrow) {
     cp_async16(dst, xrow); cp_async16(dst + NB_F, xrow + NB_F); cp_async16(dst + 2 * NB_F, xrow + 2 * NB_F);

@@ -1,9 +1,50 @@
-// wgmma.cuh -- the Hopper (sm_90a) warpgroup MMA helpers shared by the tensor-core kernels: shared-memory matrix descriptors for the
-// canonical no-swizzle K-major layout (8 rows x 16 bytes per core matrix), fences / commit / wait, and m64nNk8 TF32 MMAs with an fp32
-// accumulator fragment in registers.  Fragment layout of m64nNk8 (thread t of warp w of the warpgroup): d[4j + 0, 1] = row 16 w + t / 4,
-// columns 8 j + 2 (t % 4) + {0, 1}; d[4j + 2, 3] = row 16 w + t / 4 + 8, same columns.
+// wgmma.cuh -- the Hopper (sm_90a) primitives shared by the tensor-core and bulk-copy kernels: the 3xTF32 operand split, mbarriers,
+// cp.async.bulk, the async-proxy fence, shared-memory matrix descriptors for the canonical no-swizzle K-major layout (8 rows x 16 bytes per
+// core matrix), wgmma fences / commit / wait, and m64nNk8 TF32 MMAs with an fp32 accumulator fragment in registers.  Fragment layout of
+// m64nNk8 (thread t of warp w of the warpgroup): d[4j + 0, 1] = row 16 w + t / 4, columns 8 j + 2 (t % 4) + {0, 1}; d[4j + 2, 3] =
+// row 16 w + t / 4 + 8, same columns.
 #pragma once
 #include <cstdint>
+
+__device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// round-to-nearest split (cvt.rna.tf32.f32): |x - hi| <= 2^-12 |x| and the rounding of lo costs
+// 2^-24 |x| -- fp32-level and unbiased.  (Masking the low 13 bits instead truncates toward zero.)
+__device__ __forceinline__ float tf32_rn(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return __uint_as_float(r);
+}
+__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
+    hi = tf32_rn(x);
+    lo = tf32_rn(x - hi);
+}
+__device__ __forceinline__ void split4(const float4 v, float4& hi, float4& lo) {
+    split_tf32(v.x, hi.x, lo.x); split_tf32(v.y, hi.y, lo.y); split_tf32(v.z, hi.z, lo.z); split_tf32(v.w, hi.w, lo.w);
+}
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    asm volatile(
+        "{\n.reg .pred P1;\nLAB_WAIT:\nmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n@P1 bra DONE;\nbra LAB_WAIT;\nDONE:\n}\n" ::"r"(
+            s_u32(bar)),
+        "r"(parity)
+        : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(bar)) : "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s_u32(bar)), "r"(bytes) : "memory");
+}
+// global -> shared bulk copy (TMA engine), completion counted in bytes on `bar`
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(s_u32(dst)), "l"(src), "r"(bytes),
+                 "r"(s_u32(bar))
+                 : "memory");
+}
+// shared-memory writes of this thread (generic proxy) become visible to the async proxy: wgmma operand reads, bulk copies
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // start >> 4 [0,14) | LBO >> 4 [16,30) (stride between the 16-byte k-chunks) | SBO >> 4 [32,46) (stride between 8-row groups) | no swizzle
 __device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {

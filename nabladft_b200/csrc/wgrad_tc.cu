@@ -17,7 +17,8 @@
 // terms that carry it (column `in` of D = column sums of G).  Four warpgroups: outputs [64 (g & 1), +64) x B columns [72 (g >> 1), +72).
 // Epilogue: registers -> shared-memory staging -> row-contiguous red.global.add.v4.f32 into the gradient bucket.  The sum over atom chunks
 // is therefore atomic (fp32 addition order varies from run to run at the 1e-7 relative level; cuBLAS split-K was deterministic).
-#include "tc_pipe.cuh"
+#include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -124,7 +125,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const WgParams P) {
                 *reinterpret_cast<float4*>(sb + 2 * WG_A_BYTES + hl * WG_B_BYTES + kc * WG_B_LBO + (16 + (r >> 3)) * WG_SBO + (r & 7) * 16) =
                     make_float4(one, one, one, one);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             __syncthreads();
             const uint32_t sa = s_u32(sb) + mh * 8 * WG_SBO, sbb = s_u32(sb) + 2 * WG_A_BYTES + nh * 9 * WG_SBO;
             wgmma_fence();

@@ -13,7 +13,7 @@ ALLOWED = {
     "NB200_TRAIN_STORAGE",   # default per-edge storage of the training arrays (a precision choice, INTEGRATION.md)
     "NB200_QH_PAIR_CHUNK",   # QHNet memory bound: atom pairs whose path weights exist at a time
     "NVCC",                  # build: compiler
-    "NB200_NVCC_EXTRA",      # build: extra flags (e.g. -DNF_PROF for the pipeline role timing tools)
+    "NB200_NVCC_EXTRA",      # build: extra flags
 }
 
 C_READ = re.compile(r"\bgetenv\s*\(")
