@@ -122,7 +122,8 @@ int nb200_edge_forces(const float* egrad, const float* geom, const int32_t* row_
  * Whole-model engine: PaiNN energy + forces for one batch of conformations.
  * Replaces `NeuralNetworkPotential.forward` for config/model/painn.yaml (spk roles) and
  * `PaiNN.forward` (nablaDFT/painn_pyg/painn.py:89-148) for config/model/painn-oc.yaml.
- * Node-level dense layers are plain library GEMMs (cuBLAS, fp32, no TF32).
+ * The node forward runs as fused per-layer wgmma kernels; the other node-level dense layers run on the wgmma 3xTF32 GEMM
+ * (fp32-accurate).
  * -------------------------------------------------------------------------------------- */
 typedef struct nb200_painn_weights {
     int32_t n_layers, n_feat, n_rbf, n_elem; /* L, F(=128), K(=100), rows of emb            */
@@ -149,18 +150,18 @@ typedef struct nb200_engine nb200_engine;
 int nb200_engine_create(nb200_engine** out);
 int nb200_engine_destroy(nb200_engine* eng);
 /* Optional per-category CUDA-event timing of the engine's launches (bench.py roofline leg).
- * Categories: 0 neighbour build, 1 radial filters, 2 embedding, 3 cuBLAS GEMMs, 4 node
+ * Categories: 0 neighbour build, 1 radial filters, 2 embedding, 3 node GEMMs, 4 node
  * elementwise, 5 message fwd, 6 message bwd, 7 readout, 8 force assembly.
  * read_timings synchronises on the recorded events, sums elapsed ms per category and resets. */
 int nb200_engine_set_timing(nb200_engine* eng, int32_t enable);
 int nb200_engine_read_timings(nb200_engine* eng, float* ms_per_cat, int32_t* scopes_per_cat, int32_t n_cat);
-/* Node-level dense layers: 1 (default) = hand-written wgmma 3xTF32 GEMM (fp32-accurate),
- * 0 = cuBLAS SGEMM (kept for A/B comparison). */
+/* Node-level dense layers: the hand-written wgmma 3xTF32 GEMM (fp32-accurate) is the only backend.
+ * 1 -> NB200_OK; 0 (the former cuBLAS SGEMM backend) -> NB200_EUNSUPPORTED; anything else -> NB200_EINVAL. */
 int nb200_engine_set_gemm_backend(nb200_engine* eng, int32_t backend);
-/* PaiNN inference, per-atom part of a layer (PaiNNUpdate.forward painn.py:535-548, x_proj painn.py:459-464, out_energy[0]
- * painn.py:79-83 and their backward): 1 (default) = ONE fused wgmma kernel per layer and direction (painn_fused.cu: weights
- * pre-split into TF32 hi/lo shared-memory images, chained MMAs, elementwise glue in loaders / epilogues),
- * 0 = one launch per Linear / elementwise op (the round-1 sequence; also what the training step uses). */
+/* PaiNN per-atom part of a layer (PaiNNUpdate.forward painn.py:535-548, x_proj painn.py:459-464, out_energy[0]
+ * painn.py:79-83 and their backward): ONE fused wgmma kernel per layer and direction (painn_fused.cu: weights pre-split into
+ * TF32 hi/lo shared-memory images, chained MMAs, elementwise glue in loaders / epilogues) is the only node forward.
+ * 1 -> NB200_OK; 0 (the former one-launch-per-op sequence) -> NB200_EUNSUPPORTED; anything else -> NB200_EINVAL. */
 int nb200_engine_set_node_backend(nb200_engine* eng, int32_t backend);
 /* C[M,N] = A[M,K] . op(B) (+C) (+bias), optional act = silu(C); fp32 in/out, 3xTF32 on wgmma.
  * op(B) = B[N,K]^T (trans_b=0, torch.nn.Linear forward: nablaDFT/painn_pyg/painn.py:459-464)

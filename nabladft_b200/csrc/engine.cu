@@ -7,11 +7,11 @@
 // here the backward is hand-derived and runs as the mirrored kernel sequence on one stream,
 // with no host synchronisation anywhere (edge count and error flags stay on the device).
 //
-// Node-level dense layers ([N,128]x[128,384] etc.) run on the wgmma 3xTF32 GEMM of gemm_tc.cu (fp32-accurate: the reference never
-// uses reduced precision, SURVEY.md section 0.9); cuBLAS SGEMM stays selectable (nb200_engine_set_gemm_backend).  The weight gradients of
-// the training step run on the wgmma split-K kernel of wgrad_tc.cu.
-// `run_painn` is the one orchestration for inference, the energy-seeded parameter gradients (painn_train.cu) and the force-loss tangent
-// pass (painn_tangent.cu).
+// The node forward is the fused per-layer kernels of painn_fused.cu; the remaining node-level dense layers (tangent pass, training and
+// Hessian backward) run on the wgmma 3xTF32 GEMM of gemm_tc.cu (fp32-accurate: the reference never uses reduced precision, SURVEY.md
+// section 0.9).  The weight gradients of the training step run on the wgmma split-K kernel of wgrad_tc.cu.
+// Every entry point is a short sequence of the same steps: graph + filters, the fused forward (`run_painn_fused`), the tangent forward
+// (`tangent_fwd`, painn_tangent.cu), and the training backward (`train_bwd`, painn_train.cu) or the Hessian backward (`run_painn_hvp`).
 #include <new>
 #include <utility>
 
@@ -43,16 +43,16 @@ extern "C" int nb200_engine_set_timing(nb200_engine* eng, int32_t enable) {
     return NB200_OK;
 }
 
+// The node GEMMs are the wgmma kernels and the PaiNN node forward is the fused one: both setters accept 1 and refuse 0 (the cuBLAS SGEMM /
+// one-launch-per-op paths, which no longer exist) with NB200_EUNSUPPORTED.
 extern "C" int nb200_engine_set_gemm_backend(nb200_engine* eng, int32_t backend) {
     if (!eng || (backend != 0 && backend != 1)) return NB200_EINVAL;
-    eng->gemm_backend = backend;
-    return NB200_OK;
+    return backend == 1 ? NB200_OK : NB200_EUNSUPPORTED;
 }
 
 extern "C" int nb200_engine_set_node_backend(nb200_engine* eng, int32_t backend) {
     if (!eng || (backend != 0 && backend != 1)) return NB200_EINVAL;
-    eng->node_backend = backend;
-    return NB200_OK;
+    return backend == 1 ? NB200_OK : NB200_EUNSUPPORTED;
 }
 
 // Storage of the per-edge arrays of the PaiNN TRAINING calls (nb200_painn_energy_forces_grads, nb200_painn_train_forward / _backward):
@@ -108,21 +108,21 @@ struct Workspace {
     float *h1pre[kMaxLayers], *xh[kMaxLayers], *VW[kMaxLayers], *nrm[kMaxLayers], *g1pre[kMaxLayers], *y[kMaxLayers];
     float* mu[kMaxLayers + 1];
     // transient
-    float *q, *act, *ro_pre, *eps;
+    float *ro_pre, *eps;
     // backward
     float *gq, *gmu_a, *gmu_b, *gy, *gVW, *gt, *gn, *g_ro, *egrad;
-    // training only: layer inputs that the in-place forward overwrites, activation scratch, per-edge filter gradients
-    float *q_in[kMaxLayers], *q_mid[kMaxLayers], *mu_mid[kMaxLayers], *act_t, *gW, *seed_atom;
+    // training only: activation scratch, per-edge filter gradients, per-atom energy seed
+    float *act_t, *gW, *seed_atom;
     // force-loss tangent pass (painn_tangent.cu): t_X = directional derivative of X along the position-space direction v
     float *t_geom, *t_h1[kMaxLayers], *t_xh[kMaxLayers], *t_VW[kMaxLayers], *t_nrm[kMaxLayers], *t_g1[kMaxLayers], *t_y[kMaxLayers];
     float *t_q_in[kMaxLayers], *t_q_mid[kMaxLayers], *t_mu_mid[kMaxLayers], *t_mu[kMaxLayers + 1];
     float *t_q, *t_act, *t_ro, *t_gq, *t_gmu_a, *t_gmu_b, *t_gy, *t_gVW, *t_gt, *t_gn, *t_g_ro, *t_gW, *gWd;
     // Hessian-vector product (run_painn_hvp): d2W/dd2 rows [L][E][3F] next to W, dW; tangent of the per-edge geometric gradient
     float *d2W, *t_egrad;
-    // fused node path (painn_fused.cu): per-layer inputs / post-message states instead of in-place q, mu; prepared weight tiles
+    // fused node forward (painn_fused.cu): layer inputs fq_in[l] and post-message states fq_mid[l], fmu_mid[l] (mu[l + 1] is the layer's
+    // output); the training backward reads them as the Linear inputs.  Prepared weight tiles.
     float *fq_in[kMaxLayers + 1], *fq_mid[kMaxLayers], *fmu_mid[kMaxLayers], *fdot[kMaxLayers], *gq_b, *fgn, *fgdot;
     void* wtiles;
-    void* blas_ws;
     int64_t bytes;
 };
 
@@ -138,7 +138,7 @@ Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool for
     w.deg = c.take<int32_t>(N);
     w.sort_scr = c.take<int32_t>(E + 1024);
     w.geom = c.take<float>(4 * E);
-    // filters: [L][E][3F] W and the same for dW/dd (adjacent), or -- fused inference path -- ONE array [L][E][6F] of [W | dW/dd] records over
+    // filters: [L][E][3F] W and the same for dW/dd (adjacent), or -- inference with forces -- ONE array [L][E][6F] of [W | dW/dd] records over
     // the same memory
     w.W = c.take<float>((int64_t)L * E * 3 * F * (forces ? 2 : 1));
     w.dW = forces ? w.W + (int64_t)L * E * 3 * F : nullptr;
@@ -151,8 +151,6 @@ Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool for
         w.y[l] = c.take<float>(N * 3 * F);
     }
     for (int l = 0; l <= L; ++l) w.mu[l] = c.take<float>(N * 3 * F);
-    w.q = c.take<float>(N * F);
-    w.act = c.take<float>(N * F);
     w.ro_pre = c.take<float>(N * (F / 2));
     w.eps = c.take<float>(N);
     if (forces) {
@@ -167,7 +165,6 @@ Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool for
         w.egrad = c.take<float>(4 * E);
     }
     if (train) {
-        for (int l = 0; l < L; ++l) { w.q_in[l] = c.take<float>(N * F); w.q_mid[l] = c.take<float>(N * F); w.mu_mid[l] = c.take<float>(N * 3 * F); }
         w.act_t = c.take<float>(N * F);
         w.gW = c.take<float>(E * 3 * F);
         w.seed_atom = c.take<float>(N);
@@ -206,7 +203,6 @@ Workspace carve(void* p, int L, int F, int64_t B, int64_t N, int64_t E, bool for
     w.fgn = forces ? c.take<float>(N * F) : nullptr;
     w.fgdot = forces ? c.take<float>(N * F) : nullptr;
     w.wtiles = c.take<char>(nb_fused_wtile_bytes(L));
-    w.blas_ws = c.take<char>(kBlasWs);
     w.bytes = (c.off + kAlign - 1) / kAlign * kAlign;
     return w;
 }
@@ -233,18 +229,46 @@ bool grads_ok(const nb200_painn_weights* g) {
            g->R2 && g->e2 && al(g->A1) && al(g->A2) && al(g->U) && al(g->B1) && al(g->B2) && al(g->R1);
 }
 
-// Inference (E + analytic F) with the fused node kernels of painn_fused.cu: per layer ONE message kernel and ONE node kernel per direction.
-// The graph and the radial filters are already in the workspace.  Same arithmetic as the unfused sequence below (which stays selectable with
-// nb200_engine_set_node_backend(eng, 0) and carries the training step), except that q / mu are not updated in place: layer l reads
-// fq_in[l], mu[l], the message kernel writes fq_mid[l], fmu_mid[l], the node kernel writes fq_in[l+1], mu[l+1].
-// `records` = false (kept training forward): full filter rows in two separate arrays W / dW, the layout the gradient kernels read.
+// Argument checks every PaiNN entry point makes after its own, before anything is launched.
+int args_ok(const nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const int32_t* mol_ptr, int32_t n_mol, int32_t n_atoms,
+            int32_t e_cap, const void* workspace, const int32_t* status) {
+    if (!eng || !weights_ok(w) || !z || !mol_ptr || !workspace || !status) return NB200_EINVAL;
+    if (w->n_feat != NB_F || w->n_layers <= 0 || w->n_layers > kMaxLayers) return NB200_EUNSUPPORTED;
+    if (n_mol <= 0 || n_atoms <= 0 || e_cap <= 0) return NB200_EINVAL;
+    return NB200_OK;
+}
+
+// Neighbour graph and radial filters (painn.py:104-108 / spk PairwiseDistances + filter_net).  W depends on the distance only (rows of e and
+// rev[e] are bitwise equal), so ONE filter row is stored per undirected pair and edge e reads row min(e, rev[e]): half the filter kernel's
+// work and writes; the second reader of a row mostly finds it in L2.  `records` (inference with forces): one interleaved [W | dW/dd] record
+// per row, one bulk copy per edge in the backward; otherwise W and dW/dd in two arrays, the layout the gradient kernels read.  `train` adds
+// the bin sort over every directed edge that the filter weight gradients walk (slot e holds the gradient of the opposite edge's row).
+int graph_and_filters(nb200_engine* eng, const nb200_painn_weights* w, const Workspace& ws, const float* pos, const int32_t* mol_ptr, int32_t n_mol,
+                      int N, int32_t e_cap, int32_t* status, cudaStream_t s, bool records, bool train) {
+    const int K = w->n_rbf;
+    const int bf16 = train ? eng->edge_bf16 : 0;  // bf16 rows use the first half of their fp32-sized blocks: all offsets stay in floats
+    { Scope sc(eng, s, CAT_NBR, 3);
+    NB_TRY(nb200_neighbor_build(pos, mol_ptr, n_mol, N, w->cutoff, w->max_neighbors, e_cap, ws.row_ptr, ws.col, ws.rev, ws.geom, ws.deg,
+                                status, s)); }
+    { Scope sc(eng, s, CAT_FILTER, 4);
+    NB_TRY(nb_painn_filter_ex(ws.geom, status, e_cap, w->w_rbf, w->b_rbf, w->n_layers, K, NB_F, w->radial_mode, w->cutoff, w->rbf_offsets,
+                              w->rbf_coeff, w->rbf_xscale, ws.W, ws.dW, ws.sort_scr, ws.rev, records ? 1 : 0, s, bf16)); }
+    if (!train) return NB200_OK;
+    const float dx = (w->cutoff * w->rbf_xscale) / (float)(K - 1);
+    Scope sc(eng, s, CAT_FILTER, 3);
+    return nb_bin_sort(ws.geom, status, w->rbf_xscale, 1.0f / dx, K, ws.sort_scr2, s, nullptr);
+}
+
+// The node forward (E, and with `forces` the analytic F) with the fused node kernels of painn_fused.cu: per layer ONE message kernel and
+// ONE node kernel per direction.  The graph and the radial filters are already in the workspace.  q / mu are not updated in place: layer l
+// reads fq_in[l], mu[l], the message kernel writes fq_mid[l], fmu_mid[l], the node kernel writes fq_in[l+1], mu[l+1]; every activation is
+// written whether or not forces are asked for, so the tangent pass and the training / Hessian backward read them afterwards.
+// `records` = false (training, Hessian): full filter rows in two separate arrays W / dW, the layout the gradient kernels read.
 int run_painn_fused(nb200_engine* eng, const nb200_painn_weights* w, const Workspace& ws, const int32_t* z, const int32_t* mol_ptr, int32_t n_mol,
-                    int N, int32_t e_cap, float* energy, float* forces, int32_t* status, cudaStream_t s, bool records = true, int bf16 = 0,
-                    bool half_rows_sep = false) {
+                    int N, int32_t e_cap, float* energy, float* forces, int32_t* status, cudaStream_t s, bool records, int bf16) {
     const int L = w->n_layers, F = NB_F;
     const int w_stride = (forces && records) ? 6 * F : 3 * F;    // [W | dW/dd] records when the backward runs
     const size_t wl_stride = (size_t)e_cap * w_stride;
-    const int32_t* w_rev = (records || half_rows_sep) ? ws.rev : nullptr;  // one stored row per undirected pair / one row per edge
     const float* dW0 = records ? ws.W + 3 * F : ws.dW;
     { Scope sc(eng, s, CAT_EMBED, 1); NB_TRY(nb_embed(z, w->emb, w->z_offset, w->n_elem, N, ws.fq_in[0], ws.mu[0], status, s)); }
     { Scope sc(eng, s, CAT_GEMM, 1); NB_TRY(nb_fused_prep(w, ws.wtiles, s)); }
@@ -258,7 +282,7 @@ int run_painn_fused(nb200_engine* eng, const nb200_painn_weights* w, const Works
     }
     for (int l = 0; l < L; ++l) {
         { Scope sc(eng, s, CAT_MSG_FWD, 1);
-        NB_TRY(nb_painn_msg_fwd_ex(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.fq_in[l], ws.mu[l], ws.W + l * wl_stride, w_stride, w_rev, ws.geom,
+        NB_TRY(nb_painn_msg_fwd_ex(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.fq_in[l], ws.mu[l], ws.W + l * wl_stride, w_stride, ws.rev, ws.geom,
                                    ws.row_ptr, ws.col, N, ws.fq_mid[l], ws.fmu_mid[l], s, bf16)); }
         const bool last = l + 1 == L;
         f.layer_upd = l; f.layer_mlp = last ? -1 : l + 1; f.readout = last ? 1 : 0;
@@ -287,7 +311,7 @@ int run_painn_fused(nb200_engine* eng, const nb200_painn_weights* w, const Works
         { Scope sc(eng, s, CAT_GEMM, 1); NB_TRY(nb_fused_node_bwd(b, s)); }
         { Scope sc(eng, s, CAT_MSG_BWD, 1);
         NB_TRY(nb_painn_msg_bwd_ex(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.W + l * wl_stride, dW0 + l * wl_stride, w_stride,
-                                   w_rev, ws.geom, ws.row_ptr, ws.col, N, ws.gq, cur, ws.gy, other, ws.egrad, s, bf16)); }
+                                   ws.rev, ws.geom, ws.row_ptr, ws.col, N, ws.gq, cur, ws.gy, other, ws.egrad, s, bf16)); }
         float* t = cur; cur = other; other = t;
         // layer 0: the embedding does not depend on positions, nothing below the message kernel is needed for forces
     }
@@ -296,126 +320,54 @@ int run_painn_fused(nb200_engine* eng, const nb200_painn_weights* w, const Works
     return NB200_OK;
 }
 
-// `grads` != nullptr: training step -- also writes d(sum_m seed_m E_m)/d(weights) into the arrays `grads` points to (same layout as the
-// weights; overwritten) -- see painn_train.cu.  Forces stay the true, unweighted -dE/dR.
-int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr, int32_t n_mol,
-              int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes, float* energy, float* forces, int32_t* status,
-              void* stream, const float* seed_mol, const nb200_painn_weights* grads, const float* v_dir = nullptr, int phase = 0,
-              bool carve_tangent = false) {
-    // phase 0: one call (inference, or the whole training step).  Training split over two calls on the SAME workspace (the forward is not
-    // recomputed): phase 1 = graph + filters + fused forward + fused force backward, every activation the gradient pass reads stays in the
-    // training workspace; phase 2 = tangent pass + backward with the weight gradients from those kept arrays.
-    if (!eng || !weights_ok(w) || !z || !mol_ptr || !workspace || !status) return NB200_EINVAL;
-    if (phase != 2 && (!pos || !energy)) return NB200_EINVAL;
-    const bool train = grads != nullptr || phase == 1;
-    if (phase != 1 && train && !grads_ok(grads)) return NB200_EINVAL;
-    if (phase != 2 && train && !forces) return NB200_EINVAL;
-    if (w->n_feat != NB_F || w->n_layers <= 0 || w->n_layers > kMaxLayers) return NB200_EUNSUPPORTED;
-    if (n_mol <= 0 || n_atoms <= 0 || e_cap <= 0) return NB200_EINVAL;
-    const int L = w->n_layers, F = NB_F, K = w->n_rbf, N = n_atoms;
-    const bool want_f = forces != nullptr || phase == 2;
-    const bool tan = train && v_dir != nullptr;
-    Workspace ws = carve(workspace, L, F, n_mol, N, e_cap, want_f, train, phase ? carve_tangent : tan);
-    if (ws.bytes > workspace_bytes) return NB200_EINVAL;
-    if (phase == 2) {  // the fused forward of phase 1 left layer inputs / post-message states in its own arrays: same values, other names
-        for (int l = 0; l < L; ++l) { ws.q_in[l] = ws.fq_in[l]; ws.q_mid[l] = ws.fq_mid[l]; ws.mu_mid[l] = ws.fmu_mid[l]; }
-        ws.q = ws.fq_in[L];
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    cublasHandle_t h = eng->blas;
-    NB_BLAS(cublasSetStream(h, s) == CUBLAS_STATUS_SUCCESS);
-    NB_BLAS(cublasSetWorkspace(h, ws.blas_ws, kBlasWs) == CUBLAS_STATUS_SUCCESS);
-
-    const size_t wl_stride = (size_t)e_cap * 3 * F;
-    const int bf16 = train ? eng->edge_bf16 : 0;  // bf16 rows use the first half of their fp32-sized blocks: all offsets below stay in floats
-    // training, like inference, stores ONE filter row (W and dW/dd, two arrays here) per undirected pair: edge e reads row min(e, rev[e]).  Half the filter
-    // kernel's work and writes; the second reader of a row mostly finds it in L2.
-    const int32_t* t_rev = train ? ws.rev : nullptr;
-    if (phase != 2) {
-    // ---- graph + radial filters (painn.py:104-108 / spk PairwiseDistances + filter_net)
-    { Scope sc(eng, s, CAT_NBR, 3);
-    NB_TRY(nb200_neighbor_build(pos, mol_ptr, n_mol, N, w->cutoff, w->max_neighbors, e_cap, ws.row_ptr, ws.col, ws.rev, ws.geom, ws.deg,
-                                status, s)); }
-    // fused inference path: ONE filter row per undirected pair (W depends on the distance only: rows of e and rev[e] are bitwise equal), and
-    // with forces one interleaved [W | dW/dd] record per row -- half the filter work and HBM writes, one bulk copy per edge in the backward
-    const bool half_rows = eng->node_backend == 1 && !train;
-    { Scope sc(eng, s, CAT_FILTER, 4);
-    NB_TRY(nb_painn_filter_ex(ws.geom, status, e_cap, w->w_rbf, w->b_rbf, L, K, F, w->radial_mode, w->cutoff, w->rbf_offsets, w->rbf_coeff,
-                              w->rbf_xscale, ws.W, ws.dW, ws.sort_scr, (half_rows || train) ? ws.rev : nullptr, half_rows && want_f ? 1 : 0, s, bf16)); }
-    if (train) {  // the filter weight gradients still walk every directed edge (slot e holds the gradient of the opposite edge's row): their own sort
-        const float dx = (w->cutoff * w->rbf_xscale) / (float)(K - 1);
-        Scope sc(eng, s, CAT_FILTER, 3);
-        NB_TRY(nb_bin_sort(ws.geom, status, w->rbf_xscale, 1.0f / dx, K, ws.sort_scr2, s, nullptr));
-    }
-    if (eng->node_backend == 1 && !train) return run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s);
-    if (phase == 1) return run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s, false, bf16, true);
-    // ---- embedding (painn.py:110-111)
-    { Scope sc(eng, s, CAT_EMBED, 1); NB_TRY(nb_embed(z, w->emb, w->z_offset, w->n_elem, N, ws.q, ws.mu[0], status, s)); }
-
+// Tangent forward along the position-space direction v (painn_tangent.cu): the directional derivative of every saved activation of the fused
+// forward (weights carry no tangent).  The message and the update add to t_q and t_mu[l + 1] in place; `keep_inputs` keeps the values the
+// Linear layers saw (t_q_in, t_q_mid, t_mu_mid) for the weight gradients of the training step -- the Hessian does not read them.
+// The caller opens the timing scope (1 + 6 L own launches besides the GEMMs).
+int tangent_fwd(nb200_engine* eng, const nb200_painn_weights* w, const Workspace& ws, const float* v, int N, int32_t e_cap, int bf16, bool keep_inputs,
+                cudaStream_t s) {
+    const int L = w->n_layers, F = NB_F;
+    const size_t wl = (size_t)e_cap * 3 * F;
+    NB_TRY(nb_geom_tan(ws.geom, ws.row_ptr, ws.col, v, N, ws.t_geom, s));
+    if (cudaMemsetAsync(ws.t_q, 0, (size_t)N * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();        // embedding: no tangent
+    if (cudaMemsetAsync(ws.t_mu[0], 0, (size_t)N * 3 * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();
     for (int l = 0; l < L; ++l) {
         const float* A1 = w->A1 + (size_t)l * F * F;
         const float* A2 = w->A2 + (size_t)l * 3 * F * F;
         const float* U = w->U + (size_t)l * 2 * F * F;
         const float* B1 = w->B1 + (size_t)l * F * 2 * F;
         const float* B2 = w->B2 + (size_t)l * 3 * F * F;
-        // message (painn.py:475-509): xh = MLP(q); q,mu += segmented sums
-        if (train && cudaMemcpyAsync(ws.q_in[l], ws.q, (size_t)N * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess) return nb_check_launch();
-        NB_TRY(linear_fwd(eng, s, N, F, F, ws.q, F, A1, F, ws.h1pre[l], F, false, w->c1 + (size_t)l * F, ws.act));
-        NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.act, F, A2, F, ws.xh[l], 3 * F, false, nullptr, nullptr));
-        { Scope sc(eng, s, CAT_MSG_FWD, 1);
-        NB_TRY(nb_painn_msg_fwd_ex(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.q, ws.mu[l], ws.W + l * wl_stride, 3 * F, t_rev, ws.geom, ws.row_ptr, ws.col,
-                                   N, ws.q, ws.mu[l + 1], s, bf16)); }
-        // the update below adds to q and mu[l+1] in place: training keeps the values the update's Linear layers saw
-        if (train && (cudaMemcpyAsync(ws.q_mid[l], ws.q, (size_t)N * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess ||
-                      cudaMemcpyAsync(ws.mu_mid[l], ws.mu[l + 1], (size_t)N * 3 * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess))
+        if (keep_inputs && cudaMemcpyAsync(ws.t_q_in[l], ws.t_q, (size_t)N * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
             return nb_check_launch();
-        // update / mixing (painn.py:535-548)
-        NB_TRY(linear_fwd(eng, s, 3 * N, 2 * F, F, ws.mu[l + 1], F, U, F, ws.VW[l], 2 * F, false, nullptr, nullptr));
-        { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_upd_norm(ws.VW[l], w->epsilon, N, ws.nrm[l], s)); }
-        NB_TRY(linear_fwd(eng, s, N, F, F, ws.q, F, B1, 2 * F, ws.g1pre[l], F, false, nullptr, nullptr));
-        NB_TRY(linear_fwd(eng, s, N, F, F, ws.nrm[l], F, B1 + F, 2 * F, ws.g1pre[l], F, true, w->d1 + (size_t)l * F, ws.act));
-        NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.act, F, B2, F, ws.y[l], 3 * F, false, nullptr, nullptr));
-        { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_upd_combine(ws.q, ws.mu[l + 1], ws.VW[l], ws.y[l], w->d2 + (size_t)l * 3 * F, N, s)); }
+        NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, A1, F, ws.t_h1[l], F, false, nullptr, nullptr));
+        NB_TRY(nb_mul_dact(ws.h1pre[l], ws.t_h1[l], (int64_t)N * F, ws.t_act, s));
+        NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, A2, F, ws.t_xh[l], 3 * F, false, nullptr, nullptr));
+        NB_TRY(nb_msg_fwd_tan(ws.xh[l], ws.t_xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.t_mu[l], ws.W + l * wl, ws.dW + l * wl, ws.geom,
+                              ws.t_geom, ws.row_ptr, ws.col, N, ws.t_q, ws.t_mu[l + 1], s, bf16, ws.rev));
+        if (keep_inputs && (cudaMemcpyAsync(ws.t_q_mid[l], ws.t_q, (size_t)N * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess ||
+                            cudaMemcpyAsync(ws.t_mu_mid[l], ws.t_mu[l + 1], (size_t)N * 3 * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess))
+            return nb_check_launch();
+        NB_TRY(linear_fwd(eng, s, 3 * N, 2 * F, F, ws.t_mu[l + 1], F, U, F, ws.t_VW[l], 2 * F, false, nullptr, nullptr));
+        NB_TRY(nb_upd_norm_tan(ws.VW[l], ws.t_VW[l], ws.nrm[l], N, ws.t_nrm[l], s));
+        NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, B1, 2 * F, ws.t_g1[l], F, false, nullptr, nullptr));
+        NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_nrm[l], F, B1 + F, 2 * F, ws.t_g1[l], F, true, nullptr, nullptr));
+        NB_TRY(nb_mul_dact(ws.g1pre[l], ws.t_g1[l], (int64_t)N * F, ws.t_act, s));
+        NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, B2, F, ws.t_y[l], 3 * F, false, nullptr, nullptr));
+        NB_TRY(nb_upd_combine_tan(ws.t_q, ws.t_mu[l + 1], ws.VW[l], ws.t_VW[l], ws.y[l], ws.t_y[l], N, s));
     }
-    // ---- readout (painn.py:127-128; spk Atomwise + AddOffsets)
-    NB_TRY(linear_fwd(eng, s, N, F / 2, F, ws.q, F, w->R1, F, ws.ro_pre, F / 2, false, nullptr, nullptr));
-    { Scope sc(eng, s, CAT_READOUT, 1); NB_TRY(nb_readout(ws.ro_pre, w->e1, w->R2, w->e2, N, F / 2, ws.eps, s)); }
-    { Scope sc(eng, s, CAT_READOUT, 1); NB_TRY(nb_mol_sum(ws.eps, mol_ptr, n_mol, w->energy_shift_per_atom, energy, s)); }
-    if (!want_f) { Scope sc(eng, s, CAT_READOUT, 1); return nb_poison_on_error(status, energy, n_mol, nullptr, 0, s); }
-    }  // phase != 2
+    return linear_fwd(eng, s, N, F / 2, F, ws.t_q, F, w->R1, F, ws.t_ro, F / 2, false, nullptr, nullptr);
+}
 
-    // ---- force-loss tangent pass, forward half: directional derivative of every saved activation along v (weights carry no tangent)
-    if (tan) {
-        Scope sc(eng, s, CAT_NODE, 1 + 6 * L);
-        NB_TRY(nb_geom_tan(ws.geom, ws.row_ptr, ws.col, v_dir, N, ws.t_geom, s));
-        if (cudaMemsetAsync(ws.t_q, 0, (size_t)N * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();        // embedding: no tangent
-        if (cudaMemsetAsync(ws.t_mu[0], 0, (size_t)N * 3 * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();
-        for (int l = 0; l < L; ++l) {
-            const float* A1 = w->A1 + (size_t)l * F * F;
-            const float* A2 = w->A2 + (size_t)l * 3 * F * F;
-            const float* U = w->U + (size_t)l * 2 * F * F;
-            const float* B1 = w->B1 + (size_t)l * F * 2 * F;
-            const float* B2 = w->B2 + (size_t)l * 3 * F * F;
-            if (cudaMemcpyAsync(ws.t_q_in[l], ws.t_q, (size_t)N * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess) return nb_check_launch();
-            NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, A1, F, ws.t_h1[l], F, false, nullptr, nullptr));
-            NB_TRY(nb_mul_dact(ws.h1pre[l], ws.t_h1[l], (int64_t)N * F, ws.t_act, s));
-            NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, A2, F, ws.t_xh[l], 3 * F, false, nullptr, nullptr));
-            NB_TRY(nb_msg_fwd_tan(ws.xh[l], ws.t_xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.t_mu[l], ws.W + l * wl_stride, ws.dW + l * wl_stride,
-                                  ws.geom, ws.t_geom, ws.row_ptr, ws.col, N, ws.t_q, ws.t_mu[l + 1], s, bf16, t_rev));
-            if (cudaMemcpyAsync(ws.t_q_mid[l], ws.t_q, (size_t)N * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess ||
-                cudaMemcpyAsync(ws.t_mu_mid[l], ws.t_mu[l + 1], (size_t)N * 3 * F * sizeof(float), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
-                return nb_check_launch();
-            NB_TRY(linear_fwd(eng, s, 3 * N, 2 * F, F, ws.t_mu[l + 1], F, U, F, ws.t_VW[l], 2 * F, false, nullptr, nullptr));
-            NB_TRY(nb_upd_norm_tan(ws.VW[l], ws.t_VW[l], ws.nrm[l], N, ws.t_nrm[l], s));
-            NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, B1, 2 * F, ws.t_g1[l], F, false, nullptr, nullptr));
-            NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_nrm[l], F, B1 + F, 2 * F, ws.t_g1[l], F, true, nullptr, nullptr));
-            NB_TRY(nb_mul_dact(ws.g1pre[l], ws.t_g1[l], (int64_t)N * F, ws.t_act, s));
-            NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, B2, F, ws.t_y[l], 3 * F, false, nullptr, nullptr));
-            NB_TRY(nb_upd_combine_tan(ws.t_q, ws.t_mu[l + 1], ws.VW[l], ws.t_VW[l], ws.y[l], ws.t_y[l], N, s));
-        }
-        NB_TRY(linear_fwd(eng, s, N, F / 2, F, ws.t_q, F, w->R1, F, ws.t_ro, F / 2, false, nullptr, nullptr));
-    }
-
+// Training backward (painn_train.cu) from the activations the fused forward kept: d(sum_m seed_m E_m)/d(weights) -- and with a tangent pass
+// (`tan`) the force-seed term -- into the arrays `grads` points to (same layout as the weights; overwritten).  With `forces` it also returns
+// the true, unweighted -dE/dR of the same backward and poisons energy / forces on a device error.
+int train_bwd(nb200_engine* eng, const nb200_painn_weights* w, const Workspace& ws, const int32_t* z, const int32_t* mol_ptr, int32_t n_mol, int N,
+              int32_t e_cap, const float* seed_mol, const nb200_painn_weights* grads, bool tan, float* energy, float* forces, int32_t* status,
+              cudaStream_t s) {
+    const int L = w->n_layers, F = NB_F, K = w->n_rbf;
+    const size_t wl_stride = (size_t)e_cap * 3 * F;
+    const int bf16 = eng->edge_bf16;
+    const float* q_out = ws.fq_in[L];  // input of the readout
     // ---- analytic backward: forces = -dE/dR with dE/dE_m = 1 (painn.py:135-146)
     if (cudaMemsetAsync(ws.egrad, 0, (size_t)e_cap * 4 * sizeof(float), s) != cudaSuccess) return nb_check_launch();
     if (cudaMemsetAsync(ws.gmu_a, 0, (size_t)N * 3 * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();
@@ -424,11 +376,11 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
     // energy-seed weight gradients: dW += (c o g)^T x and dbias += colsum(c o g), c = the per-atom seed (`rs_div` rows of g per atom: 3 for the
     // (atom, xyz) rows of U).  One wgmma split-K launch (wgrad_tc.cu: the row scale is applied while loading g).
     // Weight-gradient launches are LEAVES of the step: they read buffers of the backward chain and only add into `grads`.  They run on a
-    // second stream of the engine, next to the chain (whose 76-CTA GEMMs and latency-bound phases leave SMs idle): fork = the side stream
+    // second stream of the engine, next to the chain (whose 76-CTA GEMMs and latency-bound steps leave SMs idle): fork = the side stream
     // waits for the chain's current point, and the chain waits for a leaf only right before it overwrites that leaf's inputs (`need`).  The
     // side stream is in order, so one event per input group is enough.
-    bool use_side = train && phase != 1;
-    if (use_side && !eng->side && cudaStreamCreateWithFlags(&eng->side, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); use_side = false; }
+    bool use_side = true;
+    if (!eng->side && cudaStreamCreateWithFlags(&eng->side, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); use_side = false; }
     const cudaStream_t ls = use_side ? eng->side : s;
     size_t ev_next = 0;
     auto ev_get = [&]() -> cudaEvent_t {
@@ -470,7 +422,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         leaf_done();
         return rc;
     };
-    if (train) {
+    {
         Scope sc(eng, s, CAT_NODE, 8);
         NB_TRY(nb_seed_atom(seed_mol, mol_ptr, n_mol, ws.seed_atom, s));
         // every gradient array starts at zero: the energy-seed terms and the force-seed (tangent) terms both ACCUMULATE into it
@@ -484,7 +436,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         NB_TRY(nb_act_only(ws.ro_pre, ws.seed_atom, N, F / 2, NB_ACT_SILU, ws.act_t, s));                    // c_i silu(pre_i)
         NB_TRY(nb_colsum(ws.act_t, N, F / 2, const_cast<float*>(grads->R2), s, 1.0f, 1));
         NB_TRY(nb_colsum(ws.seed_atom, N, 1, const_cast<float*>(grads->e2), s, 1.0f, 1));
-        NB_TRY(wg_primal(N, F / 2, F, ws.g_ro, F / 2, ws.q, F, const_cast<float*>(grads->R1), F, const_cast<float*>(grads->e1), 1));
+        NB_TRY(wg_primal(N, F / 2, F, ws.g_ro, F / 2, q_out, F, const_cast<float*>(grads->R1), F, const_cast<float*>(grads->e1), 1));
     }
     // tangent weight gradients enter with sign -1:  d/dtheta sum_i v_i.F_i = -(v.d/dR) dE_tot/dtheta   (seed 1, not the energy seed)
     // One launch: (c o g)^T x - tg^T x - g^T tx and the bias sums.
@@ -502,7 +454,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         NB_TRY(nb_readout_bwd_tan(ws.ro_pre, ws.t_ro, w->R2, N, F / 2, ws.t_g_ro, ws.t_act, s));  // t_act [N, F/2] = silu'(pre) pre^
         NB_TRY(linear_bwd(eng, s, N, F / 2, F, ws.t_g_ro, F / 2, w->R1, F, ws.t_gq, F, false));
         NB_TRY(nb_colsum(ws.t_act, N, F / 2, const_cast<float*>(grads->R2), s, -1.0f, 1));
-        NB_TRY(wgrad_tan(N, F / 2, F, ws.g_ro, ws.t_g_ro, F / 2, ws.q, ws.t_q, F, const_cast<float*>(grads->R1), F, const_cast<float*>(grads->e1)));
+        NB_TRY(wgrad_tan(N, F / 2, F, ws.g_ro, ws.t_g_ro, F / 2, q_out, ws.t_q, F, const_cast<float*>(grads->R1), F, const_cast<float*>(grads->e1)));
     }
     float *t_cur = ws.t_gmu_a, *t_other = ws.t_gmu_b;
     float *cur = ws.gmu_a, *other = ws.gmu_b;
@@ -517,7 +469,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         need(d_A2); need(d_U);  // the leaves of the layer above read gy / act_t (dA2) and gVW (dU)
         { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_upd_combine_bwd(ws.gq, cur, ws.y[l], ws.VW[l], N, ws.gy, ws.gVW, s)); }
         tag = &d_B2;
-        if (train) {  // dB2, dd2
+        {   // dB2, dd2
             Scope sc(eng, s, CAT_NODE, 3);
             NB_TRY(nb_act_only(ws.g1pre[l], nullptr, N, F, NB_ACT_SILU, ws.act_t, s));
             NB_TRY(wg_primal(N, 3 * F, F, ws.gy, 3 * F, ws.act_t, F, const_cast<float*>(grads->B2) + (size_t)l * 3 * F * F, F,
@@ -541,13 +493,13 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         if (tan) {  // dB1^, dd1^
             Scope sc(eng, s, CAT_NODE, 1);
             float* gB1 = const_cast<float*>(grads->B1) + (size_t)l * F * 2 * F;
-            NB_TRY(wgrad_tan(N, F, F, ws.gt, ws.t_gt, F, ws.q_mid[l], ws.t_q_mid[l], F, gB1, 2 * F, const_cast<float*>(grads->d1) + (size_t)l * F));
+            NB_TRY(wgrad_tan(N, F, F, ws.gt, ws.t_gt, F, ws.fq_mid[l], ws.t_q_mid[l], F, gB1, 2 * F, const_cast<float*>(grads->d1) + (size_t)l * F));
             NB_TRY(wgrad_tan(N, F, F, ws.gt, ws.t_gt, F, ws.nrm[l], ws.t_nrm[l], F, gB1 + F, 2 * F));
         }
-        if (train) {  // dB1 = [gt^T q_mid | gt^T nrm], dd1
+        {   // dB1 = [gt^T q_mid | gt^T nrm], dd1
             Scope sc(eng, s, CAT_NODE, 2);
             float* gB1 = const_cast<float*>(grads->B1) + (size_t)l * F * 2 * F;
-            NB_TRY(wg_primal(N, F, F, ws.gt, F, ws.q_mid[l], F, gB1, 2 * F, const_cast<float*>(grads->d1) + (size_t)l * F, 1));
+            NB_TRY(wg_primal(N, F, F, ws.gt, F, ws.fq_mid[l], F, gB1, 2 * F, const_cast<float*>(grads->d1) + (size_t)l * F, 1));
             NB_TRY(wg_primal(N, F, F, ws.gt, F, ws.nrm[l], F, gB1 + F, 2 * F, nullptr, 1));
         }
         NB_TRY(linear_bwd(eng, s, PT * N, F, F, ws.gt, F, B1, 2 * F, ws.gq, F, true));
@@ -559,27 +511,23 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
         { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_upd_norm_bwd(ws.gn, ws.VW[l], ws.nrm[l], N, ws.gVW, s)); }
         tag = &d_U;
         if (tan) {  // dU^ ; then the tangent of the gradient w.r.t. the post-message mu
-            NB_TRY(wgrad_tan(3 * N, 2 * F, F, ws.gVW, ws.t_gVW, 2 * F, ws.mu_mid[l], ws.t_mu_mid[l], F, const_cast<float*>(grads->U) + (size_t)l * 2 * F * F, F,
+            NB_TRY(wgrad_tan(3 * N, 2 * F, F, ws.gVW, ws.t_gVW, 2 * F, ws.fmu_mid[l], ws.t_mu_mid[l], F, const_cast<float*>(grads->U) + (size_t)l * 2 * F * F, F,
                              nullptr, 3));
         }
-        if (train) {  // dU over the 3N (atom, xyz) rows
+        {   // dU over the 3N (atom, xyz) rows
             Scope sc(eng, s, CAT_NODE, 1);
-            NB_TRY(wg_primal(3 * N, 2 * F, F, ws.gVW, 2 * F, ws.mu_mid[l], F, const_cast<float*>(grads->U) + (size_t)l * 2 * F * F, F, nullptr, 3));
+            NB_TRY(wg_primal(3 * N, 2 * F, F, ws.gVW, 2 * F, ws.fmu_mid[l], F, const_cast<float*>(grads->U) + (size_t)l * 2 * F * F, F, nullptr, 3));
         }
         NB_TRY(linear_bwd(eng, s, PT * 3 * N, 2 * F, F, ws.gVW, 2 * F, U, F, cur, F, true));  // (cur, t_cur) = (gmu_a, t_gmu_a) or (gmu_b, t_gmu_b): adjacent
         // message backward (by source atom; uses edge symmetry)
         need(d_B2); need(d_F);  // it overwrites gy (read by dB2) and the per-edge filter gradients (read by the filter leaves of the layer above)
         { Scope sc(eng, s, CAT_MSG_BWD, 1);
-        if (!train)
-            NB_TRY(nb200_painn_msg_bwd(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.W + l * wl_stride, ws.dW + l * wl_stride, ws.geom,
-                                       ws.row_ptr, ws.col, N, ws.gq, cur, ws.gy, other, ws.egrad, s));
-        else
-            NB_TRY(nb_painn_msg_bwd_train(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.W + l * wl_stride, ws.dW + l * wl_stride, ws.geom,
-                                          ws.row_ptr, ws.col, N, ws.gq, cur, ws.gy, other, ws.egrad, ws.gW, ws.seed_atom, s, bf16, t_rev)); }
+        NB_TRY(nb_painn_msg_bwd_train(ws.xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.W + l * wl_stride, ws.dW + l * wl_stride, ws.geom,
+                                      ws.row_ptr, ws.col, N, ws.gq, cur, ws.gy, other, ws.egrad, ws.gW, ws.seed_atom, s, bf16, ws.rev)); }
         if (tan) {  // message backward tangent reads the same gq / cur the primal call just read; its outputs go to the t_ twins
             Scope sc(eng, s, CAT_NODE, 2);
             NB_TRY(nb_msg_bwd_tan(ws.xh[l], ws.t_xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.t_mu[l], ws.W + l * wl_stride, ws.dW + l * wl_stride,
-                                  ws.geom, ws.t_geom, ws.row_ptr, ws.col, N, ws.gq, ws.t_gq, cur, t_cur, ws.t_gy, t_other, ws.t_gW, ws.gWd, s, bf16, t_rev));
+                                  ws.geom, ws.t_geom, ws.row_ptr, ws.col, N, ws.gq, ws.t_gq, cur, t_cur, ws.t_gy, t_other, ws.t_gW, ws.gWd, s, bf16, ws.rev));
             tag = &d_F; fork();
             NB_TRY(nb_filter_wgrad_tan(ws.geom, ws.t_geom, status, ws.sort_scr2, w->rbf_offsets, K, w->radial_mode, w->cutoff, w->rbf_coeff, w->rbf_xscale,
                                        ws.t_gW, ws.gWd, -1.0f, const_cast<float*>(grads->w_rbf) + (size_t)l * K * 3 * F,
@@ -588,7 +536,7 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
             float* tt = t_cur; t_cur = t_other; t_other = tt;
         }
         float* t = cur; cur = other; other = t;
-        if (train) {  // filter weights of this layer, then dA2, dc2
+        {   // filter weights of this layer, then dA2, dc2
             Scope sc(eng, s, CAT_NODE, 4);
             tag = &d_F; fork();
             NB_TRY(nb_filter_wgrad(ws.geom, status, ws.sort_scr2, w->rbf_offsets, K, w->radial_mode, w->cutoff, w->rbf_coeff, w->rbf_xscale, ws.gW,
@@ -605,31 +553,30 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
             NB_TRY(wgrad_tan(N, 3 * F, F, ws.gy, ws.t_gy, 3 * F, ws.act_t, ws.t_act, F, const_cast<float*>(grads->A2) + (size_t)l * 3 * F * F, F,
                              const_cast<float*>(grads->c2) + (size_t)l * 3 * F));
         }
-        if (l > 0 || train) {  // inference: the embedding does not depend on positions, layer 0 stops here
-            need(d_B1);  // dB1 read gt
-            NB_TRY(linear_bwd(eng, s, PT * N, 3 * F, F, ws.gy, 3 * F, A2, F, ws.gt, F, false));
-            tag = &d_A1;
-            if (tan) {
-                Scope sc(eng, s, CAT_NODE, 1);
-                NB_TRY(nb_act_bwd_tan(ws.t_gt, ws.gt, ws.h1pre[l], ws.t_h1[l], (int64_t)N * F, s));
-            }
-            { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_act_bwd(ws.gt, ws.h1pre[l], (int64_t)N * F, NB_ACT_SILU, s)); }
-            if (tan) {  // dA1^, dc1^
-                Scope sc(eng, s, CAT_NODE, 1);
-                NB_TRY(wgrad_tan(N, F, F, ws.gt, ws.t_gt, F, ws.q_in[l], ws.t_q_in[l], F, const_cast<float*>(grads->A1) + (size_t)l * F * F, F,
-                                 const_cast<float*>(grads->c1) + (size_t)l * F));
-            }
-            if (train) {  // dA1, dc1
-                Scope sc(eng, s, CAT_NODE, 2);
-                NB_TRY(wg_primal(N, F, F, ws.gt, F, ws.q_in[l], F, const_cast<float*>(grads->A1) + (size_t)l * F * F, F,
-                                 const_cast<float*>(grads->c1) + (size_t)l * F, 1));
-            }
-            NB_TRY(linear_bwd(eng, s, PT * N, F, F, ws.gt, F, A1, F, ws.gq, F, true));
+        // message MLP backward, through layer 0: the embedding gradient needs dE/dq of the embedding
+        need(d_B1);  // dB1 read gt
+        NB_TRY(linear_bwd(eng, s, PT * N, 3 * F, F, ws.gy, 3 * F, A2, F, ws.gt, F, false));
+        tag = &d_A1;
+        if (tan) {
+            Scope sc(eng, s, CAT_NODE, 1);
+            NB_TRY(nb_act_bwd_tan(ws.t_gt, ws.gt, ws.h1pre[l], ws.t_h1[l], (int64_t)N * F, s));
         }
+        { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_act_bwd(ws.gt, ws.h1pre[l], (int64_t)N * F, NB_ACT_SILU, s)); }
+        if (tan) {  // dA1^, dc1^
+            Scope sc(eng, s, CAT_NODE, 1);
+            NB_TRY(wgrad_tan(N, F, F, ws.gt, ws.t_gt, F, ws.fq_in[l], ws.t_q_in[l], F, const_cast<float*>(grads->A1) + (size_t)l * F * F, F,
+                             const_cast<float*>(grads->c1) + (size_t)l * F));
+        }
+        {   // dA1, dc1
+            Scope sc(eng, s, CAT_NODE, 2);
+            NB_TRY(wg_primal(N, F, F, ws.gt, F, ws.fq_in[l], F, const_cast<float*>(grads->A1) + (size_t)l * F * F, F,
+                             const_cast<float*>(grads->c1) + (size_t)l * F, 1));
+        }
+        NB_TRY(linear_bwd(eng, s, PT * N, F, F, ws.gt, F, A1, F, ws.gq, F, true));
     }
-    if (train) { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_emb_grad(ws.gq, ws.seed_atom, z, w->z_offset, w->n_elem, N, const_cast<float*>(grads->emb), s)); }
+    { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_emb_grad(ws.gq, ws.seed_atom, z, w->z_offset, w->n_elem, N, const_cast<float*>(grads->emb), s)); }
     if (tan) { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_emb_grad(ws.t_gq, nullptr, z, w->z_offset, w->n_elem, N, const_cast<float*>(grads->emb), s, -1.0f)); }
-    if (phase == 2) return NB200_OK;  // energies / forces were returned (and poisoned on error) by phase 1
+    if (!forces) return NB200_OK;
     { Scope sc(eng, s, CAT_FORCE, 2); NB_TRY(nb200_edge_forces(ws.egrad, ws.geom, ws.row_ptr, ws.rev, N, forces, s));
       NB_TRY(nb_poison_on_error(status, energy, n_mol, forces, (int64_t)3 * N, s)); }
     return NB200_OK;
@@ -637,10 +584,17 @@ int run_painn(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z,
 
 }  // namespace
 
+// Inference: graph + filters with half-row [W | dW/dd] records, then the fused forward (and force backward).
 extern "C" int nb200_painn_energy_forces(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos,
                                          const int32_t* mol_ptr, int32_t n_mol, int32_t n_atoms, int32_t e_cap, void* workspace,
                                          int64_t workspace_bytes, float* energy, float* forces, int32_t* status, void* stream) {
-    return run_painn(eng, w, z, pos, mol_ptr, n_mol, n_atoms, e_cap, workspace, workspace_bytes, energy, forces, status, stream, nullptr, nullptr);
+    if (!pos || !energy) return NB200_EINVAL;
+    NB_TRY(args_ok(eng, w, z, mol_ptr, n_mol, n_atoms, e_cap, workspace, status));
+    const Workspace ws = carve(workspace, w->n_layers, NB_F, n_mol, n_atoms, e_cap, forces != nullptr);
+    if (ws.bytes > workspace_bytes) return NB200_EINVAL;
+    const cudaStream_t s = (cudaStream_t)stream;
+    NB_TRY(graph_and_filters(eng, w, ws, pos, mol_ptr, n_mol, n_atoms, e_cap, status, s, forces != nullptr, false));
+    return run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, n_atoms, e_cap, energy, forces, status, s, true, 0);
 }
 
 extern "C" int64_t nb200_painn_train_workspace_bytes(const nb200_painn_weights* w, int32_t b_cap, int32_t n_cap, int32_t e_cap,
@@ -652,53 +606,75 @@ extern "C" int64_t nb200_painn_train_workspace_bytes(const nb200_painn_weights* 
 // Training step in two calls on one training workspace (sized by nb200_painn_train_workspace_bytes with the SAME with_force_seed flag for
 // both): the forward + forces first, the parameter gradients once the loss has produced the seeds.  Nothing else may use the workspace in
 // between; weights, z, mol_ptr, n_* and e_cap must be those of the forward call.
+// Forward: graph + training filters + the directed-edge bin sort, then the fused forward with forces; every activation the backward reads
+// stays in the workspace.
 extern "C" int nb200_painn_train_forward(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
                                          int32_t n_mol, int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes,
                                          int32_t with_force_seed, float* energy, float* forces, int32_t* status, void* stream) {
-    if (!forces) return NB200_EINVAL;
-    return run_painn(eng, w, z, pos, mol_ptr, n_mol, n_atoms, e_cap, workspace, workspace_bytes, energy, forces, status, stream, nullptr, nullptr, nullptr,
-                     1, with_force_seed != 0);
+    if (!pos || !energy || !forces) return NB200_EINVAL;
+    NB_TRY(args_ok(eng, w, z, mol_ptr, n_mol, n_atoms, e_cap, workspace, status));
+    const Workspace ws = carve(workspace, w->n_layers, NB_F, n_mol, n_atoms, e_cap, true, true, with_force_seed != 0);
+    if (ws.bytes > workspace_bytes) return NB200_EINVAL;
+    const cudaStream_t s = (cudaStream_t)stream;
+    NB_TRY(graph_and_filters(eng, w, ws, pos, mol_ptr, n_mol, n_atoms, e_cap, status, s, false, true));
+    return run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, n_atoms, e_cap, energy, forces, status, s, false, eng->edge_bf16);
 }
 
+// Backward: the tangent forward if there is a force seed, then the training backward (energies / forces were returned, and poisoned on
+// error, by the forward call).
 extern "C" int nb200_painn_train_backward(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const int32_t* mol_ptr, int32_t n_mol,
                                           int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes, int32_t with_force_seed,
                                           const float* energy_seed, const float* force_seed, const nb200_painn_weights* grads, int32_t* status,
                                           void* stream) {
-    if (!grads || (force_seed && !with_force_seed)) return NB200_EINVAL;
-    return run_painn(eng, w, z, nullptr, mol_ptr, n_mol, n_atoms, e_cap, workspace, workspace_bytes, nullptr, nullptr, status, stream, energy_seed, grads,
-                     force_seed, 2, with_force_seed != 0);
+    if (!grads_ok(grads) || (force_seed && !with_force_seed)) return NB200_EINVAL;
+    NB_TRY(args_ok(eng, w, z, mol_ptr, n_mol, n_atoms, e_cap, workspace, status));
+    const Workspace ws = carve(workspace, w->n_layers, NB_F, n_mol, n_atoms, e_cap, true, true, with_force_seed != 0);
+    if (ws.bytes > workspace_bytes) return NB200_EINVAL;
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (force_seed) {
+        Scope sc(eng, s, CAT_NODE, 1 + 6 * w->n_layers);
+        NB_TRY(tangent_fwd(eng, w, ws, force_seed, n_atoms, e_cap, eng->edge_bf16, true, s));
+    }
+    return train_bwd(eng, w, ws, z, mol_ptr, n_mol, n_atoms, e_cap, energy_seed, grads, force_seed != nullptr, nullptr, nullptr, status, s);
 }
 
+// The training step in one call: the forward of nb200_painn_train_forward without its force backward (the training backward produces the
+// forces), then the tangent forward and the training backward.
 extern "C" int nb200_painn_energy_forces_grads(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos,
                                                const int32_t* mol_ptr, int32_t n_mol, int32_t n_atoms, int32_t e_cap, void* workspace,
                                                int64_t workspace_bytes, const float* energy_seed, const float* force_seed,
                                                const nb200_painn_weights* grads, float* energy, float* forces, int32_t* status, void* stream) {
-    if (!grads) return NB200_EINVAL;
-    return run_painn(eng, w, z, pos, mol_ptr, n_mol, n_atoms, e_cap, workspace, workspace_bytes, energy, forces, status, stream, energy_seed, grads,
-                     force_seed);
+    if (!pos || !energy || !forces || !grads_ok(grads)) return NB200_EINVAL;
+    NB_TRY(args_ok(eng, w, z, mol_ptr, n_mol, n_atoms, e_cap, workspace, status));
+    const bool tan = force_seed != nullptr;
+    const Workspace ws = carve(workspace, w->n_layers, NB_F, n_mol, n_atoms, e_cap, true, true, tan);
+    if (ws.bytes > workspace_bytes) return NB200_EINVAL;
+    const cudaStream_t s = (cudaStream_t)stream;
+    NB_TRY(graph_and_filters(eng, w, ws, pos, mol_ptr, n_mol, n_atoms, e_cap, status, s, false, true));
+    NB_TRY(run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, n_atoms, e_cap, energy, nullptr, status, s, false, eng->edge_bf16));
+    if (tan) {
+        Scope sc(eng, s, CAT_NODE, 1 + 6 * w->n_layers);
+        NB_TRY(tangent_fwd(eng, w, ws, force_seed, n_atoms, e_cap, eng->edge_bf16, true, s));
+    }
+    return train_bwd(eng, w, ws, z, mol_ptr, n_mol, n_atoms, e_cap, energy_seed, grads, tan, energy, forces, status, s);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Hessian-vector products H v = -dF/dR . v (DESIGN.md section 3.13): the primal forward (fused node kernels, activations kept, as the first
-// call of the two-call training step) runs once; then, per direction, the tangent forward of painn_tangent.cu and the stacked
-// [primal ; tangent] backward of the training step without any weight gradient, the message backward tangent also producing the tangent
-// of the per-edge geometric gradient (t_egrad), and the tangent of the force assembly.  The workspace holds ONE direction's tangent
-// arrays whatever n_dir is.
+// call of the two-call training step) runs once; then, per direction, the tangent forward and the stacked [primal ; tangent] backward of
+// the training step without any weight gradient, the message backward tangent also producing the tangent of the per-edge geometric
+// gradient (t_egrad), and the tangent of the force assembly.  The workspace holds ONE direction's tangent arrays whatever n_dir is.
 namespace {
 
 int run_painn_hvp(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr, int32_t n_mol,
                   int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes, int32_t n_dir, const float* v, float* energy, float* forces,
                   float* hv, int32_t* status, void* stream) {
-    if (!eng || !weights_ok(w) || !z || !pos || !mol_ptr || !workspace || !v || !energy || !hv || !status || n_dir < 1) return NB200_EINVAL;
-    if (w->n_feat != NB_F || w->n_layers <= 0 || w->n_layers > kMaxLayers) return NB200_EUNSUPPORTED;
-    if (n_mol <= 0 || n_atoms <= 0 || e_cap <= 0) return NB200_EINVAL;
+    if (!pos || !v || !energy || !hv || n_dir < 1) return NB200_EINVAL;
+    NB_TRY(args_ok(eng, w, z, mol_ptr, n_mol, n_atoms, e_cap, workspace, status));
     const int L = w->n_layers, F = NB_F, K = w->n_rbf, N = n_atoms;
     Workspace ws = carve(workspace, L, F, n_mol, N, e_cap, true, false, true, true);
     if (ws.bytes > workspace_bytes) return NB200_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
-    cublasHandle_t h = eng->blas;
-    NB_BLAS(cublasSetStream(h, s) == CUBLAS_STATUS_SUCCESS);
-    NB_BLAS(cublasSetWorkspace(h, ws.blas_ws, kBlasWs) == CUBLAS_STATUS_SUCCESS);
     const size_t wl = (size_t)e_cap * 3 * F;
     { Scope sc(eng, s, CAT_NBR, 3);
     NB_TRY(nb200_neighbor_build(pos, mol_ptr, n_mol, N, w->cutoff, w->max_neighbors, e_cap, ws.row_ptr, ws.col, ws.rev, ws.geom, ws.deg, status, s)); }
@@ -707,37 +683,12 @@ int run_painn_hvp(nb200_engine* eng, const nb200_painn_weights* w, const int32_t
     NB_TRY(nb_painn_filter_d2(ws.geom, status, e_cap, w->w_rbf, w->b_rbf, L, K, w->radial_mode, w->cutoff, w->rbf_offsets, w->rbf_coeff, w->rbf_xscale, ws.W,
                               ws.dW, ws.d2W, ws.sort_scr, ws.rev, s)); }
     // energies (and forces) with every activation the tangent pass reads kept: layer inputs / post-message states in fq_in, fmu_mid
-    NB_TRY(run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s, false, 0, true));
+    NB_TRY(run_painn_fused(eng, w, ws, z, mol_ptr, n_mol, N, e_cap, energy, forces, status, s, false, 0));
 
     for (int32_t dir = 0; dir < n_dir; ++dir) {
-        // ---- tangent forward along v_dir (painn_tangent.cu; the same sequence as the force-loss term of the training step).  With timing on,
-        // its CAT_MSG_FWD scope brackets the whole tangent forward, GEMMs included (bench_hessian.py splits forward / backward with it).
-        {
-            Scope sc(eng, s, CAT_MSG_FWD, 1 + 6 * L);
-            NB_TRY(nb_geom_tan(ws.geom, ws.row_ptr, ws.col, v + (size_t)dir * 3 * N, N, ws.t_geom, s));
-            if (cudaMemsetAsync(ws.t_q, 0, (size_t)N * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();  // embedding: no tangent
-            if (cudaMemsetAsync(ws.t_mu[0], 0, (size_t)N * 3 * F * sizeof(float), s) != cudaSuccess) return nb_check_launch();
-            for (int l = 0; l < L; ++l) {
-                const float* A1 = w->A1 + (size_t)l * F * F;
-                const float* A2 = w->A2 + (size_t)l * 3 * F * F;
-                const float* U = w->U + (size_t)l * 2 * F * F;
-                const float* B1 = w->B1 + (size_t)l * F * 2 * F;
-                const float* B2 = w->B2 + (size_t)l * 3 * F * F;
-                NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, A1, F, ws.t_h1[l], F, false, nullptr, nullptr));
-                NB_TRY(nb_mul_dact(ws.h1pre[l], ws.t_h1[l], (int64_t)N * F, ws.t_act, s));
-                NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, A2, F, ws.t_xh[l], 3 * F, false, nullptr, nullptr));
-                NB_TRY(nb_msg_fwd_tan(ws.xh[l], ws.t_xh[l], w->c2 + (size_t)l * 3 * F, ws.mu[l], ws.t_mu[l], ws.W + l * wl, ws.dW + l * wl, ws.geom,
-                                      ws.t_geom, ws.row_ptr, ws.col, N, ws.t_q, ws.t_mu[l + 1], s, 0, ws.rev));
-                NB_TRY(linear_fwd(eng, s, 3 * N, 2 * F, F, ws.t_mu[l + 1], F, U, F, ws.t_VW[l], 2 * F, false, nullptr, nullptr));
-                NB_TRY(nb_upd_norm_tan(ws.VW[l], ws.t_VW[l], ws.nrm[l], N, ws.t_nrm[l], s));
-                NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_q, F, B1, 2 * F, ws.t_g1[l], F, false, nullptr, nullptr));
-                NB_TRY(linear_fwd(eng, s, N, F, F, ws.t_nrm[l], F, B1 + F, 2 * F, ws.t_g1[l], F, true, nullptr, nullptr));
-                NB_TRY(nb_mul_dact(ws.g1pre[l], ws.t_g1[l], (int64_t)N * F, ws.t_act, s));
-                NB_TRY(linear_fwd(eng, s, N, 3 * F, F, ws.t_act, F, B2, F, ws.t_y[l], 3 * F, false, nullptr, nullptr));
-                NB_TRY(nb_upd_combine_tan(ws.t_q, ws.t_mu[l + 1], ws.VW[l], ws.t_VW[l], ws.y[l], ws.t_y[l], N, s));
-            }
-            NB_TRY(linear_fwd(eng, s, N, F / 2, F, ws.t_q, F, w->R1, F, ws.t_ro, F / 2, false, nullptr, nullptr));
-        }
+        // ---- tangent forward along v_dir.  With timing on, its CAT_MSG_FWD scope brackets the whole tangent forward, GEMMs included
+        // (bench_hessian.py splits forward / backward with it).
+        { Scope sc(eng, s, CAT_MSG_FWD, 1 + 6 * L); NB_TRY(tangent_fwd(eng, w, ws, v + (size_t)dir * 3 * N, N, e_cap, 0, false, s)); }
         // ---- backward, primal and tangent: every Linear backward on the stacked rows [g ; g^] (carve: adjacent pairs)
         if (cudaMemsetAsync(ws.egrad, 0, (size_t)e_cap * 4 * sizeof(float), s) != cudaSuccess ||
             cudaMemsetAsync(ws.t_egrad, 0, (size_t)e_cap * 4 * sizeof(float), s) != cudaSuccess ||

@@ -10,10 +10,8 @@
 enum { CAT_NBR = 0, CAT_FILTER, CAT_EMBED, CAT_GEMM, CAT_NODE, CAT_MSG_FWD, CAT_MSG_BWD, CAT_READOUT, CAT_FORCE, NCAT };
 
 struct nb200_engine {
-    cublasHandle_t blas;
+    cublasHandle_t blas;          // weight gradients of the GemNet-OC and SchNet training steps (goc_wgrad, gemnet_pf.cuh)
     bool timing = false;
-    int gemm_backend = 1;         // 1 = wgmma 3xTF32 (gemm_tc.cu), 0 = cuBLAS SGEMM
-    int node_backend = 1;         // PaiNN inference: 1 = fused per-layer node kernels (painn_fused.cu), 0 = one launch per Linear / elementwise op
     cudaStream_t side = nullptr;  // PaiNN training: weight-gradient ("leaf") launches run here, next to the backward chain on the caller's stream
     std::vector<cudaEvent_t> side_ev;
     int edge_bf16 = 0;            // PaiNN training: per-edge arrays (filter rows W, dW/dd, per-edge filter gradients) stored as bf16, fp32 arithmetic
@@ -50,7 +48,6 @@ struct Scope {
 
 
 constexpr int64_t kAlign = 256;
-constexpr int64_t kBlasWs = 32ll << 20;
 
 struct Carver {
     char* base;
@@ -66,44 +63,23 @@ struct Carver {
 };
 
 
+// Linear layers on the wgmma 3xTF32 GEMM of gemm_tc.cu.
 // Y[M,out] (ldy) = X[M,in] (ldx) . W[out,in]^T (ldw) (+ Y) (+ bias) ; optional act = silu(Y)   -- torch.nn.Linear forward
 inline int linear_fwd(nb200_engine* e, cudaStream_t s, int M, int out, int in, const float* X, int ldx, const float* W, int ldw, float* Y,
                       int ldy, bool accumulate, const float* bias, float* act, int act_kind = NB_ACT_SILU) {
-    if (e->gemm_backend == 1) {
-        Scope sc(e, s, CAT_GEMM, 1);
-        return nb_gemm_tf32x3_ex(M, out, in, X, ldx, W, ldw, 0, Y, ldy, accumulate ? 1 : 0, bias, act, act_kind, s);
-    }
-    {
-        Scope sc(e, s, CAT_GEMM, 0);
-        const float alpha = 1.0f, beta = accumulate ? 1.0f : 0.0f;
-        if (cublasSgemm(e->blas, CUBLAS_OP_T, CUBLAS_OP_N, out, M, in, &alpha, W, ldw, X, ldx, &beta, Y, ldy) != CUBLAS_STATUS_SUCCESS)
-            return NB200_ECUDA;
-    }
-    if (bias || act) {
-        if (!bias || ldy != out) return NB200_EINVAL;  // cuBLAS path: bias (+ optional activation) on dense rows
-        Scope sc(e, s, CAT_NODE, 1);
-        return nb_bias_act(Y, bias, act, M, out, act_kind, s);
-    }
-    return NB200_OK;
+    Scope sc(e, s, CAT_GEMM, 1);
+    return nb_gemm_tf32x3_ex(M, out, in, X, ldx, W, ldw, 0, Y, ldy, accumulate ? 1 : 0, bias, act, act_kind, s);
 }
 // gX[M,in] (ldgx) = gY[M,out] (ldgy) . W[out,in] (ldw)  (+ gX)                                   -- Linear backward w.r.t. input
 inline int linear_bwd(nb200_engine* e, cudaStream_t s, int M, int out, int in, const float* gY, int ldgy, const float* W, int ldw, float* gX,
                       int ldgx, bool accumulate) {
-    Scope sc(e, s, CAT_GEMM, e->gemm_backend == 1 ? 1 : 0);
-    if (e->gemm_backend == 1) return nb200_gemm_tf32x3(M, in, out, gY, ldgy, W, ldw, 1, gX, ldgx, accumulate ? 1 : 0, nullptr, nullptr, s);
-    const float alpha = 1.0f, beta = accumulate ? 1.0f : 0.0f;
-    return cublasSgemm(e->blas, CUBLAS_OP_N, CUBLAS_OP_N, in, M, out, &alpha, W, ldw, gY, ldgy, &beta, gX, ldgx) == CUBLAS_STATUS_SUCCESS
-               ? NB200_OK
-               : NB200_ECUDA;
+    Scope sc(e, s, CAT_GEMM, 1);
+    return nb200_gemm_tf32x3(M, in, out, gY, ldgy, W, ldw, 1, gX, ldgx, accumulate ? 1 : 0, nullptr, nullptr, s);
 }
 
 #define NB_TRY(expr)                  \
     do {                              \
         int _rc = (expr);             \
         if (_rc != NB200_OK) return _rc; \
-    } while (0)
-#define NB_BLAS(expr)                 \
-    do {                              \
-        if (!(expr)) return NB200_ECUDA; \
     } while (0)
 

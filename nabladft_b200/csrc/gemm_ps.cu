@@ -2,7 +2,7 @@
 //
 // Replaces the round-1 3xTF32 kernels of gemm_tc.cu where they were slowest: torch.nn.Linear / e3nn FullyConnectedNet layers applied to every
 // atom pair or edge (QHNet weight generation [1e5 x 8320 x 128], qhnet/layers.py:191-203,376-459; GemNet-OC Dense layers [6e5 x 512 x 512],
-// gemnet_oc/layers/base_layers.py; the unfused PaiNN / SchNet paths).  There the MMA issuer idled 70 % of the time waiting for producer
+// gemnet_oc/layers/base_layers.py; the per-Linear PaiNN / SchNet paths).  There the MMA issuer idled 70 % of the time waiting for producer
 // warps that split the WEIGHT operand into TF32 hi / lo again for every 128-row slab.  Here
 //   * the weight matrix is split ONCE per call into ready-made shared-memory tile images (k_prep_gemm, 128 KB per 128 x 128 tile) in a scratch
 //     buffer, and streamed by single cp.async.bulk copies -- nobody splits weights inside the GEMM;

@@ -29,17 +29,6 @@ __global__ void __launch_bounds__(NODE_THREADS) k_embed(const int32_t* __restric
     st4(m, f4(0.f)); st4(m + NB_F, f4(0.f)); st4(m + 2 * NB_F, f4(0.f));
 }
 
-// pre += bias (kept for the backward), act = silu(pre)
-__global__ void __launch_bounds__(NODE_THREADS) k_bias_silu(float* __restrict__ pre, const float* __restrict__ bias,
-                                                           float* __restrict__ act, int64_t n4, int width4, int kind) {
-    const int64_t t = (int64_t)blockIdx.x * NODE_THREADS + threadIdx.x;
-    if (t >= n4) return;
-    const int c = (int)(t % width4) * 4;
-    float4 p = *reinterpret_cast<const float4*>(pre + 4 * t) + ldg4(bias + c);
-    st4(pre + 4 * t, p);
-    if (act) st4(act + 4 * t, make_float4(actf_(p.x, kind), actf_(p.y, kind), actf_(p.z, kind), actf_(p.w, kind)));
-}
-
 __global__ void __launch_bounds__(NODE_THREADS) k_silu_bwd(float* __restrict__ g, const float* __restrict__ pre, int64_t n4, int kind) {
     const int64_t t = (int64_t)blockIdx.x * NODE_THREADS + threadIdx.x;
     if (t >= n4) return;
@@ -48,44 +37,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_silu_bwd(float* __restrict__ g
     st4(g + 4 * t, make_float4(v.x * dactf_(p.x, kind), v.y * dactf_(p.y, kind), v.z * dactf_(p.z, kind), v.w * dactf_(p.w, kind)));
 }
 
-// nrm = sqrt(sum_x V[x]^2 + eps)   (painn.py:541; spk PaiNNMixing epsilon)
-__global__ void __launch_bounds__(NODE_THREADS) k_upd_norm(const float* __restrict__ VW, float eps, int n_atoms, float* __restrict__ nrm) {
-    const int t = blockIdx.x * NODE_THREADS + threadIdx.x;
-    const int i = t >> 5, c = (t & 31) * 4;
-    if (i >= n_atoms) return;
-    const float* v = VW + (size_t)i * 6 * NB_F + c;
-    const float4 v0 = ldg4(v), v1 = ldg4(v + 2 * NB_F), v2 = ldg4(v + 4 * NB_F);
-    float4 s = v0 * v0; fma4(s, v1, v1); fma4(s, v2, v2);
-    st4(nrm + (size_t)i * NB_F + c, make_float4(sqrtf(s.x + eps), sqrtf(s.y + eps), sqrtf(s.z + eps), sqrtf(s.w + eps)));
-}
-
-__global__ void __launch_bounds__(NODE_THREADS) k_upd_combine(float* __restrict__ q, float* __restrict__ mu, const float* __restrict__ VW,
-                                                             float* __restrict__ y, const float* __restrict__ y_bias, int n_atoms) {
-    const int t = blockIdx.x * NODE_THREADS + threadIdx.x;
-    const int i = t >> 5, c = (t & 31) * 4;
-    if (i >= n_atoms) return;
-    float* yi = y + (size_t)i * 3 * NB_F + c;
-    const float4 y0 = *reinterpret_cast<const float4*>(yi) + ldg4(y_bias + c);
-    const float4 y1 = *reinterpret_cast<const float4*>(yi + NB_F) + ldg4(y_bias + NB_F + c);
-    const float4 y2 = *reinterpret_cast<const float4*>(yi + 2 * NB_F) + ldg4(y_bias + 2 * NB_F + c);
-    st4(yi, y0); st4(yi + NB_F, y1); st4(yi + 2 * NB_F, y2);  // biased y is what the backward needs
-    const float* v = VW + (size_t)i * 6 * NB_F + c;
-    float4 dot = f4(0.f);
-    float* m = mu + (size_t)i * 3 * NB_F + c;
-#pragma unroll
-    for (int x = 0; x < 3; ++x) {
-        const float4 V = ldg4(v + x * 2 * NB_F), Wv = ldg4(v + x * 2 * NB_F + NB_F);
-        fma4(dot, V, Wv);
-        float4 mx = *reinterpret_cast<const float4*>(m + x * NB_F);
-        fma4(mx, y1, Wv);
-        st4(m + x * NB_F, mx);
-    }
-    float4 qi = *reinterpret_cast<const float4*>(q + (size_t)i * NB_F + c) + y0;
-    fma4(qi, y2, dot);
-    st4(q + (size_t)i * NB_F + c, qi);
-}
-
-// gy = (gq, sum_x gmu[x]*Wv[x], gq*dot) ; gVW[x] = (gdot*Wv[x], gmu[x]*y1 + gdot*V[x]), gdot = gq*y2
+// gy =(gq, sum_x gmu[x]*Wv[x], gq*dot) ; gVW[x] = (gdot*Wv[x], gmu[x]*y1 + gdot*V[x]), gdot = gq*y2
 __global__ void __launch_bounds__(NODE_THREADS) k_upd_combine_bwd(const float* __restrict__ gq, const float* __restrict__ gmu,
                                                                  const float* __restrict__ y, const float* __restrict__ VW, int n_atoms,
                                                                  float* __restrict__ gy, float* __restrict__ gVW) {
@@ -190,21 +142,8 @@ int nb_embed(const int32_t* z, const float* emb, int z_offset, int n_elem, int n
     k_embed<<<grid_for((int64_t)n_atoms * 32), NODE_THREADS, 0, s>>>(z, emb, z_offset, n_elem, n_atoms, q, mu, status);
     return nb_check_launch();
 }
-int nb_bias_act(float* pre, const float* bias, float* act, int n_rows, int width, int kind, cudaStream_t s) {
-    const int64_t n4 = (int64_t)n_rows * width / 4;
-    k_bias_silu<<<grid_for(n4), NODE_THREADS, 0, s>>>(pre, bias, act, n4, width / 4, kind);
-    return nb_check_launch();
-}
 int nb_act_bwd(float* g, const float* pre, int64_t n, int kind, cudaStream_t s) {
     k_silu_bwd<<<grid_for(n / 4), NODE_THREADS, 0, s>>>(g, pre, n / 4, kind);
-    return nb_check_launch();
-}
-int nb_upd_norm(const float* VW, float eps, int n_atoms, float* nrm, cudaStream_t s) {
-    k_upd_norm<<<grid_for((int64_t)n_atoms * 32), NODE_THREADS, 0, s>>>(VW, eps, n_atoms, nrm);
-    return nb_check_launch();
-}
-int nb_upd_combine(float* q, float* mu, const float* VW, float* y, const float* y_bias, int n_atoms, cudaStream_t s) {
-    k_upd_combine<<<grid_for((int64_t)n_atoms * 32), NODE_THREADS, 0, s>>>(q, mu, VW, y, y_bias, n_atoms);
     return nb_check_launch();
 }
 int nb_upd_combine_bwd(const float* gq, const float* gmu, const float* y, const float* VW, int n_atoms, float* gy, float* gVW,

@@ -4,10 +4,7 @@
 
 int nb_embed(const int32_t* z, const float* emb, int z_offset, int n_elem, int n_atoms, float* q, float* mu, int32_t* status,
              cudaStream_t s);
-int nb_bias_act(float* pre, const float* bias, float* act, int n_rows, int width, int kind, cudaStream_t s);
 int nb_act_bwd(float* g, const float* pre, int64_t n, int kind, cudaStream_t s);
-int nb_upd_norm(const float* VW, float eps, int n_atoms, float* nrm, cudaStream_t s);
-int nb_upd_combine(float* q, float* mu, const float* VW, float* y, const float* y_bias, int n_atoms, cudaStream_t s);
 int nb_upd_combine_bwd(const float* gq, const float* gmu, const float* y, const float* VW, int n_atoms, float* gy, float* gVW,
                        cudaStream_t s);
 int nb_upd_norm_bwd(const float* gn, const float* VW, const float* nrm, int n_atoms, float* gVW, cudaStream_t s);

@@ -110,7 +110,8 @@ __global__ void __launch_bounds__(TN_THREADS) k_upd_norm_tan(const float* __rest
     st4(t_nrm + (size_t)i * NB_F + c, div4(s, ldg4(nrm + (size_t)i * NB_F + c)));
 }
 
-// tangent of k_upd_combine (y is the stored, biased y; t_y has no bias): q^ += y0^ + y2^ S + y2 S^ ; mu^[x] += y1^ Wv[x] + y1 Wv^[x]
+// tangent of the update combine q += y0 + y2 S, mu[x] += y1 Wv[x], S = <V, Wv> (y is the stored, biased y; t_y has no bias):
+// q^ += y0^ + y2^ S + y2 S^ ; mu^[x] += y1^ Wv[x] + y1 Wv^[x]
 __global__ void __launch_bounds__(TN_THREADS) k_upd_combine_tan(float* __restrict__ t_q, float* __restrict__ t_mu, const float* __restrict__ VW,
                                                                const float* __restrict__ t_VW, const float* __restrict__ y,
                                                                const float* __restrict__ t_y, int n_atoms) {

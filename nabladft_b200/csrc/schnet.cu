@@ -212,7 +212,6 @@ struct SWorkspace {
     float *y[16], *t[16];
     float *x, *agg, *act, *ro_pre, *eps, *mu_dummy;
     float *gx, *gt, *gagg, *gy, *g_ro, *egrad;
-    void* blas_ws;
     int64_t bytes;
 };
 
@@ -246,7 +245,6 @@ SWorkspace s_carve(void* p, int L, int64_t N, int64_t E, bool forces) {
         w.g_ro = c.take<float>(N * (F / 2));
         w.egrad = c.take<float>(4 * E);
     }
-    w.blas_ws = c.take<char>(kBlasWs);
     w.bytes = (c.off + kAlign - 1) / kAlign * kAlign;
     return w;
 }
@@ -278,8 +276,6 @@ extern "C" int nb200_schnet_energy_forces(nb200_engine* eng, const nb200_schnet_
     SWorkspace ws = s_carve(workspace, L, N, e_cap, want_f);
     if (ws.bytes > workspace_bytes) return NB200_EINVAL;
     cudaStream_t s = (cudaStream_t)stream;
-    if (cublasSetStream(eng->blas, s) != CUBLAS_STATUS_SUCCESS || cublasSetWorkspace(eng->blas, ws.blas_ws, kBlasWs) != CUBLAS_STATUS_SUCCESS)
-        return NB200_ECUDA;
 
     { Scope sc(eng, s, CAT_NBR, 3);
     NB_TRY(nb200_neighbor_build(pos, mol_ptr, n_mol, N, w->cutoff, 0x7fffffff, e_cap, ws.row_ptr, ws.col, ws.rev, ws.geom, ws.deg, status, s)); }

@@ -1,6 +1,6 @@
 """Host-side driver of the PaiNN energy+forces engine (`nb200_painn_energy_forces`).
 
-Owns: the C engine object (cuBLAS handle), the device workspace, the canonical weight export.
+Owns: the C engine object, the device workspace, the canonical weight export.
 The model classes (`painn_oc.PaiNN`, `spk.NeuralNetworkPotential`) only describe how their
 reference-named parameters map onto the canonical layout.
 """
@@ -127,7 +127,8 @@ class PainnEngine:
     GRAD_KEYS = ("emb", "w_rbf", "b_rbf", "A1", "c1", "A2", "c2", "U", "B1", "d1", "B2", "d2", "R1", "e1", "R2", "e2")
 
     def run_train(self, z, pos, mol_ptr, n_mol, seed: Optional[torch.Tensor], force_seed: Optional[torch.Tensor] = None):
-        """One training step of the PaiNN engine (`nb200_painn_energy_forces_grads`): energy, true forces and
+        """One training step of the PaiNN engine in one call (`nb200_painn_energy_forces_grads`: the fused forward of
+        `run_train_forward`, then the backward of `run_train_backward`): energy, true forces and
         d(sum_m seed_m E_m + sum_i force_seed_i . F_i)/d(canonical weights) as a dict of fresh tensors shaped like the exported weights.
         The first call of an engine is synchronous (checks the device status; regrows the edge capacity once like `run`); later calls
         enqueue and defer the status check like `run_async`."""

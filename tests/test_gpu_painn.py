@@ -424,41 +424,47 @@ def test_linear_wgrad_matches_fp64(M, out, inn, terms, bias, scale_div, lddw_ext
         assert errb < 2e-6 * G0.abs().sum(0).max().item(), f"bias err {errb:.2e}"
 
 
-def test_engine_gemm_backends_agree():
-    """Whole-model E,F with the wgmma GEMMs vs the cuBLAS SGEMM path: both within tolerance of each other."""
+def test_backend_setters_accept_only_the_remaining_paths():
+    """The node GEMMs are the wgmma kernels and the PaiNN node forward is the fused one: nb200_engine_set_gemm_backend and
+    nb200_engine_set_node_backend accept 1, refuse 0 (the cuBLAS SGEMM and one-launch-per-op paths, which no longer exist) with
+    NB200_EUNSUPPORTED and any other value with NB200_EINVAL, and a PaiNN call after them returns bitwise what it returned before."""
     net = _oc_model(6).to(dev())
     z, pos, batch = load_fixture([30, 31, 32], torch.float32)
     d = _Data(z.to(dev()), pos.to(dev()), batch.to(dev()))
     e1, f1 = net(d)
     eng = net.engine()
-    _lib_check = eng.lib.nb200_engine_set_gemm_backend(eng._h, 0)
-    assert _lib_check == 0
+    for setter in (eng.lib.nb200_engine_set_gemm_backend, eng.lib.nb200_engine_set_node_backend):
+        assert setter(eng._h, 0) == -2
+        assert setter(eng._h, 2) == -1
+        assert setter(eng._h, 1) == 0
     e0, f0 = net(d)
-    eng.lib.nb200_engine_set_gemm_backend(eng._h, 1)
-    print("backend diff: dE", (e1 - e0).abs().max().item(), "dF", (f1 - f0).abs().max().item())
-    assert (e1 - e0).abs().max() < E_TOL and (f1 - f0).abs().max() < F_TOL
+    assert torch.equal(e1, e0) and torch.equal(f1, f0)
 
 
-def test_fused_node_backend_matches_unfused_at_cfg2_size():
-    """The fused per-layer node kernels (painn_fused.cu) against the one-launch-per-Linear sequence they replace, whole model, BASELINE
-    config 2 size (256 synthetic conformations, ragged last 128-atom tile) and a 2-molecule batch (single partial tile)."""
+def test_fused_node_forward_at_cfg2_size():
+    """The fused per-layer node kernels (painn_fused.cu), whole model, at BASELINE config 2 size (256 synthetic conformations, ragged last
+    128-atom tile) and on a 2-molecule batch (single partial tile): finite and bitwise deterministic, and the 2-molecule batch matches the
+    fp64 oracle (at 256 molecules test_cfg2_slice_values_match_oracle[oc] checks the values of the same model and batch)."""
     from nabladft_b200.synth import synth_batch
+    from oracle.painn_oc import PaiNNOC
 
-    net = _oc_model(6).to(dev())
-    eng = net.engine()
+    net = _oc_model(6)
+    ref = PaiNNOC(hidden_channels=128, num_layers=6, num_rbf=100, cutoff=5.0, max_neighbors=100, num_elements=100).double()
+    ref.load_state_dict({k: v.double() for k, v in net.state_dict().items()}, strict=True)
+    net = net.to(dev())
     for n_mol in (256, 2):
         b = synth_batch(0, n_mol)
         d = _Data(torch.from_numpy(b["z"]).to(dev()), torch.from_numpy(b["pos"]).to(dev()), torch.from_numpy(b["batch"]).to(dev()))
-        assert eng.lib.nb200_engine_set_node_backend(eng._h, 1) == 0
         e1, f1 = net(d)
         e1b, f1b = net(d)
-        assert eng.lib.nb200_engine_set_node_backend(eng._h, 0) == 0
-        e0, f0 = net(d)
-        eng.lib.nb200_engine_set_node_backend(eng._h, 1)
-        print(f"fused vs unfused, {n_mol} molecules: dE {(e1 - e0).abs().max().item():.2e} Ha (|E| <= {e0.abs().max().item():.1f}), dF {(f1 - f0).abs().max().item():.2e} Ha/A")
         assert torch.isfinite(e1).all() and torch.isfinite(f1).all()
         assert torch.equal(e1, e1b) and torch.equal(f1, f1b)  # deterministic
-        assert (e1 - e0).abs().max() < E_TOL and (f1 - f0).abs().max() < F_TOL
+        if n_mol == 2:
+            e_ref, f_ref = ref(torch.from_numpy(b["z"]).long(), torch.from_numpy(b["pos"]).double(), torch.from_numpy(b["batch"]).long())
+            de = (e1.double().cpu() - e_ref.detach()).abs().max().item()
+            df = (f1.double().cpu() - f_ref.detach()).abs().max().item()
+            print(f"fused vs fp64 oracle, {n_mol} molecules: dE {de:.2e} Ha (|E| <= {e_ref.abs().max().item():.1f}), dF {df:.2e} Ha/A")
+            assert de < E_TOL and df < F_TOL
 
 
 @pytest.mark.parametrize("flavour", ["oc", "spk"])
@@ -513,8 +519,7 @@ def _spk_schnet_model(n_interactions=6):
     return m.eval()
 
 
-@pytest.mark.parametrize("gemm_backend", [1, 0])
-def test_spk_schnet_engine_matches_oracle(gemm_backend):
+def test_spk_schnet_engine_matches_oracle():
     """SchNet (config/model/schnet.yaml) E+F through the CUDA path vs the fp64 oracle; also energy-only
     (BASELINE config 1 is SchNet energy-only)."""
     from oracle.graph import ase_neighbor_list, batch_to_ptr
@@ -529,14 +534,12 @@ def test_spk_schnet_engine_matches_oracle(gemm_backend):
     idx_i, idx_j = ase_neighbor_list(pos, batch_to_ptr(batch), 5.0)
     out_ref = ref({"_atomic_numbers": z, "_positions": pos.clone(), "_idx_i": idx_i, "_idx_j": idx_j, "_idx_m": batch})
     model = model.to(dev())
-    eng = model.engine(True)
-    eng.lib.nb200_engine_set_gemm_backend(eng._h, gemm_backend)
     inp = {"_atomic_numbers": z.to(dev()), "_positions": pos.float().to(dev()), "_idx_m": batch.to(dev()), "_n_atoms": torch.bincount(batch).to(dev())}
     out = model(inp)
     e_ref, f_ref = out_ref["energy"].detach().numpy(), out_ref["forces"].numpy()
     de = np.abs(out["energy"].cpu().numpy() - e_ref).max()
     df = np.abs(out["forces"].cpu().numpy() - f_ref).max()
-    print(f"schnet backend {gemm_backend}: |E| {np.abs(e_ref).max():.3f} dE {de:.2e} |F| {np.abs(f_ref).max():.3f} dF {df:.2e}")
+    print(f"schnet: |E| {np.abs(e_ref).max():.3f} dE {de:.2e} |F| {np.abs(f_ref).max():.3f} dF {df:.2e}")
     assert de < E_TOL and df < F_TOL
     model._forces = False
     out_e = model(inp)

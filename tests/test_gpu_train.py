@@ -194,8 +194,8 @@ def test_gradient_step_reduces_energy_mse_as_predicted():
 def test_two_call_training_step_matches_the_recomputing_path():
     """The training forward keeps its activations in the engine workspace and the backward call builds the gradients from them
     (nb200_painn_train_forward / _backward); a second forward on the same engine before the backward invalidates the kept state and the
-    backward falls back to the one-call form that recomputes.  Both must give the same gradients (the node layers run as fused kernels in
-    the kept forward and as separate GEMMs in the recomputing call: agreement at the 1e-5 level of each tensor's largest entry)."""
+    backward falls back to the one-call form that recomputes.  Both must give the same gradients (both run the fused node forward; the
+    weight-gradient kernels accumulate with atomics, so their sums are reordered: agreement within 5e-5 of each tensor's largest entry)."""
     z, pos, batch = load_fixture([0, 4, 7, 9])
     g = torch.Generator().manual_seed(11)
     e_t = torch.tensor([-9.0, -12.0, -10.5, -8.0])
