@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+
 #include "../../include/nabla_b200.h"
 
 #define NB_F 128          // hidden size of every SchNet/PaiNN config in the reference
@@ -16,10 +18,20 @@
 
 extern thread_local int g_nb200_last_cuda_error;
 
-// streaming multiprocessors of the current device (queried once per process): grid sizing of the persistent / grid-stride launches
+constexpr int NB_MAX_DEVICES = 64;
+
+// streaming multiprocessors of the current device (queried once per device): grid sizing of the persistent / grid-stride launches and the
+// tile width of the fused PaiNN node kernels
 static inline int nb_sm_count() {
-    static const int n = [] { int dev = 0, v = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev); return v > 0 ? v : 132; }();
-    return n;
+    static std::atomic<int> cache[NB_MAX_DEVICES];  // 0: not queried yet
+    int dev = 0, v = 0;
+    cudaGetDevice(&dev);
+    const bool cached = dev >= 0 && dev < NB_MAX_DEVICES;
+    if (cached && (v = cache[dev].load(std::memory_order_relaxed)) > 0) return v;
+    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    v = v > 0 ? v : 132;
+    if (cached) cache[dev].store(v, std::memory_order_relaxed);
+    return v;
 }
 
 static inline int nb_check_launch() {

@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
     if (warp >= WARP_ISSUE) {
         run_issuer_t(c, n_units, flags_of, [&](int u) { return (t_begin + u / KC) * KC + u % KC; }, P.wt, P.spt);
     } else {
-        const int M = P.M, m0 = blockIdx.x * NT;
+        const int M = P.M, m0 = blockIdx.x * L::NT;
         const int fl = 32 * (warp & 3) + lane, n0 = L::CPT * (warp >> 2);
         // epilogue warps [0, NEPI), loader warps [NWORK - NLOAD, NWORK): with one group every worker warp is both
         const bool isE = warp < L::NEPI, isL = warp >= NWORK - L::NLOAD;
@@ -149,7 +149,7 @@ int gemm_ps_ready(void*& ws, size_t need, cudaStream_t s) {
     }
     static bool attr = false;
     if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_ps<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL) != cudaSuccess) return nb_check_launch();
+        if (cudaFuncSetAttribute(k_gemm_ps<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_TOTAL) != cudaSuccess) return nb_check_launch();
         attr = true;
     }
     return NB200_OK;
@@ -183,13 +183,14 @@ static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const floa
     P.C = C; P.ldc = ldc; P.accumulate = accumulate; P.bias = bias; P.act = act; P.act_kind = act_kind;
     P.spt = KC == 1 ? (K + KSTAGE - 1) / KSTAGE : STAGES_PER_TILE;
     P.epi = epi; P.epi_alpha = epi_alpha;
-    const int m_tiles = (M + NT - 1) / NT;
+    static_assert(OneGroup::NT == TwoGroups::NT, "one row tiling for both layouts");
+    const int m_tiles = (M + OneGroup::NT - 1) / OneGroup::NT;
     int ny = 1;
     while (m_tiles * ny < nb_sm_count() && ny < n_nt) ++ny;  // few row slabs: split the N walk (the activation slab is re-staged per CTA)
     P.tiles_per_cta = (n_nt + ny - 1) / ny;
     dim3 grid(m_tiles, (n_nt + P.tiles_per_cta - 1) / P.tiles_per_cta);
-    if (two_groups) k_gemm_ps<TwoGroups><<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
-    else k_gemm_ps<OneGroup><<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
+    if (two_groups) k_gemm_ps<TwoGroups><<<grid, NTHREADS, TwoGroups::SMEM_TOTAL, s>>>(P);
+    else k_gemm_ps<OneGroup><<<grid, NTHREADS, OneGroup::SMEM_TOTAL, s>>>(P);
     return nb_check_launch();
 }
 
@@ -229,7 +230,7 @@ int nb_gemm_ps_lm(int M, int N, int K, const float* A, int lda, const float* W_l
     P.spt = KC == 1 ? (K + KSTAGE - 1) / KSTAGE : STAGES_PER_TILE;
     P.lm_batch = 1; P.a_boff = K; P.c_boff = N; P.w_boff = (long long)per_w;
     P.tiles_per_cta = n_nt;
-    dim3 grid((M + NT - 1) / NT, 1, n_lm);
-    k_gemm_ps<OneGroup><<<grid, NTHREADS, SMEM_TOTAL, s>>>(P);
+    dim3 grid((M + OneGroup::NT - 1) / OneGroup::NT, 1, n_lm);
+    k_gemm_ps<OneGroup><<<grid, NTHREADS, OneGroup::SMEM_TOTAL, s>>>(P);
     return nb_check_launch();
 }

@@ -8,19 +8,19 @@
 // layer and direction, each re-staging and re-splitting its activation slab.
 //
 // Design (the pipeline itself is tc_pipe.cuh):
-//   * CTA = 64 atoms.  Every GEMM of the chain is computed TRANSPOSED: D[feature, atom] = W[feature, k] . X[atom, k]^T, i.e. the weight
-//     tile is the MMA's A operand (M = 128 output features, two warpgroups of 64) and the activations are the B operand (N = 64 atoms).
-//     The staged result has features on rows and atoms on columns: an epilogue thread owns one feature and 32 atoms, so every global
+//   * CTA = NT = 64 or 80 atoms (wide_tiles).  Every GEMM of the chain is computed TRANSPOSED: D[feature, atom] = W[feature, k] . X[atom, k]^T,
+//     i.e. the weight tile is the MMA's A operand (M = 128 output features, two warpgroups of 64) and the activations are the B operand (N = NT atoms).
+//     The staged result has features on rows and atoms on columns: an epilogue thread owns one feature and NT / 2 atoms, so every global
 //     store / load of an [atom][feature] array is a 128-byte coalesced warp access, the bias is a per-thread scalar, and writing the next
 //     activation operand into shared memory ([atoms] x K, K-major) is a conflict-free 4-byte store pattern.
 //   * weights are split into TF32 hi / lo ONCE per call by k_prep_painn into ready-made shared-memory images (one 128 x 128 tile =
 //     4 stages x [hi | lo] x 16 KB, canonical no-swizzle K-major), streamed with one cp.async.bulk per stage through a 3-stage mbarrier ring.
-//   * the activation operand X [64 atoms x 128 k] (hi + lo) is written by the 8 worker warps: either by a LOADER functor (coalesced global
+//   * the activation operand X [NT atoms x 128 k] (hi + lo) is written by the 8 worker warps: either by a LOADER functor (coalesced global
 //     loads, elementwise math fused in: sqrt-norm, the combine backward, silu' ...) or directly from the previous GEMM's epilogue registers
 //     (silu(h) -> next operand) -- chained activations never go through global memory to be re-read as operands.
 //   * 3xTF32: lo.hi + hi.lo into a correction accumulator, hi.hi alternating over two main accumulators so that no accumulator chain is
 //     longer than 8 per 128 k (the tensor core truncates on accumulate, see gemm_tc.cu); the MMA warpgroups sum them into a shared-memory
-//     staging tile, which the epilogues walk in 16-atom chunks inside ROLLED loops (compact code).  K > 128 (backward) accumulates over
+//     staging tile, which the epilogues walk in 16-atom (NT = 80: 8-atom) chunks inside ROLLED loops (compact code).  K > 128 (backward) accumulates over
 //     several X operands in place.
 //   * roles meet only through mbarriers: W ring full/empty, X ready/free, staging full / free.
 // Forward  kernel = update(l) [+ message MLP(l+1) | readout Linear]
@@ -116,7 +116,10 @@ struct FwdParams {
     float* ro_pre;  // readout: [N, F/2] WITHOUT the bias e1 (k_readout adds it)
 };
 
+// L: Node64 / Node80 (the atoms per CTA, see launch_tiles)
+template <class L>
 __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdParams P) {
+    constexpr int CW = L::CW;
     extern __shared__ __align__(1024) unsigned char smem[];
     __shared__ Prog prog;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -141,14 +144,16 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
         }
         if (P.do_ro) prog_add(prog, P.tile_ro, U_NEWX | U_FIRST | U_LAST | U_XLAST);
     }
-    Ctx<OneGroup> c = setup<OneGroup>(smem, tid);  // every worker warp loads operands and runs epilogues
+    Ctx<L> c = setup<L>(smem, tid);  // every worker warp loads operands and runs epilogues
 
     if (warp >= WARP_ISSUE) {
+        role_regs<L>(true);
         run_issuer(c, prog, P.wt);
     } else {
-        const int N = P.n_atoms, A0 = blockIdx.x * NT;
+        role_regs<L>(false);
+        const int N = P.n_atoms, A0 = blockIdx.x * L::NT;
         const int fl = 32 * (warp & 3) + lane;   // my feature inside a 128-row weight tile
-        const int n0 = OneGroup::CPT * (warp >> 2);  // my first atom column
+        const int n0 = L::CPT * (warp >> 2);  // my first atom column
         if (P.do_upd) {
             // ---- VW[(atom, x)] = mu_mid[(atom, x)] . U^T : V half, W half per cartesian component
 #pragma unroll 1
@@ -157,11 +162,11 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
 #pragma unroll 1
                 for (int half = 0; half < 2; ++half) {
                     drain(c, warp);
-                    epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                        float* dst = P.VW + (size_t)(A0 + n0 + 16 * cb) * (6 * F) + x * 2 * F + half * F + fl;
+                    epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                        float* dst = P.VW + (size_t)(A0 + n0 + CW * cb) * (6 * F) + x * 2 * F + half * F + fl;
 #pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            if (A0 + n0 + 16 * cb + j < N) dst[(size_t)j * (6 * F)] = v[j];
+                        for (int j = 0; j < CW; ++j)
+                            if (A0 + n0 + CW * cb + j < N) dst[(size_t)j * (6 * F)] = v[j];
                     });
                 }
             }
@@ -173,18 +178,18 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 //  shared memory per CTA little L1 is left for local memory)
                 const int kc = tid & 31, w = tid >> 5;
 #pragma unroll 1
-                for (int it0 = 0; it0 < OneGroup::RPT; it0 += 2) {
+                for (int it0 = 0; it0 < L::RPT; it0 += 2) {
                     float4 V[2][3], Wv[2][3];
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
-                        const int a = A0 + w + OneGroup::NLOAD * (it0 + b);
+                        const int a = A0 + w + L::NLOAD * (it0 + b);
                         const float* vv = P.VW + (size_t)min(a, N - 1) * (6 * F) + 4 * kc;
 #pragma unroll
                         for (int x = 0; x < 3; ++x) { V[b][x] = ld4(vv + x * 2 * F); Wv[b][x] = ld4(vv + x * 2 * F + F); }
                     }
 #pragma unroll
                     for (int b = 0; b < 2; ++b) {
-                        const int a = A0 + w + OneGroup::NLOAD * (it0 + b);
+                        const int a = A0 + w + L::NLOAD * (it0 + b);
                         if (a < N) {
                             float4 sq = V[b][0] * V[b][0]; fma4(sq, V[b][1], V[b][1]); fma4(sq, V[b][2], V[b][2]);
                             float4 dt = f4(0.f); fma4(dt, V[b][0], Wv[b][0]); fma4(dt, V[b][1], Wv[b][1]); fma4(dt, V[b][2], Wv[b][2]);
@@ -201,16 +206,16 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 drain(c, warp, 1);   // + nrm half
                 const float b = __ldg(P.d1 + fl);
                 const XPut xp(c, fl);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {   // operand first: the tensor core restarts before anything is stored
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {   // operand first: the tensor core restarts before anything is stored
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, A0 + n0 + 16 * cb + j < N ? siluf_(v[j] + b) : 0.f);
+                    for (int j = 0; j < CW; ++j) xp.put(n0 + CW * cb + j, A0 + n0 + CW * cb + j < N ? siluf_(v[j] + b) : 0.f);
                 });
                 xp.done(c);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float* g = P.g1pre + (size_t)(A0 + n0 + 16 * cb) * F + fl;
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                    float* g = P.g1pre + (size_t)(A0 + n0 + CW * cb) * F + fl;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) g[(size_t)j * F] = v[j] + b;
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) g[(size_t)j * F] = v[j] + b;
                 });
             }
             // ---- y = silu(g1pre) . B2^T + d2, tiles in the order (gate y1, scalar y0, dot-scale y2)
@@ -218,9 +223,9 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 drain(c, warp);
                 const float b = __ldg(P.d2 + F + fl);
 #pragma unroll 1
-                for (int cb = 0; cb < OneGroup::CPT / 8; ++cb) {  // 8 atoms per round: 48 loads in flight per thread
-                    float v16[16];
-                    stage_ld16(c, warp, cb >> 1, v16);
+                for (int cb = 0; cb < L::CPT / 8; ++cb) {  // 8 atoms per round: 48 loads in flight per thread
+                    float v8[8];
+                    stage_ld(c, warp, 8 * cb, v8);
                     float tw[8][3], tm[8][3];
 #pragma unroll
                     for (int jj = 0; jj < 8; ++jj) {
@@ -234,7 +239,7 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                     for (int jj = 0; jj < 8; ++jj) {
                         const int a = A0 + n0 + 8 * cb + jj;
                         if (a < N) {
-                            const float y1 = ((cb & 1) ? v16[8 + jj] : v16[jj]) + b;
+                            const float y1 = v8[jj] + b;
                             P.y[(size_t)a * (3 * F) + F + fl] = y1;
                             float* mo = P.mu_next + (size_t)a * (3 * F) + fl;
 #pragma unroll
@@ -246,13 +251,13 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
             {   // y0: stored, and q_next <- q_mid + y0 (completed by the y2 tile)
                 drain(c, warp);
                 const float b = __ldg(P.d2 + fl);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float t[16];
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                    float t[CW];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) t[j] = __ldg(P.q_mid + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
+                    for (int j = 0; j < CW; ++j) t[j] = __ldg(P.q_mid + (size_t)min(A0 + n0 + CW * cb + j, N - 1) * F + fl);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int a = A0 + n0 + 16 * cb + j;
+                    for (int j = 0; j < CW; ++j) {
+                        const int a = A0 + n0 + CW * cb + j;
                         if (a < N) {
                             const float y0 = v[j] + b;
                             P.y[(size_t)a * (3 * F) + fl] = y0;
@@ -265,30 +270,30 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 drain(c, warp);
                 const float b = __ldg(P.d2 + 2 * F + fl);
                 const XPut xp(c, fl);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float tq[16], td[16];
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                    float tq[CW], td[CW];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const size_t a = (size_t)min(A0 + n0 + 16 * cb + j, N - 1);
+                    for (int j = 0; j < CW; ++j) {
+                        const size_t a = (size_t)min(A0 + n0 + CW * cb + j, N - 1);
                         tq[j] = P.q_next[a * F + fl];
                         td[j] = P.dot[a * F + fl];
                     }
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int a = A0 + n0 + 16 * cb + j;
+                    for (int j = 0; j < CW; ++j) {
+                        const int a = A0 + n0 + CW * cb + j;
                         float qn = 0.f;
                         if (a < N) {
                             qn = fmaf(v[j] + b, td[j], tq[j]);
                             P.q_next[(size_t)a * F + fl] = qn;
                         }
-                        xp.put(n0 + 16 * cb + j, qn);
+                        xp.put(n0 + CW * cb + j, qn);
                     }
                 });
                 xp.done(c);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) P.y[(size_t)(A0 + n0 + 16 * cb + j) * (3 * F) + 2 * F + fl] = v[j] + b;
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) P.y[(size_t)(A0 + n0 + CW * cb + j) * (3 * F) + 2 * F + fl] = v[j] + b;
                 });
             }
         } else {
@@ -299,36 +304,36 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_fwd(const FwdPar
                 drain(c, warp);
                 const float b = __ldg(P.c1 + fl);
                 const XPut xp(c, fl);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, siluf_(v[j] + b));
+                    for (int j = 0; j < CW; ++j) xp.put(n0 + CW * cb + j, siluf_(v[j] + b));
                 });
                 xp.done(c);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) P.h1pre[(size_t)(A0 + n0 + 16 * cb + j) * F + fl] = v[j] + b;
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) P.h1pre[(size_t)(A0 + n0 + CW * cb + j) * F + fl] = v[j] + b;
                 });
             }
 #pragma unroll 1
             for (int ct = 0; ct < 3; ++ct) {  // xh = act . A2^T  (bias c2 is added inside the message kernel)
                 drain(c, warp);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float* dst = P.xh + (size_t)(A0 + n0 + 16 * cb) * (3 * F) + ct * F + fl;
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                    float* dst = P.xh + (size_t)(A0 + n0 + CW * cb) * (3 * F) + ct * F + fl;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) dst[(size_t)j * (3 * F)] = v[j];
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) dst[(size_t)j * (3 * F)] = v[j];
                 });
             }
         }
         if (P.do_ro) {
             drain(c, warp);
-            epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
+            epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
                 if (fl < F / 2) {
-                    float* dst = P.ro_pre + (size_t)(A0 + n0 + 16 * cb) * (F / 2) + fl;
+                    float* dst = P.ro_pre + (size_t)(A0 + n0 + CW * cb) * (F / 2) + fl;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) dst[(size_t)j * (F / 2)] = v[j];
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) dst[(size_t)j * (F / 2)] = v[j];
                 }
             });
         }
@@ -348,7 +353,9 @@ struct BwdParams {
     const float *y, *VW, *nrm, *g1pre;
 };
 
+template <class L>
 __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdParams P) {
+    constexpr int CW = L::CW;
     extern __shared__ __align__(1024) unsigned char smem[];
     __shared__ Prog prog;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -374,14 +381,16 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
             }
         }
     }
-    Ctx<OneGroup> c = setup<OneGroup>(smem, tid);  // every worker warp loads operands and runs epilogues
+    Ctx<L> c = setup<L>(smem, tid);  // every worker warp loads operands and runs epilogues
 
     if (warp >= WARP_ISSUE) {
+        role_regs<L>(true);
         run_issuer(c, prog, P.wt);
     } else {
-        const int N = P.n_atoms, A0 = blockIdx.x * NT;
+        role_regs<L>(false);
+        const int N = P.n_atoms, A0 = blockIdx.x * L::NT;
         const int fl = 32 * (warp & 3) + lane;
-        const int n0 = OneGroup::CPT * (warp >> 2);
+        const int n0 = L::CPT * (warp >> 2);
         if (P.do_mlp) {
             // ---- gt = g_xh . A2 (K = 384) ; gt *= silu'(h1pre) ; gq_b = gq_a + gt . A1
 #pragma unroll 1
@@ -389,12 +398,12 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
                 load_x(c, tid, [&](int r, int kc) { return A0 + r < N ? ldg4(P.g_xh + (size_t)(A0 + r) * (3 * F) + ck * F + 4 * kc) : f4(0.f); });
             drain(c, warp);
             const XPut xp(c, fl);
-            epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                float t[16];
+            epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                float t[CW];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) t[j] = __ldg(P.h1pre + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
+                for (int j = 0; j < CW; ++j) t[j] = __ldg(P.h1pre + (size_t)min(A0 + n0 + CW * cb + j, N - 1) * F + fl);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, A0 + n0 + 16 * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
+                for (int j = 0; j < CW; ++j) xp.put(n0 + CW * cb + j, A0 + n0 + CW * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
             });
             xp.done(c);
         } else if (P.do_ro) {
@@ -407,17 +416,17 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
         }
         if (P.do_mlp || P.do_ro) {  // gq_b = dE/dq_in of the layer above; gdot = gq_b * y2 is what the combine backward needs three times
             drain(c, warp);
-            epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                float t[16], ty[16];
+            epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                float t[CW], ty[CW];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const size_t a = (size_t)min(A0 + n0 + 16 * cb + j, N - 1);
+                for (int j = 0; j < CW; ++j) {
+                    const size_t a = (size_t)min(A0 + n0 + CW * cb + j, N - 1);
                     t[j] = P.do_mlp ? P.gq_a[a * F + fl] : 0.f;
                     ty[j] = P.do_upd ? __ldg(P.y + a * (3 * F) + 2 * F + fl) : 0.f;
                 }
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int a = A0 + n0 + 16 * cb + j;
+                for (int j = 0; j < CW; ++j) {
+                    const int a = A0 + n0 + CW * cb + j;
                     if (a < N) {
                         const float g = t[j] + v[j];
                         P.gq_b[(size_t)a * F + fl] = g;
@@ -444,34 +453,34 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
             });
             drain(c, warp);
             const XPut xp(c, fl);
-            epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                float t[16];
+            epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                float t[CW];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) t[j] = __ldg(P.g1pre + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
+                for (int j = 0; j < CW; ++j) t[j] = __ldg(P.g1pre + (size_t)min(A0 + n0 + CW * cb + j, N - 1) * F + fl);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) xp.put(n0 + 16 * cb + j, A0 + n0 + 16 * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
+                for (int j = 0; j < CW; ++j) xp.put(n0 + CW * cb + j, A0 + n0 + CW * cb + j < N ? v[j] * dsiluf_(t[j]) : 0.f);
             });
             xp.done(c);
             {   // gq_a = gq_b + gt . B1[:, :F]   (dE/dq_mid of this layer: what the message backward reads)
                 drain(c, warp);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float t[16];
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                    float t[CW];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) t[j] = P.gq_b[(size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl];
+                    for (int j = 0; j < CW; ++j) t[j] = P.gq_b[(size_t)min(A0 + n0 + CW * cb + j, N - 1) * F + fl];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) P.gq_a[(size_t)(A0 + n0 + 16 * cb + j) * F + fl] = t[j] + v[j];
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) P.gq_a[(size_t)(A0 + n0 + CW * cb + j) * F + fl] = t[j] + v[j];
                 });
             }
             {   // gn = gt . B1[:, F:], stored as s = gn / nrm (norm backward: gV_x += s V_x)
                 drain(c, warp);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float t[16];
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                    float t[CW];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) t[j] = __ldg(P.nrm + (size_t)min(A0 + n0 + 16 * cb + j, N - 1) * F + fl);
+                    for (int j = 0; j < CW; ++j) t[j] = __ldg(P.nrm + (size_t)min(A0 + n0 + CW * cb + j, N - 1) * F + fl);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) P.gn[(size_t)(A0 + n0 + 16 * cb + j) * F + fl] = v[j] / t[j];
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) P.gn[(size_t)(A0 + n0 + CW * cb + j) * F + fl] = v[j] / t[j];
                 });
             }
             work_barrier();  // s visible
@@ -493,22 +502,45 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_node_bwd(const BwdPar
                     return o;
                 });
                 drain(c, warp);
-                epi_chunks(c, warp, [&](int cb, float (&v)[16]) {
-                    float t[16];
+                epi_chunks(c, warp, [&](int cb, float (&v)[CW]) {
+                    float t[CW];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) t[j] = P.cur[(size_t)min(A0 + n0 + 16 * cb + j, N - 1) * (3 * F) + x * F + fl];
+                    for (int j = 0; j < CW; ++j) t[j] = P.cur[(size_t)min(A0 + n0 + CW * cb + j, N - 1) * (3 * F) + x * F + fl];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (A0 + n0 + 16 * cb + j < N) P.cur[(size_t)(A0 + n0 + 16 * cb + j) * (3 * F) + x * F + fl] = t[j] + v[j];
+                    for (int j = 0; j < CW; ++j)
+                        if (A0 + n0 + CW * cb + j < N) P.cur[(size_t)(A0 + n0 + CW * cb + j) * (3 * F) + x * F + fl] = t[j] + v[j];
                 });
             }
         }
     }
 }
 
-template <class K>
-int set_smem(K kernel) {
-    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL) == cudaSuccess ? NB200_OK : nb_check_launch();
+using Node64 = Layout<false, 64>;
+using Node80 = Layout<false, 80>;
+
+// Atoms per CTA.  A CTA takes a whole SM (shared memory), so the grid runs in waves of one CTA per SM, and a last wave takes about as long
+// as a full one however few CTAs it holds (9,750 atoms: 153 CTAs of 64 atoms on 132 SMs, the second wave on 21).  An 80-atom CTA streams
+// the same weight tiles and a full wave of them takes about 1.2x as long as a full wave of 64-atom CTAs (DESIGN.md §3), so 80-atom tiles
+// pay off exactly when they need fewer waves; at the same number of waves 64-atom tiles are faster.
+bool wide_tiles(int n_atoms) {
+    const int sm = nb_sm_count();
+    const int waves64 = ((n_atoms + Node64::NT - 1) / Node64::NT + sm - 1) / sm, waves80 = ((n_atoms + Node80::NT - 1) / Node80::NT + sm - 1) / sm;
+    return waves80 < waves64;
+}
+
+// launch of a fused node kernel instantiated for layout L (its shared-memory limit is raised once per kernel and device)
+template <class L, class Params>
+int launch_tiles(void (*kernel)(Params), const Params& P, int n_atoms, cudaStream_t s) {
+    static std::atomic<bool> attr[NB_MAX_DEVICES];
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const bool cached = dev >= 0 && dev < NB_MAX_DEVICES;
+    if (!cached || !attr[dev].load(std::memory_order_relaxed)) {
+        if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_TOTAL) != cudaSuccess) { nb_check_launch(); return NB200_ECUDA; }
+        if (cached) attr[dev].store(true, std::memory_order_relaxed);
+    }
+    kernel<<<(n_atoms + L::NT - 1) / L::NT, NTHREADS, L::SMEM_TOTAL, s>>>(P);
+    return nb_check_launch();
 }
 
 }  // namespace
@@ -522,8 +554,6 @@ int nb_fused_prep(const nb200_painn_weights* w, void* wtiles, cudaStream_t s) {
 }
 
 int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s) {
-    static bool attr = false;
-    if (!attr) { if (set_smem(k_node_fwd) != NB200_OK) return NB200_ECUDA; attr = true; }
     FwdParams P{};
     // One worker group, whole-operand hand-over: the K-halves hand-over of tc_pipe.cuh's two-group layout gains nothing here, because most
     // operands of these kernels are written by the previous GEMM's epilogue, which cannot start earlier.
@@ -534,13 +564,10 @@ int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s) {
     P.q_next = a.q_next; P.mu_next = a.mu_next; P.eps = a.eps; P.q_mlp_in = a.q_mlp_in; P.c1 = a.c1; P.h1pre = a.h1pre; P.xh = a.xh;
     P.ro_pre = a.ro_pre;
     if (a.n_atoms <= 0) return NB200_OK;
-    k_node_fwd<<<(a.n_atoms + NT - 1) / NT, NTHREADS, SMEM_TOTAL, s>>>(P);
-    return nb_check_launch();
+    return wide_tiles(a.n_atoms) ? launch_tiles<Node80>(k_node_fwd<Node80>, P, a.n_atoms, s) : launch_tiles<Node64>(k_node_fwd<Node64>, P, a.n_atoms, s);
 }
 
 int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s) {
-    static bool attr = false;
-    if (!attr) { if (set_smem(k_node_bwd) != NB200_OK) return NB200_ECUDA; attr = true; }
     BwdParams P{};
     P.n_atoms = a.n_atoms; P.do_mlp = a.layer_mlp >= 0; P.do_ro = a.readout; P.do_upd = a.layer_upd >= 0;
     P.wt = static_cast<const unsigned char*>(a.wtiles);
@@ -548,6 +575,5 @@ int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s) {
     P.gq_a = a.gq_a; P.gq_b = a.gq_b; P.cur = a.cur; P.gn = a.gn; P.gdot = a.gdot; P.dot = a.dot; P.g_xh = a.g_xh; P.h1pre = a.h1pre; P.ro_pre = a.ro_pre; P.R2 = a.R2;
     P.y = a.y; P.VW = a.VW; P.nrm = a.nrm; P.g1pre = a.g1pre;
     if (a.n_atoms <= 0) return NB200_OK;
-    k_node_bwd<<<(a.n_atoms + NT - 1) / NT, NTHREADS, SMEM_TOTAL, s>>>(P);
-    return nb_check_launch();
+    return wide_tiles(a.n_atoms) ? launch_tiles<Node80>(k_node_bwd<Node80>, P, a.n_atoms, s) : launch_tiles<Node64>(k_node_bwd<Node64>, P, a.n_atoms, s);
 }

@@ -1,7 +1,7 @@
 // tc_pipe.cuh -- the warp-specialised wgmma pipeline shared by the fused PaiNN node kernels (painn_fused.cu) and the pre-split-weight GEMM
 // (gemm_ps.cu): weight tiles as ready-made TF32 hi / lo shared-memory images streamed by cp.async.bulk through an mbarrier ring, the
 // activation operand X written by worker warps (loader functors or epilogue registers), one MMA warpgroup (3xTF32: a correction and a main
-// accumulator in registers), a shared-memory staging tile of the summed accumulators, epilogues in rolled 16-column chunks.
+// accumulator in registers), a shared-memory staging tile of the summed accumulators, epilogues in rolled chunks of L::CW columns (16; 8 at NT = 80).
 // D[feature, row] = W[feature, k] . X[row, k]^T: features on the staging rows, rows (atoms / edges / pairs) on its columns.
 #pragma once
 #include "common.cuh"
@@ -11,24 +11,17 @@ namespace {
 
 
 constexpr int F = NB_F;
-// CTA = NT atoms, 8 worker warps, two MMA warpgroups (features [0, 64) and [64, 128) of a weight tile) whose first thread also issues the
-// weight copies (a separate producer warp made 17 warps, and ptxas then capped the registers at 96); 3 ring stages of 32 k.  An MMA
-// warpgroup holds its 64 features x NT atoms three times (correction + two alternating main accumulators: 96 fp32 registers per thread
-// at NT = 64; one warpgroup for all 128 features spilled), and the staging tile the epilogues read lives in shared memory next to the hi / lo activation operand and
-// the weight ring: 65 + 96 + 34 KB at NT = 64 (NT = 128 would not fit the 227 KB of an SM).
-constexpr int NT = 64, KSTAGE = 32, W_STAGES = 3, NWORK = 8, CTAS_PER_SM = 1;
-constexpr int XLBO = NT * 16 + 16;         // bytes between 16-byte k-chunks of X (padded: the 8 chunk writers of a row hit 8 bank groups)
-constexpr int XLBOF = XLBO / 4;
-constexpr int X_BYTES = 32 * XLBO;         // one of hi / lo, K = 128
+// CTA = NT atoms (the template parameter of Layout below), 8 worker warps, two MMA warpgroups (features [0, 64) and [64, 128) of a
+// weight tile) whose first thread also issues the weight copies (a separate producer warp made 17 warps, and ptxas then capped the
+// registers at 96); 3 ring stages of 32 k.  An MMA warpgroup holds its 64 features x NT atoms three times (correction + two alternating
+// main accumulators: 3 NT / 2 fp32 registers per thread; one warpgroup for all 128 features spilled), and the staging tile the epilogues
+// read lives in shared memory next to the hi / lo activation operand and the weight ring: 65 + 96 + 34 KB at NT = 64, 81 + 96 + 42 KB at
+// NT = 80 (NT = 128 would not fit the 227 KB of an SM).
+constexpr int KSTAGE = 32, W_STAGES = 3, NWORK = 8, CTAS_PER_SM = 1;
 constexpr int WLBO = 128 * 16;             // weight stages are written by the bulk-copy engine: no padding needed
 constexpr int WST_BYTES = 2 * (KSTAGE / 4) * WLBO;  // one ring stage: [hi | lo] x KSTAGE/4 chunks x 128 rows x 16 B
 constexpr int STAGES_PER_TILE = 128 / KSTAGE;
 constexpr int WTILE_BYTES = STAGES_PER_TILE * WST_BYTES;  // 128 rows x 128 k, hi + lo = 128 KB
-constexpr int SROW = NT + 4;               // staging row stride (floats): the 16-byte reads of 8 consecutive feature rows hit 8 bank groups
-constexpr int STAGE_BYTES = 128 * SROW * 4;
-constexpr int SMEM_BARS = 2 * X_BYTES + W_STAGES * WST_BYTES + STAGE_BYTES;
-constexpr int SMEM_TOTAL = SMEM_BARS + 256;
-static_assert(SMEM_TOTAL <= 227 * 1024, "shared memory of one CTA");
 // Worker layouts (the template parameter L of the pipeline below; the choice is fixed per kernel instantiation):
 //   OneGroup:  all NWORK worker warps load operands AND run epilogues, in program order; the operand is handed over whole.
 //   TwoGroups: warps [0, NEPI) only drain, run epilogues and write chained operands, warps [NEPI, NWORK) only run the loader functors and
@@ -36,18 +29,56 @@ static_assert(SMEM_TOTAL <= 227 * 1024, "shared memory of one CTA");
 //     (k < 64: x_ready / x_free, k >= 64: x_ready2 / x_free2), so that the next operand's first half is written while the MMAs still read
 //     the second half of the current one (and the MMAs start on the first half while the second is written): double buffering at
 //     half-operand granularity, no extra shared memory.
-template <bool TWO_GROUPS>
+// NT_: atoms (rows) per CTA, the N of every wgmma: 64, or 80 for the fused PaiNN node kernels when 64-atom tiles need more than one wave.
+template <bool TWO_GROUPS, int NT_ = 64>
 struct Layout {
     static constexpr bool two_groups = TWO_GROUPS;
+    static constexpr int NT = NT_;
     static constexpr int NEPI = TWO_GROUPS ? NWORK / 2 : NWORK, NLOAD = TWO_GROUPS ? NWORK / 2 : NWORK;
     static constexpr int CPT = NT / (NEPI / 4);  // staged columns (atoms) per epilogue thread (4 feature groups of 32 x NEPI/4 column parts)
+    // epilogue chunk: staged columns per round of epi_chunks (CPT = 40 at NT = 80: chunks of 20 spilled in 88 worker registers)
+    static constexpr int CW = CPT % 16 == 0 ? 16 : 8;
     static constexpr int RPT = NT / NLOAD;       // operand rows per loader thread
+    static constexpr int XLBO = NT * 16 + 16;    // bytes between 16-byte k-chunks of X (padded: the 8 chunk writers of a row hit 8 bank groups)
+    static constexpr int XLBOF = XLBO / 4;
+    static constexpr int X_BYTES = 32 * XLBO;    // one of hi / lo, K = 128
+    static constexpr int SROW = NT + 4;          // staging row stride (floats): the 16-byte reads of 8 consecutive feature rows hit 8 bank groups
+    static constexpr int STAGE_BYTES = 128 * SROW * 4;
+    static constexpr int SMEM_BARS = 2 * X_BYTES + W_STAGES * WST_BYTES + STAGE_BYTES;
+    static constexpr int SMEM_TOTAL = SMEM_BARS + 256;
+    // registers per thread of the worker / MMA warpgroups (setmaxnreg, see role_regs); 0: the even split of the launch (128 each).
+    // At NT = 80 an MMA thread holds 120 accumulators; 2 x 128 x (88 + 168) = the 64 K registers of the SM.
+    static constexpr int WORK_REGS = NT == 64 ? 0 : 88, MMA_REGS = NT == 64 ? 0 : 168;
+    static_assert(NT == 64 || NT == 80, "the wgmma N of the pipeline (wgmma_tf32_nt)");
+    static_assert(SMEM_TOTAL <= 227 * 1024, "shared memory of one CTA");
+    static_assert((XLBO / 16) % 2 == 1 && XLBO % 128 == 16, "X padding: 8 chunk writers of a row / 32 feature writers of a column hit distinct banks");
+    static_assert((SROW / 4) % 2 == 1, "staging padding: the 16-byte reads of 8 consecutive feature rows hit 8 bank groups");
+    static_assert(CPT % CW == 0 && CW % 4 == 0, "epilogue chunks");
+    static_assert(WORK_REGS + MMA_REGS == 0 || WORK_REGS + MMA_REGS == 2 * 128, "the register split must hand over exactly what it takes");
 };
 using OneGroup = Layout<false>;
 using TwoGroups = Layout<true>;
 constexpr int WARP_ISSUE = NWORK;          // first warp of the two MMA warpgroups (warpgroups start at a multiple of 4 warps)
 constexpr int NTHREADS = 32 * (NWORK + 8);
 static_assert(NWORK % 4 == 0, "the MMA warpgroups must start on a warpgroup boundary");
+static_assert(NWORK * 32 == NTHREADS / 2, "role_regs: the worker and MMA warpgroups hold the same number of threads");
+
+// Moves registers from the worker warpgroups to the MMA warpgroups (L::MMA_REGS > 0).  Called once by every thread at the role split; the
+// launch must give 128 registers per thread (__launch_bounds__(NTHREADS, 1)), so that the MMA side's increase is exactly what the workers
+// release (setmaxnreg.inc waits for free registers of the CTA).
+template <class L>
+__device__ __forceinline__ void role_regs(bool mma) {
+    if constexpr (L::MMA_REGS > 0) {
+        if (mma) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(L::MMA_REGS));
+        else asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(L::WORK_REGS));
+    }
+}
+
+template <int NT>
+__device__ __forceinline__ void wgmma_tf32_nt(float (&d)[NT / 2], uint64_t da, uint64_t db) {
+    if constexpr (NT == 64) wgmma_tf32_n64(d, da, db);
+    else wgmma_tf32_n80(d, da, db);
+}
 enum { U_NEWX = 1, U_FIRST = 2, U_LAST = 4, U_XLAST = 8 };
 
 struct Prog {
@@ -82,6 +113,7 @@ struct Ctx {
 // one cp.async.bulk per stage, W_STAGES ahead; a slot is refilled once both warpgroups have released it.
 template <class L, class FlagFn, class TileFn>
 __device__ __forceinline__ void run_issuer_t(Ctx<L>& c, int n_units, FlagFn flags_of, TileFn tile_of, const unsigned char* wt, int spt = STAGES_PER_TILE) {
+    constexpr int NT = L::NT, XLBO = L::XLBO;
     const int wl = ((threadIdx.x >> 5) - WARP_ISSUE) & 3, h = ((threadIdx.x >> 5) - WARP_ISSUE) >> 2, lane = threadIdx.x & 31;
     float corr[NT / 2], main0[NT / 2], main1[NT / 2];
     const uint32_t x_hi0 = s_u32(c.x_hi), x_lo0 = s_u32(c.x_lo);
@@ -123,10 +155,10 @@ __device__ __forceinline__ void run_issuer_t(Ctx<L>& c, int n_units, FlagFn flag
             for (int ks = 0; ks < KSTAGE / 8; ++ks) {
                 const uint64_t dxh = gmma_desc(x_hi0 + xoff + 2 * ks * XLBO, XLBO, 128), dxl = gmma_desc(x_lo0 + xoff + 2 * ks * XLBO, XLBO, 128);
                 const uint64_t dwh = gmma_desc(wh + 2 * ks * WLBO + h * 1024, WLBO, 128), dwl = gmma_desc(wlo + 2 * ks * WLBO + h * 1024, WLBO, 128);
-                wgmma_tf32_n64(corr, dwl, dxh);
-                wgmma_tf32_n64(corr, dwh, dxl);
-                if (ks & 1) wgmma_tf32_n64(main1, dwh, dxh);
-                else wgmma_tf32_n64(main0, dwh, dxh);
+                wgmma_tf32_nt<NT>(corr, dwl, dxh);
+                wgmma_tf32_nt<NT>(corr, dwh, dxl);
+                if (ks & 1) wgmma_tf32_nt<NT>(main1, dwh, dxh);
+                else wgmma_tf32_nt<NT>(main0, dwh, dxh);
             }
             wgmma_commit();
             wgmma_wait<1>();  // the previous stage's group has completed: free its ring slot
@@ -150,8 +182,8 @@ __device__ __forceinline__ void run_issuer_t(Ctx<L>& c, int n_units, FlagFn flag
 #pragma unroll
             for (int j = 0; j < NT / 8; ++j) {
                 const int n = 8 * j + 2 * (lane & 3);
-                *reinterpret_cast<float2*>(c.stage + f * SROW + n) = make_float2(corr[4 * j] + (main0[4 * j] + main1[4 * j]), corr[4 * j + 1] + (main0[4 * j + 1] + main1[4 * j + 1]));
-                *reinterpret_cast<float2*>(c.stage + (f + 8) * SROW + n) = make_float2(corr[4 * j + 2] + (main0[4 * j + 2] + main1[4 * j + 2]), corr[4 * j + 3] + (main0[4 * j + 3] + main1[4 * j + 3]));
+                *reinterpret_cast<float2*>(c.stage + f * L::SROW + n) = make_float2(corr[4 * j] + (main0[4 * j] + main1[4 * j]), corr[4 * j + 1] + (main0[4 * j + 1] + main1[4 * j + 1]));
+                *reinterpret_cast<float2*>(c.stage + (f + 8) * L::SROW + n) = make_float2(corr[4 * j + 2] + (main0[4 * j + 2] + main1[4 * j + 2]), corr[4 * j + 3] + (main0[4 * j + 3] + main1[4 * j + 3]));
             }
             mbar_arrive(c.acc_full);
             ++c.o;
@@ -163,14 +195,14 @@ __device__ __forceinline__ void run_issuer(Ctx<L>& c, const Prog& prog, const un
     run_issuer_t(c, prog.n, [&](int u) { return (int)prog.flag[u]; }, [&](int u) { return (int)prog.tile[u]; }, wt);
 }
 
-// worker warps: fill the activation operand with f(row 0..127 of the tile, chunk 0..31) -> 4 consecutive k values.
-// Two halves of 8 rows per thread (rolled).  Per half: ALL global loads are issued (and f's arithmetic done) BEFORE the thread waits for
-// the previous operand to be released, so their latency overlaps the MMAs still reading that operand; only split + 16 shared-memory
-// stores follow the wait.  (8 worker warps per SM: a load -> use -> store sequence per element would expose one L2 round trip each.)
+// worker warps: fill the activation operand with f(row 0..NT-1 of the tile, chunk 0..31) -> 4 consecutive k values.
+// One group: rounds of RB rows per thread (rolled; one round of 8 at NT = 64, two rounds of 5 at NT = 80).  Per round: ALL global loads are
+// issued (and f's arithmetic done) BEFORE the thread waits for the previous operand to be released, so their latency overlaps the MMAs still
+// reading that operand; only split + 2 RB shared-memory stores follow the wait.  (8 worker warps per SM: a load -> use -> store sequence per element would expose one L2 round trip each.)
 // wtid: the thread's index among the loader warps.
 template <class L, class Fn>
 __device__ __forceinline__ void load_x(Ctx<L>& c, int wtid, Fn f) {
-    constexpr int NLOAD = L::NLOAD;
+    constexpr int NLOAD = L::NLOAD, NT = L::NT, XLBOF = L::XLBOF;
     if constexpr (L::two_groups) {
         // half-operand hand-over: the two K halves must be written by DIFFERENT WARPS -- a warp whose lanes wait on two barriers reconverges
         // after the wait loop, i.e. both halves would wait for the later barrier (first version, by lane: no gain at all).  Warps [0, NLOAD/2)
@@ -197,16 +229,19 @@ __device__ __forceinline__ void load_x(Ctx<L>& c, int wtid, Fn f) {
         ++c.xg;
         return;
     }
+    // rows per round: 8, or 5 (two rounds) for the RPT = 10 rows of a thread at NT = 80 -- one round of 10 spilled in 88 worker registers
+    constexpr int RB = L::RPT % 8 == 0 ? 8 : L::RPT / 2;
+    static_assert(L::RPT % RB == 0, "load_x one-group mapping");
     const int kc = wtid & 31, w = wtid >> 5;
 #pragma unroll 1
-    for (int h = 0; h < L::RPT / 8; ++h) {
-        float4 t[8];
+    for (int h = 0; h < L::RPT / RB; ++h) {
+        float4 t[RB];
 #pragma unroll
-        for (int it = 0; it < 8; ++it) t[it] = f(w + NLOAD * (8 * h + it), kc);
+        for (int it = 0; it < RB; ++it) t[it] = f(w + NLOAD * (RB * h + it), kc);
         if (c.xg > 0) mbar_wait(c.x_free, (uint32_t)((c.xg - 1) & 1));  // every MMA that read the previous operand has retired
 #pragma unroll
-        for (int it = 0; it < 8; ++it) {
-            const int r = w + NLOAD * (8 * h + it);
+        for (int it = 0; it < RB; ++it) {
+            const int r = w + NLOAD * (RB * h + it);
             float4 hi, lo;
             split4(t[it], hi, lo);
             st4(c.x_hi + kc * XLBOF + r * 4, hi);
@@ -226,8 +261,8 @@ struct XPut {
     __device__ __forceinline__ XPut(const Ctx<L>& c, int k) {
         second = L::two_groups && k >= 64;
         if (c.xg > 0) mbar_wait(second ? c.x_free2 : c.x_free, (uint32_t)((c.xg - 1) & 1));
-        hi = c.x_hi + (k >> 2) * XLBOF + (k & 3);
-        lo = c.x_lo + (k >> 2) * XLBOF + (k & 3);
+        hi = c.x_hi + (k >> 2) * L::XLBOF + (k & 3);
+        lo = c.x_lo + (k >> 2) * L::XLBOF + (k & 3);
     }
     __device__ __forceinline__ void put(int n, float v) const {
         float h, l;
@@ -246,7 +281,7 @@ struct XPut {
 // add_stage: K > 128 split over two output tiles (forward g1pre): this thread's part of the previous tile is kept and added to the new one.
 template <class L>
 __device__ __forceinline__ void drain(Ctx<L>& c, int warp, int add_stage = 0) {
-    float* mine = c.stage + (32 * (warp & 3) + (threadIdx.x & 31)) * SROW + (warp >> 2) * L::CPT;
+    float* mine = c.stage + (32 * (warp & 3) + (threadIdx.x & 31)) * L::SROW + (warp >> 2) * L::CPT;
     if (add_stage) {
         float4 keep[L::CPT / 4];
 #pragma unroll
@@ -262,12 +297,12 @@ __device__ __forceinline__ void drain(Ctx<L>& c, int warp, int add_stage = 0) {
     ++c.o;
 }
 
-// 16 staged values of this thread: atoms CPT (warp >> 2) + 16 cb .. + 15 of its feature
-template <class L>
-__device__ __forceinline__ void stage_ld16(const Ctx<L>& c, int warp, int cb, float (&v)[16]) {
-    const float4* src = reinterpret_cast<const float4*>(c.stage + (32 * (warp & 3) + (threadIdx.x & 31)) * SROW + (warp >> 2) * L::CPT + cb * 16);
+// W staged values of this thread: atoms CPT (warp >> 2) + col .. + W - 1 of its feature (col, W multiples of 4)
+template <class L, int W>
+__device__ __forceinline__ void stage_ld(const Ctx<L>& c, int warp, int col, float (&v)[W]) {
+    const float4* src = reinterpret_cast<const float4*>(c.stage + (32 * (warp & 3) + (threadIdx.x & 31)) * L::SROW + (warp >> 2) * L::CPT + col);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < W / 4; ++i) {
         const float4 t = src[i];
         v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
     }
@@ -284,10 +319,10 @@ template <class L>
 __device__ __forceinline__ Ctx<L> setup(unsigned char* smem, int tid) {
     Ctx<L> c;
     c.x_hi = reinterpret_cast<float*>(smem);
-    c.x_lo = reinterpret_cast<float*>(smem + X_BYTES);
-    c.ring = smem + 2 * X_BYTES;
-    c.stage = reinterpret_cast<float*>(smem + 2 * X_BYTES + W_STAGES * WST_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SMEM_BARS);
+    c.x_lo = reinterpret_cast<float*>(smem + L::X_BYTES);
+    c.ring = smem + 2 * L::X_BYTES;
+    c.stage = reinterpret_cast<float*>(smem + 2 * L::X_BYTES + W_STAGES * WST_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::SMEM_BARS);
     c.full = bars; c.empty = bars + W_STAGES; c.x_ready = bars + 2 * W_STAGES; c.x_free = c.x_ready + 1; c.acc_full = c.x_ready + 2;
     c.stage_free = c.x_ready + 3; c.x_ready2 = c.x_ready + 4; c.x_free2 = c.x_ready + 5;
     if (tid == 0) {
@@ -307,13 +342,13 @@ __device__ __forceinline__ Ctx<L> setup(unsigned char* smem, int tid) {
     return c;
 }
 
-// epilogue loop over this thread's part of the staged tile: chunks of 16 atoms, rolled (one copy of the body in the instruction cache)
+// epilogue loop over this thread's part of the staged tile: chunks of L::CW atoms, rolled (one copy of the body in the instruction cache)
 template <class L, class Body>
 __device__ __forceinline__ void epi_chunks(const Ctx<L>& c, int warp, Body body) {
 #pragma unroll 1
-    for (int cb = 0; cb < L::CPT / 16; ++cb) {
-        float v[16];
-        stage_ld16(c, warp, cb, v);
+    for (int cb = 0; cb < L::CPT / L::CW; ++cb) {
+        float v[L::CW];
+        stage_ld(c, warp, L::CW * cb, v);
         body(cb, v);
     }
 }
