@@ -114,6 +114,27 @@ int nb200_painn_msg_bwd(const float* xh, const float* xh_bias, const float* mu,
                         const float* g_q, const float* g_mu,
                         float* g_xh, float* g_mu_in, float* egrad, void* stream);
 
+/* Test and benchmark entry points, not a supported API: they may change with the kernels they expose.
+ * Every instantiation of the two kernels above.  `w_stride` 3F: rows of W (and dW) of 3F;
+ * 6F: one [W | dW/dd] record per row (dW unused).  `rev` non-NULL: edge e reads row min(e, rev[e]), one row per
+ * undirected pair; NULL: row e.  `bf16` != 0: W, dW (and gW) hold bf16.  Backward with `gW` non-NULL (w_stride 3F
+ * only): also gW[e][3F] = seed_atom[j] * dE/dW of the opposite edge, for the filter's weight gradients. */
+int nb200_painn_msg_fwd_ex(const float* xh, const float* xh_bias, const float* q, const float* mu,
+                           const void* W, int32_t w_stride, const int32_t* rev, const float* geom,
+                           const int32_t* row_ptr, const int32_t* col, int32_t n_atoms, float* q_out,
+                           float* mu_out, int32_t bf16, void* stream);
+int nb200_painn_msg_bwd_ex(const float* xh, const float* xh_bias, const float* mu, const void* W,
+                           const void* dW, int32_t w_stride, const int32_t* rev, const float* geom,
+                           const int32_t* row_ptr, const int32_t* col, int32_t n_atoms, const float* g_q,
+                           const float* g_mu, float* g_xh, float* g_mu_in, float* egrad, void* gW,
+                           const float* seed_atom, int32_t bf16, void* stream);
+/* Gather-bandwidth probe (test and benchmark entry point): the per-edge L2 reads of the message kernels without
+ * their arithmetic.  bwd_pattern 0: A = xh [N,3F], B = mu [N,3F], first 3F of record row min(e, rev[e]);
+ * 1: A = g_q [N,F], B = g_mu [N,3F], whole 6F record.  out[N*32] receives sums that keep the loads alive. */
+int nb200_msg_gather_probe(const float* A, const float* B, const float* rec, int32_t rec_stride,
+                           const int32_t* rev, const int32_t* row_ptr, const int32_t* col, int32_t n_atoms,
+                           int32_t bwd_pattern, float* out, void* stream);
+
 /* Forces from accumulated edge gradients:  F_j = -sum_{e in row j} (G(e) - G(rev e)). */
 int nb200_edge_forces(const float* egrad, const float* geom, const int32_t* row_ptr,
                       const int32_t* rev, int32_t n_atoms, float* forces, void* stream);

@@ -79,6 +79,9 @@ SIGNATURES = {
     "nb200_painn_msg_fwd": (c_int32, [c_void_p] * 8 + [c_int32, c_void_p, c_void_p, c_void_p]),
     "nb200_painn_msg_bwd": (c_int32, [c_void_p] * 8 + [c_int32] + [c_void_p] * 6),
     "nb200_edge_forces": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
+    "nb200_painn_msg_fwd_ex": (c_int32, [c_void_p] * 5 + [c_int32] + [c_void_p] * 4 + [c_int32] + [c_void_p] * 2 + [c_int32, c_void_p]),
+    "nb200_painn_msg_bwd_ex": (c_int32, [c_void_p] * 5 + [c_int32] + [c_void_p] * 4 + [c_int32] + [c_void_p] * 7 + [c_int32, c_void_p]),
+    "nb200_msg_gather_probe": (c_int32, [c_void_p] * 3 + [c_int32] + [c_void_p] * 3 + [c_int32, c_int32, c_void_p, c_void_p]),
     "nb200_engine_create": (c_int32, [POINTER(c_void_p)]),
     "nb200_engine_destroy": (c_int32, [c_void_p]),
     "nb200_engine_set_timing": (c_int32, [c_void_p, c_int32]),
