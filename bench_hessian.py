@@ -1,11 +1,14 @@
-"""Throughput of exact Hessians (nb200_painn_hvp) on the config-2 batch: 256 synthetic conformations (synth.py), one JSON line.
+"""Throughput of exact Hessians (nb200_painn_hvp, nb200_schnet_hvp) on the config-2 batch: 256 synthetic conformations (synth.py), one JSON
+line.
 
-    python bench_hessian.py [--model painn|painn-oc] [--max-dir D] [--repeats R]
+    python bench_hessian.py [--model painn|painn-oc|schnet] [--max-dir D] [--repeats R]
 
 Reports Hessians / s and HVP directions / s for the whole batch (3 n_max shared directions, chunks of --max-dir), peak device memory, ms per
 direction split into the tangent forward and the backward (CUDA events around the engine's launch categories), and the same Hessians by
-batched central finite differences of nb200_painn_energy_forces (two force calls per direction, step 1e-3 A) with their deviation from the
-analytic ones.  Card name and power limit come from the same run.  Writes nothing into the tree.
+batched central finite differences of the inference engine (nb200_painn_energy_forces, nb200_schnet_energy_forces; two force calls per
+direction, step 1e-3 A) with their deviation from the analytic ones.  For SchNet the per-direction split is also given per launch category
+(marginal ms per direction of each, from the engine's CUDA-event timing of an n_dir call minus a one-direction call).  Card name and power
+limit come from the same run.  Writes nothing into the tree.
 """
 import argparse
 import ctypes
@@ -30,7 +33,7 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="painn", choices=["painn", "painn-oc"])
+    ap.add_argument("--model", default="painn", choices=["painn", "painn-oc", "schnet"])
     ap.add_argument("--max-dir", type=int, default=None)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--fd-step", type=float, default=1e-3)
@@ -48,7 +51,7 @@ def main():
     z = torch.from_numpy(b["z"]).to(dev)
     pos = torch.from_numpy(b["pos"]).to(dev)
     bt = torch.from_numpy(b["batch"]).to(dev)
-    if args.model == "painn":
+    if args.model in ("painn", "schnet"):
         batch = {"_atomic_numbers": z.long(), "_positions": pos, "_idx_m": bt, "_n_atoms": torch.bincount(bt)}
     else:
         class D:
@@ -90,13 +93,25 @@ def main():
     t1 = float(np.median([timed(v[:1]) for _ in range(args.repeats)]))
     tn = float(np.median([timed(v) for _ in range(args.repeats)]))
     per_dir = (tn - t1) / (n_dir - 1)
-    lib.nb200_engine_set_timing(eng._h, 1)
-    eng.run_hvp(zi, posf, mol_ptr, n_mol, v, with_forces=False)
-    ms = (ctypes.c_float * 16)()
-    cnt = (ctypes.c_int32 * 16)()
-    lib.nb200_engine_read_timings(eng._h, ms, cnt, 16)
-    lib.nb200_engine_set_timing(eng._h, 0)
+    def categories(vv):
+        lib.nb200_engine_set_timing(eng._h, 1)
+        eng.run_hvp(zi, posf, mol_ptr, n_mol, vv, with_forces=False)
+        ms = (ctypes.c_float * 16)()
+        cnt = (ctypes.c_int32 * 16)()
+        lib.nb200_engine_read_timings(eng._h, ms, cnt, 16)
+        lib.nb200_engine_set_timing(eng._h, 0)
+        return list(ms)
+
+    ms = categories(v)
     tan_fwd = ms[5] / n_dir  # ms
+    split = None
+    if args.model == "schnet":
+        ms1 = categories(v[:1])
+        names = ("graph", "filter", "embed", "gemm", "node", "msg_fwd", "msg_bwd", "readout", "edge_grad_and_assembly")
+        split = {k: (ms[i] - ms1[i]) / (n_dir - 1) for i, k in enumerate(names)}
+        edges = eng.last_edges
+        tan_fwd = split["msg_fwd"]  # the once-per-call primal message kernels cancel in the difference
+        eng.run(zi, posf, mol_ptr, n_mol, True)  # sizes the inference engine's edge capacity for the finite-difference launches
 
     # finite differences: two batched force calls per shared direction
     h = args.fd_step
@@ -115,8 +130,8 @@ def main():
     dev_rel = max(float((a - b).abs().max() / a.abs().max()) for a, b in zip(hs, fd))
 
     name, limit = card()
-    print(json.dumps({
-        "metric": "painn_hessians", "model": args.model, "batch": n_mol, "atoms": N, "n_max": n_max, "directions": n_dir,
+    rec = {
+        "metric": "schnet_hessians" if args.model == "schnet" else "painn_hessians", "model": args.model, "batch": n_mol, "atoms": N, "n_max": n_max, "directions": n_dir,
         "hessians_per_s": n_mol / t_an, "directions_per_s": n_dir / t_an, "ms_per_batch": 1e3 * t_an, "ms_per_direction": 1e3 * t_an / n_dir,
         "ms_once_per_call": 1e3 * (t1 - per_dir), "ms_per_direction_marginal": 1e3 * per_dir,
         "ms_per_direction_tangent_forward": tan_fwd, "ms_per_direction_backward": 1e3 * per_dir - tan_fwd,
@@ -124,7 +139,11 @@ def main():
         "fd_ms_per_batch": 1e3 * t_fd, "fd_hessians_per_s": n_mol / t_fd, "fd_step_A": h, "fd_max_rel_dev": dev_rel,
         "analytic_speedup_vs_fd": t_fd / t_an, "max_asymmetry": hs.max_asymmetry,
         "card": name, "power_limit": limit,
-    }))
+    }
+    if split is not None:
+        rec["ms_per_direction_by_category"] = split
+        rec["edges"] = edges
+    print(json.dumps(rec))
 
 
 if __name__ == "__main__":

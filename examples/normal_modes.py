@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Relax a batch of fixture molecules with the batched L-BFGS, then check each relaxed conformer with its exact normal modes: the lowest
 non-rigid wavenumbers and the count of imaginary modes (what `PYGAseInterface.compute_normal_modes` does with ASE Vibrations, one
-molecule at a time)."""
+molecule at a time).  --model picks the spk representation: PaiNN or SchNet."""
 import argparse
 import os
 import sys
@@ -22,13 +22,15 @@ from nabladft_b200.optimization import ASEBatchwiseLBFGS, SimpleAtoms, SpkBatchw
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--mols", type=int, nargs="+", default=[0, 3, 26, 99])
-    ap.add_argument("--weights", help="state dict of the spk PaiNN model (default: the seeded test weights)")
+    ap.add_argument("--model", default="painn", choices=["painn", "schnet"])
+    ap.add_argument("--weights", help="state dict of the spk model (default: the seeded test weights)")
     ap.add_argument("--fmax", type=float, default=1e-4)
     ap.add_argument("--steps", type=int, default=1000)
     a = ap.parse_args()
+    rep = spk.PaiNN if a.model == "painn" else spk.SchNet
     model = spk.NeuralNetworkPotential(
-        representation=spk.PaiNN(n_atom_basis=128, n_interactions=3, radial_basis=spk.GaussianRBF(n_rbf=100, cutoff=5.0),
-                                 cutoff_fn=spk.CosineCutoff(cutoff=5.0)),
+        representation=rep(n_atom_basis=128, n_interactions=3, radial_basis=spk.GaussianRBF(n_rbf=100, cutoff=5.0),
+                           cutoff_fn=spk.CosineCutoff(cutoff=5.0)),
         input_modules=[spk.PairwiseDistances()], output_modules=[spk.Atomwise(n_in=128, output_key="energy"), spk.Forces()])
     if a.weights:
         model.load_state_dict(torch.load(a.weights, map_location="cpu"), strict=True)

@@ -310,6 +310,16 @@ int nb200_schnet_energy_grads(nb200_engine* eng, const nb200_schnet_weights* w, 
                               int32_t n_mol, int32_t n_atoms, const int32_t* row_ptr, int64_t n_edges, void* workspace,
                               int64_t workspace_bytes, const float* energy_seed, const float* force_seed,
                               const nb200_schnet_weights* grads, float* energy, void* stream);
+/* Hessian-vector products of the SchNet energy (csrc/schnet_hvp.inc, DESIGN.md 3.13.1): for each of n_dir position-space directions v[d]
+ * ([N,3], Angstrom)  hv[d] = H v[d] = -(dF/dR) v[d] in Ha/A, exact (forward-over-reverse, no finite step), fp32 arithmetic and storage.  The
+ * primal forward, the filter's radial derivatives and the reverse sweep run once per call, the directions one after another, so the workspace
+ * does not depend on n_dir.  energy[B] follows w->energy_shift_per_atom; forces[N,3] (NULL => not written) are those of the same pass.
+ * row_ptr / n_edges come from nb200_schnet_train_count.  No atomics: bitwise repeatable, independent of how directions are chunked.
+ * NB200_EINVAL (nothing launched) for a null required pointer, n_dir < 1, a short workspace or an invalid configuration. */
+int64_t nb200_schnet_hvp_workspace_bytes(const nb200_schnet_weights* w, int32_t n_mol, int32_t n_atoms, int64_t n_edges);
+int nb200_schnet_hvp(nb200_engine* eng, const nb200_schnet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
+                     int32_t n_mol, int32_t n_atoms, const int32_t* row_ptr, int64_t n_edges, void* workspace, int64_t workspace_bytes,
+                     int32_t n_dir, const float* v, float* energy, float* forces, float* hv, void* stream);
 
 /* ----------------------------------------------------------------------------------------
  * QHNet (config/model/qhnet.yaml; nablaDFT/qhnet/qhnet.py + layers.py over e3nn 0.5.1) operators.

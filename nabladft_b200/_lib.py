@@ -156,6 +156,9 @@ SIGNATURES = {
     "nb200_schnet_train_workspace_bytes": (c_int64, [POINTER(SchnetWeights), c_int32, c_int32, c_int64, c_int32]),
     "nb200_schnet_energy_grads": (c_int32, [c_void_p, POINTER(SchnetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_void_p,
                                             c_int64, c_void_p, c_void_p, POINTER(SchnetWeights), c_void_p, c_void_p]),
+    "nb200_schnet_hvp_workspace_bytes": (c_int64, [POINTER(SchnetWeights), c_int32, c_int32, c_int64]),
+    "nb200_schnet_hvp": (c_int32, [c_void_p, POINTER(SchnetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_void_p,
+                                   c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_gemnet_oc_train_workspace_bytes": (c_int64, [POINTER(GemNetOCWeights), c_int32, c_int32, POINTER(c_int64)]),
     "nb200_gemnet_oc_energy_forces_grads": (c_int32, [c_void_p, POINTER(GemNetOCWeights), c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
                                                       c_void_p, c_int64, POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

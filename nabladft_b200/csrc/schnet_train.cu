@@ -576,3 +576,5 @@ extern "C" int nb200_schnet_energy_grads(nb200_engine* eng, const nb200_schnet_w
     }
     return pfor(eng, s, CAT_EMBED, (int64_t)w->n_elem * F, SEmbGradK{z, w->z_offset, w->n_elem, wk.gxd, n_atoms, (float*)g->emb, A});
 }
+
+#include "schnet_hvp.inc"

@@ -4,7 +4,7 @@ Owns: the C engine object, the device workspace, the canonical weight export.
 The model classes (`painn_oc.PaiNN`, `spk.NeuralNetworkPotential`) only describe how their
 reference-named parameters map onto the canonical layout.
 """
-from ctypes import byref, c_void_p
+from ctypes import byref, c_int64, c_void_p
 from typing import Dict, Optional, Tuple
 
 import torch
@@ -23,10 +23,11 @@ _KINDS = {
 class PainnEngine:
     """One engine per (module, device). Not thread-safe; one CUDA stream per call."""
 
-    def __init__(self, kind: str = "painn"):
+    def __init__(self, kind: str = "painn", lib=None):
+        """`lib`: a bound library exporting the C ABI (default: libnabla_b200.so)."""
         self.kind = kind
         self._wtype, self._ws_fn, self._run_fn, self._wkeys = _KINDS[kind]
-        self.lib = _lib.load()
+        self.lib = _lib.load() if lib is None else lib
         h = c_void_p()
         check(self.lib.nb200_engine_create(byref(h)), "nb200_engine_create")
         self._h = h
@@ -253,23 +254,33 @@ class PainnEngine:
         return grads
 
     # ------------------------------------------------------------------ Hessian-vector products
+    # device check and stream of the calls below: tests/test_schnet_hvp_emu.py runs the same host code on CPU tensors against the emulation build
+    def _on_device(self, t: torch.Tensor) -> bool:
+        return t.is_cuda
+
+    def _stream(self):
+        return current_stream()
+
     def run_hvp(self, z, pos, mol_ptr, n_mol, v, with_forces: bool = True):
-        """Exact Hessian-vector products of the energy (`nb200_painn_hvp`): v [n_dir, n_atoms, 3] (or [n_atoms, 3]) fp32 CUDA, in Angstrom.
-        Returns (energy [B], forces [N, 3] or None, hv [n_dir, N, 3] = H v in Ha/A).  Synchronous like `run`: checks the device status and
-        regrows the edge capacity once."""
-        if self.kind != "painn":
-            raise NotImplementedError("Hessian-vector products are built for the PaiNN engine only")
+        """Exact Hessian-vector products of the energy (`nb200_painn_hvp`, `nb200_schnet_hvp`): v [n_dir, n_atoms, 3] (or [n_atoms, 3]) fp32
+        CUDA, in Angstrom.  Returns (energy [B], forces [N, 3] or None, hv [n_dir, N, 3] = H v in Ha/A).  Synchronous like `run`: the PaiNN
+        engine checks the device status and regrows the edge capacity once; the SchNet engine counts the edges first (one host sync)."""
+        if self.kind not in ("painn", "schnet"):
+            raise NotImplementedError(f"Hessian-vector products are not built for the {self.kind} engine")
         if self._weights is None:
             raise NablaB200Error("set_weights() first")
         n_atoms, dev = z.shape[0], z.device
-        if not (z.is_cuda and z.dtype == torch.int32 and pos.dtype == torch.float32 and mol_ptr.dtype == torch.int32):
+        if not (self._on_device(z) and z.dtype == torch.int32 and pos.dtype == torch.float32 and mol_ptr.dtype == torch.int32):
             raise NablaB200Error("run_hvp(): need CUDA int32 z / mol_ptr and fp32 pos")
         if v.dim() == 2:
             v = v.unsqueeze(0)
-        if not (v.is_cuda and v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n_atoms, 3) and v.shape[0] >= 1):
+        if not (self._on_device(v) and v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n_atoms, 3)
+                and v.shape[0] >= 1):
             raise NablaB200Error("run_hvp(): v must be a contiguous fp32 CUDA tensor [n_dir, n_atoms, 3] with n_dir >= 1")
         n_dir = v.shape[0]
         self._kept_token = 0  # this call overwrites the workspace a kept training forward lives in
+        if self.kind == "schnet":
+            return self._run_schnet_hvp(z, pos, mol_ptr, n_mol, v, with_forces)
         for _ in range(2):
             e_cap = max(self.e_cap, n_atoms * self.edges_per_atom_guess)
             self.e_cap = e_cap
@@ -294,6 +305,29 @@ class PainnEngine:
             self.raise_on_status(st)
             return energy, forces, hv
         raise NablaB200Error("edge capacity regrow failed")
+
+    def _run_schnet_hvp(self, z, pos, mol_ptr, n_mol, v, with_forces):
+        """`nb200_schnet_train_count` (exact edge count, one host sync), then `nb200_schnet_hvp` on the engine's weights."""
+        lib, n_atoms, dev, n_dir = self.lib, z.shape[0], z.device, v.shape[0]
+        s = self._stream()
+        row_ptr = torch.empty(n_atoms + 1, dtype=torch.int32, device=dev)
+        scratch = torch.empty(2 * n_atoms, dtype=torch.int32, device=dev)
+        n_edges = c_int64(0)
+        check(lib.nb200_schnet_train_count(byref(self._weights), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, ptr(row_ptr), ptr(scratch), byref(n_edges), s),
+              "nb200_schnet_train_count")
+        need = lib.nb200_schnet_hvp_workspace_bytes(byref(self._weights), n_mol, n_atoms, n_edges.value)
+        if need < 0:
+            check(int(need), "nb200_schnet_hvp_workspace_bytes")
+        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
+            self._ws = None
+            self._ws = torch.empty(int(need * 1.05) + 256, dtype=torch.uint8, device=dev)
+        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+        forces = torch.empty(n_atoms, 3, dtype=torch.float32, device=dev) if with_forces else None
+        hv = torch.empty(n_dir, n_atoms, 3, dtype=torch.float32, device=dev)
+        check(lib.nb200_schnet_hvp(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, ptr(row_ptr), n_edges.value,
+                                   ptr(self._ws), self._ws.numel(), n_dir, ptr(v), ptr(energy), ptr(forces), ptr(hv), s), "nb200_schnet_hvp")
+        self.last_edges = int(n_edges.value)
+        return energy, forces, hv
 
     # ------------------------------------------------------------------ asynchronous inference (the reference-facing forward())
     _MAX_PENDING = 8

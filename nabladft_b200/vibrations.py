@@ -1,16 +1,16 @@
-"""Analytic Hessians and normal modes of the PaiNN models on the GPU.
+"""Analytic Hessians and normal modes of the PaiNN and SchNet models on the GPU.
 
 The reference's `PYGAseInterface.compute_normal_modes` (nablaDFT/optimization/pyg_ase_interface.py) runs ASE `Vibrations`: central finite
 differences of the forces, one molecule at a time, 6N + 1 force calls per molecule with a 0.01 A step.  Here the engine computes exact
-Hessian-vector products H v = -(dF/dR) v (`PainnEngine.run_hvp`, DESIGN.md section 3.13), and since molecules do not interact, ONE direction
-displaces atom k of every molecule of the batch at once: the Hessians of a whole batch take 3 * n_max directions, n_max = the atom count
-of the largest molecule.
+Hessian-vector products H v = -(dF/dR) v (`PainnEngine.run_hvp`; DESIGN.md section 3.13 for PaiNN, 3.13.1 for SchNet), and since
+molecules do not interact, ONE direction displaces atom k of every molecule of the batch at once: the Hessians of a whole batch take
+3 * n_max directions, n_max = the atom count of the largest molecule.
 
     hessian_vector_product(model, batch, v) -> (energy, forces, hv)
     hessians(model, batch, max_dir=None)    -> per-molecule [3n, 3n] Hessians, Ha/A^2
     normal_modes(model, batch, masses=None) -> per-molecule eigenvalues, modes, wavenumbers (cm^-1) and ASE-style energies (meV)
 
-`model` is either mirror: `spk.NeuralNetworkPotential` (PaiNN representation; `batch` = its inputs dict) or `painn_oc.PaiNN` (`batch` has
+`model` is `spk.NeuralNetworkPotential` (PaiNN or SchNet representation; `batch` = its inputs dict) or `painn_oc.PaiNN` (`batch` has
 .z, .pos, .batch and optionally .ptr).  Everything runs in fp32 on the device except the diagonalisation (float64, `torch.linalg.eigh`).
 """
 import math
@@ -45,8 +45,6 @@ def _engine_inputs(model, batch):
     from . import painn_oc, spk
 
     if isinstance(model, spk.NeuralNetworkPotential):
-        if model._kind != "painn":
-            raise NotImplementedError("Hessians are built for the PaiNN engine only (this model has a SchNet representation)")
         eng, z, pos, mol_ptr, n_mol = model._prepare(batch)  # raises on CPU inputs and periodic systems
         if model._training_mode():
             raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
