@@ -1,8 +1,5 @@
 """N>1 path on CPU: world_size-2 gloo processes run the sharding / gathering host logic around
 a stand-in evaluator (the oracle) and must reproduce the unsharded result exactly."""
-import os
-import socket
-
 import pytest
 import torch
 import torch.distributed as dist
@@ -11,18 +8,14 @@ import torch.multiprocessing as mp
 from helpers import load_fixture, load_golden_weights
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+def _init(rank, world, init_file):
+    # rendezvous through a file store in the test's temporary directory: unlike a free port picked in advance, no other process can take it
     torch.set_num_threads(2)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+    dist.init_process_group("gloo", init_method=f"file://{init_file}", rank=rank, world_size=world)
+
+
+def _worker(rank, world, init_file, q):
+    _init(rank, world, init_file)
     try:
         from nabladft_b200.parallel import energy_forces_sharded, max_over_ranks
         from oracle.painn_oc import PaiNNOC
@@ -34,9 +27,14 @@ def _worker(rank, world, port, q):
         mol_ptr[1:] = torch.cumsum(counts, 0)
 
         def fn(z_r, pos_r, ptr_r):
-            b = torch.repeat_interleave(torch.arange(ptr_r.numel() - 1), ptr_r[1:] - ptr_r[:-1])
-            e, f = net(z_r, pos_r.clone(), b)
-            return e.detach(), f.detach()
+            # one molecule per oracle call: the float64 GEMMs then have the same shapes whichever shard holds the molecule (BLAS may
+            # round a row differently when the row count changes), so the results below are comparable bit for bit
+            es, fs = [], []
+            for a, b in zip(ptr_r[:-1].tolist(), ptr_r[1:].tolist()):
+                e, f = net(z_r[a:b], pos_r[a:b].clone(), torch.zeros(b - a, dtype=torch.long))
+                es.append(e.detach())
+                fs.append(f.detach())
+            return torch.cat(es), torch.cat(fs)
 
         e, f = energy_forces_sharded(fn, z, pos, mol_ptr)
         t = max_over_ranks(10.0 + rank, torch.device("cpu"))
@@ -61,11 +59,11 @@ def test_balanced_ranges_cover_everything_once():
 
 
 @pytest.mark.timeout(300)
-def test_sharded_energy_forces_world2_gloo():
+def test_sharded_energy_forces_world2_gloo(tmp_path):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
+    init_file = str(tmp_path / "store")
+    procs = [ctx.Process(target=_worker, args=(r, 2, init_file, q)) for r in range(2)]
     for p in procs:
         p.start()
     same_e, df, t = q.get(timeout=240)
@@ -76,10 +74,8 @@ def test_sharded_energy_forces_world2_gloo():
     assert t == 11.0  # MAX over ranks
 
 
-def _grad_worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    torch.set_num_threads(2)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _grad_worker(rank, world, init_file, q):
+    _init(rank, world, init_file)
     try:
         from nabladft_b200.parallel import GradBucket, allreduce_gradients, shard_batch
         from oracle.painn_oc import PaiNNOC
@@ -121,11 +117,11 @@ def _grad_worker(rank, world, port, q):
 
 
 @pytest.mark.timeout(300)
-def test_gradient_allreduce_world2_gloo_equals_full_batch_gradient():
+def test_gradient_allreduce_world2_gloo_equals_full_batch_gradient(tmp_path):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_grad_worker, args=(r, 2, port, q)) for r in range(2)]
+    init_file = str(tmp_path / "store")
+    procs = [ctx.Process(target=_grad_worker, args=(r, 2, init_file, q)) for r in range(2)]
     for p in procs:
         p.start()
     n, err = q.get(timeout=240)
