@@ -3,7 +3,12 @@
 batch of synthetic molecules with PaiNN (config/model/painn.yaml) for a fixed number of L-BFGS steps through the public API
 (`nabladft_b200.optimization.ASEBatchwiseLBFGS.run`), host Atoms in -> host Atoms out.  Reports optimiser steps/s for the whole
 batch and molecule-steps/s; `--cpu` times the oracle loop (oracle L-BFGS + oracle PaiNN) on a few molecules for comparison.
-Secondary benchmark (the driver's headline is bench.py); prints one JSON line."""
+Secondary benchmark (the driver's headline is bench.py); prints one JSON line.
+
+`--model gemnet-oc` relaxes with GemNet-OC (reference job config/gemnet-oc_optim.yaml) at batch 32 and 256 and alternates two arms in one
+process: the device loop (asynchronous forward sized by per-batch upper bounds, one host look per `check_every` steps) and the same loop with
+the synchronous two-phase forward (`GemNetOCRunner.run`, which waits for the edge counts) at every step.  It also reports the host
+synchronisations of a run, real count / bound of the five edge counts, the workspace size, and the card's name and power limit."""
 import argparse
 import json
 import os
@@ -16,8 +21,96 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
 
+def gemnet_main(args):
+    import subprocess
+
+    import numpy as np
+    import torch
+    import yaml
+    from weights import golden_state_dict
+
+    from nabladft_b200.gemnet_oc import C_NAMES, GemNetOC, GemNetOCEngine
+    from nabladft_b200.optimization import ASEBatchwiseLBFGS, PyGBatchwiseCalculator, SimpleAtoms
+    from nabladft_b200.synth import synth_batch
+
+    dev = torch.device("cuda:0")
+    cfg = yaml.safe_load(open(os.path.join(ROOT, "config", "model", "gemnet-oc-b200.yaml")))["net"]
+    cfg.pop("_target_")
+    net = GemNetOC(**cfg).eval()
+    sd = net.state_dict()
+    new = golden_state_dict(sd, bias_std=0.02, weight_scale=0.5)
+    for k in sd:
+        if k.endswith("scale_factor"):
+            sd[k] = torch.ones_like(sd[k])
+        elif k in new:
+            sd[k] = torch.as_tensor(np.asarray(new[k])).float().reshape(sd[k].shape)
+    net.load_state_dict(sd, strict=True)
+
+    class SyncEngine(GemNetOCEngine):
+        """Comparison arm: the two-phase forward, which copies the edge counts to the host, at every step."""
+
+        def launch(self, z, pos, mol_ptr, n_mol, e_cap=None):
+            energy, forces = self.runner.run(z, pos, mol_ptr, n_mol, self._batch[1])
+            return energy, forces, torch.zeros(8, dtype=torch.int32, device=pos.device)
+
+    class SyncCalculator(PyGBatchwiseCalculator):
+        def engine(self):
+            if getattr(self, "_sync_engine", None) is None:
+                self._sync_engine = SyncEngine(self.model, self.model._get_runner())
+            return self._sync_engine
+
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30)
+        card, power = (v.strip() for v in q.stdout.strip().split(","))
+    except Exception as exc:  # noqa: BLE001
+        card, power = torch.cuda.get_device_name(0), f"unavailable ({exc})"
+    out = {"metric": "L-BFGS steps/sec (GemNet-OC E+F + batched L-BFGS, B molecules per step)", "card": card, "power_limit": power, "steps": args.steps,
+           "check_every": args.check_every, "memory": args.memory, "dtype": "f32 model / f64 positions", "data": "synthetic",
+           "timing": "host wall clock around ASEBatchwiseLBFGS.run ending in a device synchronise; arms alternated, best of the repeats", "batches": []}
+    for batch in args.batches:
+        b = synth_batch(1, batch)
+        ptr = b["mol_ptr"]
+        atoms = [SimpleAtoms(b["pos"][ptr[m]:ptr[m + 1]], b["z"][ptr[m]:ptr[m + 1]]) for m in range(batch)]
+        arms = {"device_loop": PyGBatchwiseCalculator(net, device=dev, energy_unit="Hartree", position_unit="Ang"),
+                "sync_forward_per_step": SyncCalculator(net, device=dev, energy_unit="Hartree", position_unit="Ang")}
+        opts = {k: ASEBatchwiseLBFGS(c, logfile=None, memory=args.memory, check_every=args.check_every) for k, c in arms.items()}
+        times = {k: [] for k in arms}
+        for k, o in opts.items():
+            o.run(atoms, fmax=1e-9, steps=3)  # warm-up: allocations, module loads
+        torch.cuda.synchronize()
+        for _ in range(args.repeats):
+            for k, o in opts.items():
+                o.initialize()
+                t0 = time.perf_counter()
+                o.run(atoms, fmax=1e-9, steps=args.steps)
+                torch.cuda.synchronize()
+                times[k].append(time.perf_counter() - t0)
+                if k == "device_loop":
+                    last = arms[k].engine().runner._status.cpu().tolist()  # status words of the last launch: the counts at the final geometry
+        eng = arms["device_loop"].engine()
+        z, pos, mol_ptr, _ = arms["device_loop"].pack(atoms)
+        _, _, st = eng.run(z, pos.float().contiguous(), mol_ptr, batch)  # start geometry: real counts against the bounds
+        real = dict(zip(C_NAMES, [int(st[4]), int(st[0]), int(st[5]), int(st[6]), int(st[7])]))
+        same = all(np.array_equal(arms["device_loop"].results[k], arms["sync_forward_per_step"].results[k]) for k in ("energy", "forces"))
+        row = {"batch": batch, "atoms": int(ptr[-1]), "workspace_bytes": eng.runner.last_workspace_bytes,
+               "count_over_bound": {k: round(real[k] / max(1, eng.bounds[k]), 4) for k in C_NAMES}, "bounds": eng.bounds,
+               "count_over_bound_at_the_final_geometry": {k: round(v / max(1, eng.bounds[k]), 4) for k, v in
+                                                          zip(C_NAMES, [last[4], last[0], last[5], last[6], last[7]])},
+               "final_results_bitwise_equal_between_arms": bool(same)}
+        for k, o in opts.items():
+            dt = min(times[k])
+            row[k] = {"steps_per_s": o.nsteps / dt, "molecule_steps_per_s": o.nsteps * batch / dt, "ms_per_step": dt / o.nsteps * 1e3,
+                      "all_runs_s": [round(t, 4) for t in times[k]], "host_syncs_of_the_loop": o.host_syncs,
+                      "host_syncs_inside_each_forward": 0 if k == "device_loop" else 5}
+        out["batches"].append(row)
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", choices=["painn", "gemnet-oc"], default="painn")
+    ap.add_argument("--batches", type=int, nargs="+", default=[32, 256], help="gemnet-oc: batch sizes to run")
+    ap.add_argument("--repeats", type=int, default=2, help="gemnet-oc: timed runs of each arm (alternated)")
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--memory", type=int, default=100)
@@ -26,6 +119,8 @@ def main():
     ap.add_argument("--cpu-mols", type=int, default=8)
     ap.add_argument("--cpu-steps", type=int, default=3)
     args = ap.parse_args()
+    if args.model == "gemnet-oc":
+        return gemnet_main(args)
     import numpy as np
     import torch
 

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Batched L-BFGS relaxation of every molecule of a packed dataset (reference: job_type optimize, config/schnet_optim.yaml)."""
+"""Batched L-BFGS relaxation of every molecule of a packed dataset (reference: job_type optimize, config/schnet_optim.yaml and
+config/gemnet-oc_optim.yaml): `--model painn` (default) or `--model gemnet-oc`."""
 import argparse
 import os
 import sys
@@ -9,7 +10,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from nabladft_b200.data import PackedEnergyDataset  # noqa: E402
-from nabladft_b200.optimization import ASEBatchwiseLBFGS, PackedOptimizeTask, SpkBatchwiseCalculator  # noqa: E402
+from nabladft_b200.optimization import ASEBatchwiseLBFGS, PackedOptimizeTask, PyGBatchwiseCalculator, SpkBatchwiseCalculator  # noqa: E402
 from train_painn import build_model  # noqa: E402
 
 
@@ -17,14 +18,25 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("cache")
     ap.add_argument("--weights")
+    ap.add_argument("--model", choices=["painn", "gemnet-oc"], default="painn")
     ap.add_argument("--batch", type=int, default=32)   # config/schnet_optim.yaml: batch_size 32, fmax 1e-5, steps 500
     ap.add_argument("--fmax", type=float, default=1e-5)
     ap.add_argument("--steps", type=int, default=500)
     a = ap.parse_args()
-    model = build_model()
+    if a.model == "gemnet-oc":
+        import yaml
+
+        from nabladft_b200.gemnet_oc import GemNetOC
+
+        cfg = yaml.safe_load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "config", "model", "gemnet-oc-b200.yaml")))["net"]
+        cfg.pop("_target_")
+        model = GemNetOC(**cfg)
+    else:
+        model = build_model()
     if a.weights:
         model.load_state_dict(torch.load(a.weights, map_location="cpu"), strict=True)
-    calc = SpkBatchwiseCalculator(model, device="cuda:0", energy_unit="Hartree", position_unit="Ang")
+    calculator = PyGBatchwiseCalculator if a.model == "gemnet-oc" else SpkBatchwiseCalculator
+    calc = calculator(model, device="cuda:0", energy_unit="Hartree", position_unit="Ang")
     opt = ASEBatchwiseLBFGS(calc, logfile="-", check_every=10)
     out = PackedOptimizeTask(PackedEnergyDataset.load(a.cache), opt, a.batch, a.fmax, a.steps).run()
     np.savez_compressed("relaxed.npz", **out)

@@ -509,6 +509,23 @@ int nb200_gemnet_oc_energy_forces(nb200_engine* eng, const nb200_gemnet_oc_weigh
                                   const int32_t* mol_ptr, int32_t n_mol, int32_t n_atoms, int32_t max_atoms_per_mol,
                                   void* graph_buf, int64_t graph_bytes, const int64_t* counts_host, void* workspace,
                                   int64_t workspace_bytes, float* energy, float* forces, void* stream);
+/* Asynchronous form for loops that must not wait for the host (geometry optimisation): graph phase and model phase in ONE enqueue, no
+ * stream synchronisation, no device-to-host copy.  Arrays, grids and GEMMs are sized by UPPER BOUNDS of the five counts that follow from
+ * the molecule sizes alone, so they hold for every geometry of the batch (DESIGN.md 3.9):
+ *   nb200_gemnet_oc_count_bounds: pure host function; mol_ptr_host[n_mol + 1] -> counts_bound_host[NB200_GOC_C_COUNT].  NB200_EINVAL for an empty
+ *   molecule, a mol_ptr that does not start at 0, or a bound beyond int32.
+ *   nb200_gemnet_oc_energy_forces_async: workspace_bytes >= nb200_gemnet_oc_workspace_bytes(.., counts_bound_host).  The real counts stay on the
+ *   device; `status` is a device int32[8] rewritten by every call:
+ *     {main-graph edges, error code, max main-graph degree, atoms without a main-graph neighbour,   (words 0-3 as nb200_painn_energy_forces)
+ *      a2a edges, a2ee2a edges, qint edges, input-triplet slots}.
+ *   Error codes in status[1]: NB200_ECAPACITY a count exceeds its bound (nothing is written past a bound), NB200_ENOEDGES no main-graph edge,
+ *   NB200_EINVAL a non-finite coordinate.  With an error every energy and force of the call is NaN.  Same energies and forces as the two-phase
+ *   form. */
+int nb200_gemnet_oc_count_bounds(const nb200_gemnet_oc_weights* w, const int32_t* mol_ptr_host, int32_t n_mol, int64_t* counts_bound_host);
+int nb200_gemnet_oc_energy_forces_async(nb200_engine* eng, const nb200_gemnet_oc_weights* w, const int32_t* z, const float* pos,
+                                        const int32_t* mol_ptr, int32_t n_mol, int32_t n_atoms, int32_t max_atoms_per_mol,
+                                        void* graph_buf, int64_t graph_bytes, const int64_t* counts_bound_host, void* workspace,
+                                        int64_t workspace_bytes, float* energy, float* forces, int32_t* status, void* stream);
 /* Training (config/model/gemnet-oc.yaml trains with DIRECT forces: first-order back-propagation from dLoss/dE and dLoss/dF, the reference's
  * `loss.backward()` through GemNetOC.forward, gemnet_oc.py:1121-1251 + GemNetOCLightning.step 1361-1371).  Same two-phase protocol:
  * nb200_gemnet_oc_graph_count, then nb200_gemnet_oc_train_workspace_bytes (every activation is kept, mirrored by a gradient arena), then

@@ -151,6 +151,9 @@ SIGNATURES = {
     "nb200_gemnet_oc_workspace_bytes": (c_int64, [POINTER(GemNetOCWeights), c_int32, c_int32, POINTER(c_int64)]),
     "nb200_gemnet_oc_energy_forces": (c_int32, [c_void_p, POINTER(GemNetOCWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
                                                 c_void_p, c_int64, POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "nb200_gemnet_oc_count_bounds": (c_int32, [POINTER(GemNetOCWeights), POINTER(c_int32), c_int32, POINTER(c_int64)]),
+    "nb200_gemnet_oc_energy_forces_async": (c_int32, [c_void_p, POINTER(GemNetOCWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
+                                                      c_void_p, c_int64, POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_gemnet_oc_debug_h": (c_int32, [c_void_p, POINTER(GemNetOCWeights), c_int32, c_int32, POINTER(c_int64), c_void_p, c_void_p]),
     "nb200_schnet_train_count": (c_int32, [POINTER(SchnetWeights), c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "nb200_schnet_train_workspace_bytes": (c_int64, [POINTER(SchnetWeights), c_int32, c_int32, c_int64, c_int32]),

@@ -120,6 +120,7 @@ struct Graph {  // CSR by target, sources ascending; V = unit vector source -> t
 struct FillK {
     PairSel sel; const float* pos; const int32_t* mol_ptr; const int32_t* mol_id; const int32_t* deg_main; const int32_t* tbase;
     int32_t n; Graph a2a, mn, ae, q; int32_t* q_tin;
+    const int32_t* err;  // asynchronous forward: status word 1; non-zero (a count above its bound, ...) = write nothing.  nullptr otherwise
     GD void put(const Graph& g, int32_t e, int32_t a, int32_t j, float d, const float* v) const {
         g.src[e] = j;
         if (g.tgt) g.tgt[e] = a;
@@ -127,6 +128,7 @@ struct FillK {
         if (g.V) { g.V[3 * (int64_t)e] = v[0]; g.V[3 * (int64_t)e + 1] = v[1]; g.V[3 * (int64_t)e + 2] = v[2]; }
     }
     GD void operator()(int64_t ai) const {
+        if (err && *err) return;
         const int32_t a = (int32_t)ai, m0 = mol_ptr[mol_id[a]], m1 = mol_ptr[mol_id[a] + 1];
         int32_t e0 = a2a.ptr[a], e1 = mn.ptr[a], e2 = ae.ptr[a], e3 = q.ptr[a], tt = tbase[a];
         for (int32_t j = m0; j < m1; j++) {
@@ -143,6 +145,56 @@ struct FillK {
             if (x3) { q_tin[e3] = tt; tt += deg_main[j]; put(q, e3++, a, j, d, v); }
         }
         if (a == n - 1) q_tin[q.ptr[n]] = tbase[n];
+    }
+};
+// ------------------------------------------------------------------ status of the asynchronous forward (nb200_gemnet_oc_energy_forces_async)
+// status[8] (zeroed before): {main-graph edges, error code, max main-graph degree, atoms without a main-graph neighbour, a2a edges, a2ee2a
+// edges, qint edges, input-triplet slots}.  Words 0-3 read like the PaiNN engine's status.
+GD bool finite_f(float x) {
+    uint32_t u;
+    memcpy(&u, &x, 4);
+    return (u & 0x7f800000u) != 0x7f800000u;
+}
+GD float quiet_nan() {
+    const uint32_t u = 0x7fc00000u;
+    float x;
+    memcpy(&x, &u, 4);
+    return x;
+}
+struct StatusAtomK {
+    const float* pos; const int32_t* deg_main; int32_t* status;
+    GD void operator()(int64_t a) const {
+        // a non-finite coordinate fails every `d2 < cutoff^2` test of RankK, so the atom silently loses all its edges: report it instead
+        if (!(finite_f(pos[3 * a]) && finite_f(pos[3 * a + 1]) && finite_f(pos[3 * a + 2]))) atomicMin(status + 1, (int32_t)NB200_EINVAL);
+        const int32_t d = deg_main[a];
+        atomicMax(status + 2, d);
+        if (d == 0) atomicAdd(status + 3, 1);
+    }
+};
+struct StatusCountsK {  // one thread, after StatusAtomK: the five counts against their bounds
+    const int32_t* ptr; const int32_t* tbase; int32_t n; int32_t bound[5]; int32_t* status;
+    GD void operator()(int64_t) const {
+        const int32_t c[5] = {ptr[n], ptr[(int64_t)(n + 1) + n], ptr[2 * (int64_t)(n + 1) + n], ptr[3 * (int64_t)(n + 1) + n], tbase[n]};
+        bool over = false;
+        for (int k = 0; k < 5; k++) over = over || c[k] < 0 || c[k] > bound[k];  // < 0: int32 overflow of the scan
+        status[0] = c[NB200_GOC_C_MAIN];
+        status[4] = c[NB200_GOC_C_A2A]; status[5] = c[NB200_GOC_C_AE]; status[6] = c[NB200_GOC_C_Q]; status[7] = c[NB200_GOC_C_TIN];
+        if (status[1] == 0) status[1] = over ? NB200_ECAPACITY : (c[NB200_GOC_C_MAIN] == 0 ? NB200_ENOEDGES : NB200_OK);
+    }
+};
+// after an error every CSR row and every count becomes empty: no later kernel indexes an edge array (FillK wrote none)
+struct ClearOnErrorK {
+    const int32_t* status; int32_t* ptr; int64_t n_ptr; int32_t* tbase;
+    GD void operator()(int64_t i) const {
+        if (status[1] == 0) return;
+        if (i < n_ptr) ptr[i] = 0; else tbase[i - n_ptr] = 0;
+    }
+};
+struct NanOnErrorK {
+    const int32_t* status; float* energy; int64_t n_mol; float* forces;
+    GD void operator()(int64_t i) const {
+        if (status[1] == 0) return;
+        if (i < n_mol) energy[i] = quiet_nan(); else forces[i - n_mol] = quiet_nan();
     }
 };
 struct RevK {  // id_swap: position of the edge (t -> s) for every edge (s -> t)
@@ -262,6 +314,7 @@ constexpr int MRB_ROWS = 16;
 struct MulRbfRowsK {
     const float* x; int32_t ldx; const int32_t* row_idx; const float* rbf; int32_t ldr; const float* W; float scale; float* out; int32_t ldo; int32_t C;
     int32_t act_in; int64_t M;
+    const int32_t* M_dev;  // row count on the device when M is an upper bound (Ext), else nullptr
     static int64_t count(int64_t M, int C) { return (M + MRB_ROWS - 1) / MRB_ROWS * C; }
     GD void operator()(int64_t i) const {
         const int64_t rb = i / C; const int c = (int)(i % C);
@@ -271,7 +324,7 @@ struct MulRbfRowsK {
         const float4* w4 = reinterpret_cast<const float4*>(W + (int64_t)c * RB);
 #pragma unroll
         for (int k = 0; k < RB / 4; k++) { const float4 t = w4[k]; w[4 * k] = t.x; w[4 * k + 1] = t.y; w[4 * k + 2] = t.z; w[4 * k + 3] = t.w; }
-        const int64_t r1 = (rb + 1) * MRB_ROWS < M ? (rb + 1) * MRB_ROWS : M;
+        const int64_t Mr = ext_rows(M, M_dev), r1 = (rb + 1) * MRB_ROWS < Mr ? (rb + 1) * MRB_ROWS : Mr;
         for (int64_t r = rb * MRB_ROWS; r < r1; r++) {
             const float4* b4 = reinterpret_cast<const float4*>(rbf + r * ldr);
             float b[RB];

@@ -13,9 +13,48 @@
 #include "common.cuh"
 #include "engine_common.cuh"
 #include <cstdlib>
+#include <cstring>
 #endif
 
 #define GD __device__ __forceinline__
+
+// Extent of a launch or of a GEMM in rows.  `dev` == nullptr: exactly `n` rows.  `dev` set: `n` is an upper bound the host knows (it sizes the
+// grid, the GEMM and the arrays) and the row count is read from device memory inside the kernel, so the host never waits for it.
+struct Ext {
+    int64_t n; const int32_t* dev;
+    Ext(int64_t n_, const int32_t* dev_ = nullptr) : n(n_), dev(dev_) {}
+};
+GD int64_t ext_rows(int64_t bound, const int32_t* dev) {
+    if (!dev) return bound;
+    const int64_t r = *dev;
+    return r < bound ? r : bound;  // a count above the bound is reported through the status words (StatusCountsK), never indexed
+}
+#ifdef NB_EMU
+// host emulation of what the engines use beyond the stand-ins of emu_shim.h: int32 atomics of the status kernels (StatusAtomK) ...
+inline int32_t atomicAdd(int32_t* p, int32_t v) {
+    int32_t old;
+#pragma omp atomic capture
+    { old = *p; *p += v; }
+    return old;
+}
+inline int32_t atomicMax(int32_t* p, int32_t v) {
+    int32_t old;
+#pragma omp critical(nb_emu_minmax)
+    { old = *p; if (v > old) *p = v; }
+    return old;
+}
+inline int32_t atomicMin(int32_t* p, int32_t v) {
+    int32_t old;
+#pragma omp critical(nb_emu_minmax)
+    { old = *p; if (v < old) *p = v; }
+    return old;
+}
+// ... and the launch over an extent whose row count lives on the "device"
+template <class F>
+inline int pfor(nb200_engine* e, cudaStream_t s, int category, Ext x, int64_t per_row, const F& f) {
+    return pfor(e, s, category, ext_rows(x.n, x.dev) * per_row, f);  // host emulation: the "device" count is readable here
+}
+#endif
 
 // Workspace carver shared by the functor engines: 256-byte aligned sub-buffers of ONE caller-owned allocation (base == nullptr: size query).
 // Under host emulation every sub-buffer is followed by a guard zone filled with a sentinel; tests call nb200_emu_check_guards() after a run
@@ -50,6 +89,24 @@ inline int pfor(nb200_engine* e, cudaStream_t s, int category, int64_t n, const 
     const int64_t want = (n + 255) / 256;
     const int blocks = (int)(want < nb_sm_count() * 8 ? want : nb_sm_count() * 8);
     k_pfor<F><<<blocks, 256, 0, s>>>(n, f);
+    return nb_check_launch();
+}
+
+// the same for an extent whose row count lives on the device: grid from the bound, loop limit read inside the kernel
+template <class F>
+__global__ void __launch_bounds__(256) k_pfor_rows(int64_t bound, const int32_t* rows, int64_t per_row, F f) {
+    const int64_t n = ext_rows(bound, rows) * per_row;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) f(i);
+}
+template <class F>
+inline int pfor(nb200_engine* e, cudaStream_t s, int category, Ext x, int64_t per_row, const F& f) {
+    if (!x.dev) return pfor(e, s, category, x.n * per_row, f);
+    if (x.n <= 0) return NB200_OK;
+    static_assert(sizeof(F) <= 4000, "functor must fit the kernel parameter space");
+    Scope sc(e, s, category, 1);
+    const int64_t want = (x.n * per_row + 255) / 256;
+    const int blocks = (int)(want < nb_sm_count() * 8 ? want : nb_sm_count() * 8);
+    k_pfor_rows<F><<<blocks, 256, 0, s>>>(x.n, x.dev, per_row, f);
     return nb_check_launch();
 }
 

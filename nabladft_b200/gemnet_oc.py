@@ -11,13 +11,16 @@ Supported: the shipped configuration (non-periodic, direct coupled forces, all f
 else raises at construction.  Training mode returns (energy, forces) on one autograd node (`GemNetOCFn`): the engine back-propagates dLoss/dE
 and dLoss/dF through every kernel (csrc/gemnet_oc_train.inc) and autograd un-folds the flat export.  No CPU fallback.
 
+Relaxation: `GemNetOC.engine()` hands `optimization.ASEBatchwiseLBFGS` a forward that never waits for the host
+(`nb200_gemnet_oc_energy_forces_async`, sized by per-batch upper bounds of the edge counts: DESIGN.md 3.9).
+
 STATUS (round 1): every kernel has been checked against the oracle through the host-emulation build of the same source
 (tests/emu, tests/test_gemnet_emu.py); the GPU run of `tests/test_zz_gpu_first_runs.py` is the first execution on a device.
 """
 import ctypes
 import math
 import re
-from ctypes import POINTER, byref, c_float, c_int64, c_void_p
+from ctypes import POINTER, byref, c_float, c_int32, c_int64, c_void_p
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -280,6 +283,7 @@ class GemNetOC(nn.Module):
         self.out_forces = _Dense(ee, 1)
         self._runner: Optional[GemNetOCRunner] = None
         self._export_key = None
+        self._engine: Optional[GemNetOCEngine] = None
 
     @property
     def num_params(self) -> int:
@@ -371,13 +375,30 @@ class GemNetOC(nn.Module):
         pos = data.pos
         if not pos.is_cuda:
             raise NablaB200Error("GemNetOC runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
+        runner = self._get_runner()
+        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            return self._train_with(runner, data)
+        return self._forward_with(runner, data)
+
+    def _get_runner(self) -> "GemNetOCRunner":
         if self._runner is None:
             from . import _lib
 
             self._runner = GemNetOCRunner(bind(_lib.load()))
-        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            return self._train_with(self._runner, data)
-        return self._forward_with(self._runner, data)
+        return self._runner
+
+    def _sync_weights(self, runner: "GemNetOCRunner", device) -> None:
+        """(Re-)export the weights into `runner` when a parameter changed since the last export."""
+        key = (id(runner),) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+        if key != self._export_key:
+            runner.set_weights(self, device)
+            self._export_key = key
+
+    def engine(self) -> "GemNetOCEngine":
+        """The engine interface of the batch-wise optimiser loop (`optimization.ASEBatchwiseLBFGS`), as `PaiNN.engine()`."""
+        if self._engine is None:
+            self._engine = GemNetOCEngine(self, self._get_runner())
+        return self._engine
 
     def _batch_args(self, data):
         pos, batch, z = data.pos, data.batch, data.z
@@ -402,10 +423,7 @@ class GemNetOC(nn.Module):
 
     def _forward_with(self, runner: "GemNetOCRunner", data):
         """Host side of forward(): (re-)export the weights when a parameter changed, molecule pointers, the two-phase engine call."""
-        key = (id(runner),) + tuple((p.data_ptr(), p._version) for p in self.parameters())
-        if key != self._export_key:
-            runner.set_weights(self, data.pos.device)
-            self._export_key = key
+        self._sync_weights(runner, data.pos.device)
         z, pos, mol_ptr, n_mol, max_atoms = self._batch_args(data)
         return runner.run(z, pos, mol_ptr, n_mol, max_atoms)
 
@@ -422,6 +440,7 @@ class GemNetOCRunner:
         self._w = None
         self._keep = None
         self._graph_buf = self._ws = self._train_ws = self._train_graph_buf = None
+        self._status = None
         self.last_counts: Dict[str, int] = {}
 
     def __del__(self):
@@ -529,6 +548,92 @@ class GemNetOCRunner:
             check(lib.nb200_gemnet_oc_debug_h(ws.data_ptr(), byref(self._w), n_mol, n, counts, h.data_ptr(), s), "nb200_gemnet_oc_debug_h")
             return energy, forces, h
         return energy, forces
+
+
+    def count_bounds(self, sizes):
+        """Upper bounds of the five counts for molecules of `sizes` atoms (host): they hold for every geometry, see DESIGN.md 3.9."""
+        if self._w is None:
+            raise NablaB200Error("GemNetOCRunner.count_bounds before set_weights")
+        mol_ptr = (c_int32 * (len(sizes) + 1))(0, *[int(v) for v in torch.as_tensor(sizes).cumsum(0)])
+        bounds = (c_int64 * N_COUNTS)()
+        check(self.lib.nb200_gemnet_oc_count_bounds(byref(self._w), mol_ptr, len(sizes), bounds), "nb200_gemnet_oc_count_bounds")
+        return bounds
+
+    def launch(self, z, pos, mol_ptr, n_mol: int, max_atoms_per_mol: int, bounds):
+        """Asynchronous forward: one enqueue on the current stream, no host read.  -> (energy, forces, status); `status` is a device int32[8]
+        that the next launch rewrites (include/nabla_b200.h).  Graph buffer and workspace are sized by `bounds` (count_bounds), hence once per
+        batch: later launches of the same batch reuse them."""
+        if self._w is None:
+            raise NablaB200Error("GemNetOCRunner.launch before set_weights")
+        lib, n, dev = self.lib, int(z.shape[0]), pos.device
+        gbytes = lib.nb200_gemnet_oc_graph_bytes(n, max_atoms_per_mol)
+        if gbytes < 0:
+            check(int(gbytes), "nb200_gemnet_oc_graph_bytes")
+        wbytes = lib.nb200_gemnet_oc_workspace_bytes(byref(self._w), n_mol, n, bounds)
+        if wbytes < 0:
+            check(int(wbytes), "nb200_gemnet_oc_workspace_bytes")
+        self.last_workspace_bytes = int(wbytes)
+        gbuf, ws = self._buffer("_graph_buf", gbytes, dev), self._buffer("_ws", wbytes, dev)
+        if self._status is None or self._status.device != dev:
+            self._status = torch.zeros(N_COUNTS, dtype=torch.int32, device=dev)
+        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+        forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        check(lib.nb200_gemnet_oc_energy_forces_async(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol,
+                                                      gbuf.data_ptr(), gbuf.numel(), bounds, ws.data_ptr(), ws.numel(), energy.data_ptr(), forces.data_ptr(),
+                                                      self._status.data_ptr(), self._stream()), "nb200_gemnet_oc_energy_forces_async")
+        return energy, forces, self._status
+
+
+class GemNetOCEngine:
+    """What `optimization.ASEBatchwiseLBFGS` needs from a model, with `PainnEngine`'s method names: `run` (synchronous, validates),
+    `launch` (asynchronous), `e_cap`, `raise_on_status`.  There is no edge capacity to grow here: `run` derives upper bounds of the edge counts
+    from the molecule sizes of the batch, and `launch` sizes everything by them (`e_cap` is accepted and ignored)."""
+
+    def __init__(self, model: GemNetOC, runner: GemNetOCRunner):
+        self.model, self.runner, self.e_cap = model, runner, 0
+        self._batch = None
+        self.last_status = None
+
+    def run(self, z, pos, mol_ptr, n_mol: int):
+        """First evaluation of a batch: checks the batch on the host (once, not per step), fixes its bounds, launches and validates.
+        -> (energy, forces, status words on the host)."""
+        ptr_host = mol_ptr.cpu()
+        sizes = ptr_host[1:] - ptr_host[:-1]
+        if len(sizes) != n_mol or n_mol < 1 or int(ptr_host[0]) != 0 or int(sizes.min()) < 1 or int(ptr_host[-1]) != z.shape[0]:
+            raise NablaB200Error("GemNetOC: `mol_ptr` must hold n_mol + 1 increasing atom offsets starting at 0 (atoms of a molecule contiguous)")
+        max_atoms = int(sizes.max())
+        if max_atoms - 1 > self.model.max_neighbors_aint:
+            raise NablaB200Error(f"GemNetOC: a molecule has {max_atoms} atoms, more than max_neighbors_aint + 1 = {self.model.max_neighbors_aint + 1}; "
+                                 "the atom-atom graph of the compiled path keeps every in-cutoff pair")
+        self.model._sync_weights(self.runner, pos.device)
+        self._batch = ((mol_ptr.data_ptr(), n_mol, int(z.shape[0])), max_atoms, self.runner.count_bounds(sizes))
+        energy, forces, status = self.launch(z, pos, mol_ptr, n_mol)
+        host = status.cpu()
+        self.raise_on_status(host)
+        self.last_status = host
+        return energy, forces, host
+
+    def launch(self, z, pos, mol_ptr, n_mol: int, e_cap=None):
+        if self._batch is None or self._batch[0] != (mol_ptr.data_ptr(), n_mol, int(z.shape[0])):
+            raise NablaB200Error("GemNetOCEngine.launch: call run() on this batch first (it derives the bounds the launch is sized by)")
+        return self.runner.launch(z, pos, mol_ptr, n_mol, self._batch[1], self._batch[2])
+
+    @property
+    def bounds(self) -> Dict[str, int]:
+        return {k: int(self._batch[2][i]) for i, k in enumerate(C_NAMES)} if self._batch else {}
+
+    @staticmethod
+    def raise_on_status(status_host) -> None:
+        """`status_host`: the status words of a launch on the host (the first four suffice)."""
+        n_edges, err, max_deg, n_iso = (int(v) for v in status_host[:4])
+        if err == -4:
+            raise NablaB200Error(f"NB200_ECAPACITY: an edge count exceeds its bound ({n_edges} main-graph edges); `mol_ptr` changed under the engine?")
+        if err == -1:
+            raise NablaB200Error("GemNetOC: non-finite atom coordinates")
+        if err != 0:
+            from ._lib import ERRORS
+
+            raise NablaB200Error(f"GemNetOC graph construction failed: {ERRORS.get(err, err)} (max degree {max_deg}, {n_iso} atoms without neighbours)")
 
 
 class GemNetOCFn(torch.autograd.Function):

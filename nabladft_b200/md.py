@@ -60,6 +60,9 @@ class BatchwiseMD:
         dev = calculator.device
         if dev.type != "cuda":
             raise NablaB200Error("BatchwiseMD runs on CUDA only (no CPU fallback)")
+        if type(getattr(calculator, "model", None)).__name__ == "GemNetOC":
+            raise NotImplementedError("BatchwiseMD does not run GemNet-OC: its direct forces are not the gradient of its energy, so the dynamics "
+                                      "would not conserve energy; use it for relaxation (ASEBatchwiseLBFGS)")
         if int(check_every) < 1:
             raise ValueError("check_every must be >= 1")
         self.calculator, self.working_dir, self.seed, self.check_every = calculator, working_dir, int(seed), int(check_every)

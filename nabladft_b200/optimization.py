@@ -132,7 +132,7 @@ class BatchwiseCalculator:
 
 
 class PyGBatchwiseCalculator(BatchwiseCalculator):
-    """calculator.py:98-129 for `nabladft_b200.painn_oc.PaiNN` (net(data) -> (energy, forces))."""
+    """calculator.py:98-129 for `nabladft_b200.painn_oc.PaiNN` and `nabladft_b200.gemnet_oc.GemNetOC` (net(data) -> (energy, forces))."""
 
     def engine(self):
         return self.model.engine()
@@ -223,6 +223,7 @@ class ASEBatchwiseLBFGS(BatchwiseOptimizer):
     def initialize(self) -> None:  # optimizers.py:405-421
         self.nsteps = self.iteration = 0
         self.function_calls = self.force_calls = self.n_normalizations = 0
+        self.host_syncs = 0  # times run() waited for the device: 1 at the start, 1 per `check_every` steps, 1 at the end (+ 1 per logged step)
         self._state = None
 
     # ------------------------------------------------------------------------------------------------------------------
@@ -252,6 +253,7 @@ class ASEBatchwiseLBFGS(BatchwiseOptimizer):
         eng = calc.engine()
         energy, forces, st = eng.run(z, pos32, mol_ptr, n_mol)  # first evaluation: synchronous, sizes the edge capacity
         eng.e_cap = max(eng.e_cap, int(1.5 * int(st[0])) + 1024)  # head-room: the geometry moves without the host looking
+        self.host_syncs += 1
         if f_unit != 1.0:
             forces = forces * f_unit
         if self.nsteps == 0:
@@ -276,6 +278,7 @@ class ASEBatchwiseLBFGS(BatchwiseOptimizer):
                 if f_unit != 1.0:
                     forces = forces * f_unit
             host = unconv[:n_chunk].cpu()  # the only host<->device synchronisation of the loop
+            self.host_syncs += 1
             eng.raise_on_status(worst.cpu())
             zero = (host == 0).nonzero()
             if len(zero):
@@ -287,11 +290,13 @@ class ASEBatchwiseLBFGS(BatchwiseOptimizer):
                 self.nsteps = it
                 self._sync_atoms(pos)
                 self._log_device(forces, fixed)
+                self.host_syncs += 1
         self.nsteps = done_at if done_at is not None else it
         self.force_calls += self.nsteps
         self.function_calls += self.nsteps
         # normalisations counted after the stopping point belong to frozen molecules: there are none (p = 0 there)
         self.n_normalizations += int(n_norm.item())
+        self.host_syncs += 1  # this and the reads of the final geometry, energies and forces below
         if fixed is not None:
             forces = forces.masked_fill(fixed.bool()[:, None], 0.0)  # the reference's final log() zeroes them in results (calculator.py:86-88)
         self._sync_atoms(pos)
