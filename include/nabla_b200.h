@@ -547,6 +547,78 @@ int nb200_gemnet_oc_debug_h(const void* workspace, const nb200_gemnet_oc_weights
                             const int64_t* counts_host, float* h_out, void* stream);
 
 /* ----------------------------------------------------------------------------------------
+ * DimeNet++ energy + conservative forces, config/model/dimenetplusplus.yaml: DimeNetPlusPlusPotential
+ * (nablaDFT/dimenetplusplus/dimenetplusplus.py:22-113) around torch_geometric.nn.models.DimeNetPlusPlus (2.4.0).
+ * energy[m] = scale * y_m + mean, forces = -dy/dpos of the UNSCALED prediction y (dimenetplusplus.py:97-112); scale = 1, mean = 0
+ * without postprocessing.  Inference only: a reverse pass through output blocks, interaction blocks, the triplet aggregation and the
+ * bases, no parameter gradients; sums are gathers (no atomics), so two calls on the same input are bitwise equal (DESIGN.md 3.15).
+ * Supported: hidden 256, int_emb 64, basis_emb 8, out_emb 256, num_spherical 7, num_radial 6, before / after skip 1 / 2, 3 output
+ * layers, envelope exponent 5, 1 <= num_blocks <= 16, 2 <= node_latent_dim (= out_channels) <= 64, 1 <= max_neighbors <= 64;
+ * anything else is NB200_EUNSUPPORTED.
+ * Weights: one flat device buffer `w`, host offsets (floats) in the order
+ *   [NB200_DPP_G_*][NB200_DPP_I_* x num_blocks][NB200_DPP_O_* x (num_blocks + 1)]. */
+enum {
+    NB200_DPP_G_FREQ = 0,  /* [6]       rbf.freq                                                             */
+    NB200_DPP_G_ZEROS,     /* [42]      z_ln, first 6 zeros of j_l, l-major (SphericalBasisLayer)             */
+    NB200_DPP_G_NORMS,     /* [42]      N_ln = 1 / sqrt(0.5 j_{l+1}(z_ln)^2)                                 */
+    NB200_DPP_G_EMB_TI,    /* [95,256]  emb.lin.weight[:, 0:256] . emb.emb.weight[z] + emb.lin.bias (target)  */
+    NB200_DPP_G_EMB_TJ,    /* [95,256]  emb.lin.weight[:, 256:512] . emb.emb.weight[z] (source)              */
+    NB200_DPP_G_EMB_RBF_W, /* [256,6]   emb.lin_rbf.weight                                                   */
+    NB200_DPP_G_EMB_RBF_B, /* [256]     emb.lin_rbf.bias                                                     */
+    NB200_DPP_G_EMB_W3,    /* [256,256] emb.lin.weight[:, 512:768]                                           */
+    NB200_DPP_G_HEAD_W0, NB200_DPP_G_HEAD_B0, /* regr_or_cls_nn.0  [L,L], [L]          */
+    NB200_DPP_G_HEAD_W1, NB200_DPP_G_HEAD_B1, /* regr_or_cls_nn.2  [L/2,L], [L/2]      */
+    NB200_DPP_G_HEAD_W2, NB200_DPP_G_HEAD_B2, /* regr_or_cls_nn.4  [L/2,L/2], [L/2]    */
+    NB200_DPP_G_HEAD_W3, NB200_DPP_G_HEAD_B3, /* regr_or_cls_nn.6  [1,L/2], [1]        */
+    NB200_DPP_G_COUNT
+};
+enum { /* per interaction block */
+    NB200_DPP_I_RBF = 0, /* [256,6]  lin_rbf2.weight . lin_rbf1.weight */
+    NB200_DPP_I_SBF,     /* [64,42]  lin_sbf2.weight . lin_sbf1.weight */
+    NB200_DPP_I_SBF1,    /* [8,42]   lin_sbf1.weight                   */
+    NB200_DPP_I_SBF2,    /* [64,8]   lin_sbf2.weight                   */
+    NB200_DPP_I_JI_W, NB200_DPP_I_JI_B, NB200_DPP_I_KJ_W, NB200_DPP_I_KJ_B, /* [256,256], [256] */
+    NB200_DPP_I_DOWN,    /* [64,256] */
+    NB200_DPP_I_UP,      /* [256,64] */
+    NB200_DPP_I_RES_W,   /* 6 x [256,256]: layers_before_skip.0.lin{1,2}, layers_after_skip.{0,1}.lin{1,2} */
+    NB200_DPP_I_RES_B,   /* 6 x [256] */
+    NB200_DPP_I_LIN_W, NB200_DPP_I_LIN_B,
+    NB200_DPP_I_COUNT
+};
+enum { /* per output block */
+    NB200_DPP_O_RBF = 0, /* [256,6]   lin_rbf      */
+    NB200_DPP_O_UP,      /* [256,256] lin_up       */
+    NB200_DPP_O_LINS_W,  /* 3 x [256,256] lins.*   */
+    NB200_DPP_O_LINS_B,  /* 3 x [256]              */
+    NB200_DPP_O_LIN,     /* [L,256]   lin          */
+    NB200_DPP_O_COUNT
+};
+enum { NB200_DPP_C_EDGES = 0, NB200_DPP_C_TRIPLETS, NB200_DPP_C_COUNT = 4 }; /* counts_host[] of nb200_dimenet_graph_count */
+typedef struct nb200_dimenet_weights {
+    int32_t num_blocks, node_latent_dim, hidden, int_emb, basis_emb, out_emb, num_spherical, num_radial;
+    int32_t num_before_skip, num_after_skip, num_output_layers, envelope_exponent, max_neighbors;
+    float cutoff, scale, mean;
+    const float* w;          /* device */
+    const int64_t* off_host; /* host [G_COUNT + I_COUNT*num_blocks + O_COUNT*(num_blocks+1)] */
+} nb200_dimenet_weights;
+/* Bytes of the graph buffer for n_atoms (CSR by target with the radius_graph truncation: candidates in ascending index with d^2 < cutoff^2,
+ * the target included, the first max_neighbors + 1 kept, the self loop dropped; the by-source permutation; triplet offsets). */
+int64_t nb200_dimenet_graph_bytes(const nb200_dimenet_weights* w, int32_t n_atoms);
+/* Phase 1: builds the graph from pos and SYNCHRONISES once; counts_host[NB200_DPP_C_COUNT] = {edges, triplets, 0, 0}.
+ * NB200_EINVAL for z outside [0, 94] or a non-finite coordinate.  An atom without neighbours is not an error. */
+int nb200_dimenet_graph_count(const nb200_dimenet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr, int32_t n_mol,
+                              int32_t n_atoms, void* graph_buf, int64_t graph_bytes, int64_t* counts_host, void* stream);
+int64_t nb200_dimenet_workspace_bytes(const nb200_dimenet_weights* w, int32_t n_mol, int32_t n_atoms, const int64_t* counts_host);
+/* Phase 2 (same z, pos, mol_ptr and graph buffer as phase 1): energy[n_mol], forces[n_atoms,3] and, when graph_emb != NULL, the
+ * per-molecule sums of the output blocks graph_emb[n_mol, node_latent_dim] (the input of regr_or_cls_nn). */
+int nb200_dimenet_energy_forces(nb200_engine* eng, const nb200_dimenet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
+                                int32_t n_mol, int32_t n_atoms, void* graph_buf, int64_t graph_bytes, const int64_t* counts_host,
+                                void* workspace, int64_t workspace_bytes, float* energy, float* forces, float* graph_emb, void* stream);
+/* Test entry point, not a supported API: the spherical radial basis env(x) N_ln j_l(z_ln x), x = dist / cutoff, and its derivative
+ * with respect to dist, [n, 42] each, as the engine evaluates them in fp32. */
+int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, const float* dist, int32_t n, float* rbs, float* drbs, void* stream);
+
+/* ----------------------------------------------------------------------------------------
  * PhiSNet Clebsch-Gordan mixing layers (SURVEY.md section 8 f4).  Features are component-major:
  * x[rows][(order+1)^2][F], component index l*l + m (m = 0..2l), F in {32, 64, 96, 128}, orders <= 4.
  * Real CG tensors = the reference's vendored table (phisnet/nn/modules/clebsch_gordan_coefficients_L10.npz).

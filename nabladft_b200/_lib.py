@@ -69,6 +69,15 @@ class GemNetOCWeights(ctypes.Structure):
                 ("max_neighbors_aeaint", c_int32), ("w", c_void_p), ("off_host", POINTER(c_int64)), ("scale_host", POINTER(c_float))]
 
 
+class DimeNetWeights(ctypes.Structure):
+    """Mirror of `struct nb200_dimenet_weights` (include/nabla_b200.h)."""
+
+    _fields_ = [("num_blocks", c_int32), ("node_latent_dim", c_int32), ("hidden", c_int32), ("int_emb", c_int32), ("basis_emb", c_int32),
+                ("out_emb", c_int32), ("num_spherical", c_int32), ("num_radial", c_int32), ("num_before_skip", c_int32), ("num_after_skip", c_int32),
+                ("num_output_layers", c_int32), ("envelope_exponent", c_int32), ("max_neighbors", c_int32), ("cutoff", c_float), ("scale", c_float),
+                ("mean", c_float), ("w", c_void_p), ("off_host", POINTER(c_int64))]
+
+
 SIGNATURES = {
     "nb200_version": (c_int32, []),
     "nb200_last_cuda_error": (c_int32, []),
@@ -167,6 +176,13 @@ SIGNATURES = {
                                                       c_void_p, c_int64, POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                       POINTER(c_int64), c_void_p]),
     "nb200_gemnet_oc_backward": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "nb200_dimenet_graph_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32]),
+    "nb200_dimenet_graph_count": (c_int32, [POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
+                                            POINTER(c_int64), c_void_p]),
+    "nb200_dimenet_workspace_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32, c_int32, POINTER(c_int64)]),
+    "nb200_dimenet_energy_forces": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
+                                              POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_dimenet_debug_sbf_radial": (c_int32, [POINTER(DimeNetWeights), c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -1,0 +1,304 @@
+"""H100-native drop-in for `nablaDFT.dimenetplusplus.DimeNetPlusPlusPotential` (config/model/dimenetplusplus.yaml).
+
+Same constructor signature (nablaDFT/dimenetplusplus/dimenetplusplus.py:22-91), same `forward(data) -> (energy [B], forces [N, 3])` contract
+(dimenetplusplus.py:93-113: forces are -d(unscaled prediction)/d pos, the scaler is applied to the energy only, after the gradient) and the
+same state-dict names and shapes (`net.*` as torch_geometric's DimeNetPlusPlus, `regr_or_cls_nn.{0,2,4,6}`), so the yaml works with
+`_target_: nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential` and reference checkpoints load with strict=True.  The arithmetic -- the
+radius graph, the triplets, the bases, the embedding / interaction / output blocks, the regression head and the reverse pass for the forces --
+runs in `libnabla_b200.so` (`csrc/dimenet.cu`, C ABI `nb200_dimenet_*` in include/nabla_b200.h).  This file owns the parameters and their
+export into the flat buffer the C ABI takes (lin_rbf2 . lin_rbf1 and lin_sbf2 . lin_sbf1 folded, the embedding's atom thirds turned into
+per-element tables).
+
+Supported: the shipped sizes, with 1 <= dimenet_num_blocks <= 16, 2 <= node_latent_dim <= 64 and dimenet_max_num_neighbors <= 64; anything else
+raises at construction.  Inference only: in training mode with autograd the forward raises NotImplementedError (the reference's force loss
+needs a second-order pass).  No CPU fallback.
+"""
+import ctypes
+from ctypes import POINTER, byref, c_int64, c_void_p
+from typing import Dict, List, Optional, Tuple
+
+import numpy as np
+import torch
+from torch import nn
+
+from ._lib import SIGNATURES as _ALL_SIGNATURES
+from ._lib import DimeNetWeights, NablaB200Error, check
+
+# ---- canonical layout: keep in step with the enums of include/nabla_b200.h -----------------------------------------------------------------
+G_NAMES = ["FREQ", "ZEROS", "NORMS", "EMB_TI", "EMB_TJ", "EMB_RBF_W", "EMB_RBF_B", "EMB_W3", "HEAD_W0", "HEAD_B0", "HEAD_W1", "HEAD_B1",
+           "HEAD_W2", "HEAD_B2", "HEAD_W3", "HEAD_B3"]
+I_NAMES = ["RBF", "SBF", "SBF1", "SBF2", "JI_W", "JI_B", "KJ_W", "KJ_B", "DOWN", "UP", "RES_W", "RES_B", "LIN_W", "LIN_B"]
+O_NAMES = ["RBF", "UP", "LINS_W", "LINS_B", "LIN"]
+N_COUNTS = 4
+_FIXED = dict(dimenet_hidden_channels=256, dimenet_int_emb_size=64, dimenet_basis_emb_size=8, dimenet_out_emb_channels=256,
+              dimenet_num_spherical=7, dimenet_num_radial=6, dimenet_envelope_exponent=5, dimenet_num_before_skip=1, dimenet_num_after_skip=2,
+              dimenet_num_output_layers=3)
+
+SIGNATURES = {k: v for k, v in _ALL_SIGNATURES.items() if k.startswith("nb200_dimenet_")}
+
+
+def bind(lib):
+    """Attach the DimeNet++ prototypes to a loaded library (libnabla_b200.so is bound by _lib.load(); this is for tests/emu)."""
+    for name, (res, args) in SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = res, args
+    return lib
+
+
+def sbf_radial_constants(num_spherical: int = 7, num_radial: int = 6) -> Tuple[np.ndarray, np.ndarray]:
+    """(z_ln, N_ln) [num_spherical, num_radial]: the first zeros of the spherical Bessel functions j_l (those of j_l interlace those of
+    j_{l-1}) and the normalisers 1 / sqrt(0.5 j_{l+1}(z_ln)^2) of PyG's SphericalBasisLayer."""
+    from scipy.optimize import brentq
+    from scipy.special import spherical_jn
+
+    k = num_radial + num_spherical
+    z = np.zeros((num_spherical, k))
+    z[0] = np.pi * np.arange(1, k + 1)
+    for l in range(1, num_spherical):
+        for m in range(k - l):
+            z[l, m] = brentq(lambda x, l=l: spherical_jn(l, x), z[l - 1, m], z[l - 1, m + 1], xtol=1e-15)
+    z = z[:, :num_radial]
+    norms = np.stack([np.sqrt(2.0) / np.abs(spherical_jn(l + 1, z[l])) for l in range(num_spherical)])
+    return z, norms
+
+
+# ---- parameter holders with torch_geometric's attribute names -----------------------------------------------------------------------------
+class _Swish(nn.Module):
+    def forward(self, x):
+        return x * x.sigmoid()
+
+
+class _Bessel(nn.Module):
+    def __init__(self, num_radial):
+        super().__init__()
+        self.freq = nn.Parameter(torch.arange(1, num_radial + 1, dtype=torch.float32) * np.pi)
+
+
+class _Embedding(nn.Module):
+    def __init__(self, num_radial, hidden):
+        super().__init__()
+        self.emb = nn.Embedding(95, hidden)
+        nn.init.uniform_(self.emb.weight, -3 ** 0.5, 3 ** 0.5)
+        self.lin_rbf = nn.Linear(num_radial, hidden)
+        self.lin = nn.Linear(3 * hidden, hidden)
+
+
+class _Residual(nn.Module):
+    def __init__(self, hidden):
+        super().__init__()
+        self.lin1 = nn.Linear(hidden, hidden)
+        self.lin2 = nn.Linear(hidden, hidden)
+
+
+class _Interaction(nn.Module):
+    def __init__(self, hidden, int_emb, basis_emb, num_spherical, num_radial, num_before_skip, num_after_skip):
+        super().__init__()
+        self.lin_rbf1 = nn.Linear(num_radial, basis_emb, bias=False)
+        self.lin_rbf2 = nn.Linear(basis_emb, hidden, bias=False)
+        self.lin_sbf1 = nn.Linear(num_spherical * num_radial, basis_emb, bias=False)
+        self.lin_sbf2 = nn.Linear(basis_emb, int_emb, bias=False)
+        self.lin_kj = nn.Linear(hidden, hidden)
+        self.lin_ji = nn.Linear(hidden, hidden)
+        self.lin_down = nn.Linear(hidden, int_emb, bias=False)
+        self.lin_up = nn.Linear(int_emb, hidden, bias=False)
+        self.layers_before_skip = nn.ModuleList([_Residual(hidden) for _ in range(num_before_skip)])
+        self.lin = nn.Linear(hidden, hidden)
+        self.layers_after_skip = nn.ModuleList([_Residual(hidden) for _ in range(num_after_skip)])
+
+
+class _Output(nn.Module):
+    def __init__(self, num_radial, hidden, out_emb, out_channels, num_layers):
+        super().__init__()
+        self.lin_rbf = nn.Linear(num_radial, hidden, bias=False)
+        self.lin_up = nn.Linear(hidden, out_emb, bias=False)
+        self.lins = nn.ModuleList([nn.Linear(out_emb, out_emb) for _ in range(num_layers)])
+        self.lin = nn.Linear(out_emb, out_channels, bias=False)
+        nn.init.zeros_(self.lin.weight)  # PyG's output_initializer='zeros'
+
+
+class _Core(nn.Module):
+    def __init__(self, hidden, out_channels, num_blocks, int_emb, basis_emb, out_emb, num_spherical, num_radial, num_before_skip, num_after_skip,
+                 num_output_layers):
+        super().__init__()
+        self.rbf = _Bessel(num_radial)
+        self.emb = _Embedding(num_radial, hidden)
+        self.output_blocks = nn.ModuleList([_Output(num_radial, hidden, out_emb, out_channels, num_output_layers) for _ in range(num_blocks + 1)])
+        self.interaction_blocks = nn.ModuleList([_Interaction(hidden, int_emb, basis_emb, num_spherical, num_radial, num_before_skip, num_after_skip)
+                                                 for _ in range(num_blocks)])
+
+
+class DimeNetPlusPlusPotential(nn.Module):
+    def __init__(self, node_latent_dim: int, scaler=None, dimenet_hidden_channels=128, dimenet_num_blocks=4, dimenet_int_emb_size=64,
+                 dimenet_basis_emb_size=8, dimenet_out_emb_channels=256, dimenet_num_spherical=7, dimenet_num_radial=6, dimenet_max_num_neighbors=32,
+                 dimenet_envelope_exponent=5, dimenet_num_before_skip=1, dimenet_num_after_skip=2, dimenet_num_output_layers=3, cutoff=5.0,
+                 do_postprocessing=False):
+        super().__init__()
+        given = dict(locals())
+        bad = [f"{k}={given[k]!r} (built: {v!r})" for k, v in _FIXED.items() if given[k] != v]
+        if not 1 <= dimenet_num_blocks <= 16:
+            bad.append(f"dimenet_num_blocks={dimenet_num_blocks} (built: 1..16)")
+        if not 2 <= node_latent_dim <= 64:
+            bad.append(f"node_latent_dim={node_latent_dim} (built: 2..64)")
+        if not 1 <= dimenet_max_num_neighbors <= 64:
+            bad.append(f"dimenet_max_num_neighbors={dimenet_max_num_neighbors} (built: 1..64)")
+        if not cutoff > 0:
+            bad.append(f"cutoff={cutoff}")
+        if bad:
+            raise NablaB200Error("DimeNetPlusPlusPotential: configuration outside the compiled path (config/model/dimenetplusplus.yaml): " + "; ".join(bad))
+        self.scaler, self.do_postprocessing = scaler, do_postprocessing
+        self.node_latent_dim, self.num_blocks = node_latent_dim, dimenet_num_blocks
+        self.max_num_neighbors, self.cutoff = dimenet_max_num_neighbors, float(cutoff)
+        self.net = _Core(dimenet_hidden_channels, node_latent_dim, dimenet_num_blocks, dimenet_int_emb_size, dimenet_basis_emb_size,
+                         dimenet_out_emb_channels, dimenet_num_spherical, dimenet_num_radial, dimenet_num_before_skip, dimenet_num_after_skip,
+                         dimenet_num_output_layers)
+        L = node_latent_dim
+        self.regr_or_cls_nn = nn.Sequential(nn.Linear(L, L), _Swish(), nn.Linear(L, L // 2), _Swish(), nn.Linear(L // 2, L // 2), _Swish(),
+                                            nn.Linear(L // 2, 1))
+        self._runner: Optional[DimeNetRunner] = None
+        self._export_key = None
+
+    # ---- export: reference-named tensors -> flat buffer (include/nabla_b200.h NB200_DPP_*) ---------------------------------------------------
+    def export(self, device) -> Tuple[torch.Tensor, List[int]]:
+        f = lambda t: t.detach().to(torch.float64)
+        net, H = self.net, 256
+        z, norms = sbf_radial_constants()
+        W = f(net.emb.lin.weight)
+        emb = f(net.emb.emb.weight)
+        head = [f(t) for m in (0, 2, 4, 6) for t in (self.regr_or_cls_nn[m].weight, self.regr_or_cls_nn[m].bias)]
+        entries: List = [f(net.rbf.freq), torch.from_numpy(z).reshape(-1), torch.from_numpy(norms).reshape(-1),
+                         emb @ W[:, :H].t() + f(net.emb.lin.bias), emb @ W[:, H:2 * H].t(), f(net.emb.lin_rbf.weight), f(net.emb.lin_rbf.bias),
+                         W[:, 2 * H:]] + head
+        for b in net.interaction_blocks:
+            res = list(b.layers_before_skip) + list(b.layers_after_skip)
+            entries += [f(b.lin_rbf2.weight) @ f(b.lin_rbf1.weight), f(b.lin_sbf2.weight) @ f(b.lin_sbf1.weight), f(b.lin_sbf1.weight),
+                        f(b.lin_sbf2.weight), f(b.lin_ji.weight), f(b.lin_ji.bias), f(b.lin_kj.weight), f(b.lin_kj.bias), f(b.lin_down.weight),
+                        f(b.lin_up.weight), [f(getattr(r, n).weight) for r in res for n in ("lin1", "lin2")],
+                        [f(getattr(r, n).bias) for r in res for n in ("lin1", "lin2")], f(b.lin.weight), f(b.lin.bias)]
+        for o in net.output_blocks:
+            entries += [f(o.lin_rbf.weight), f(o.lin_up.weight), [f(l.weight) for l in o.lins], [f(l.bias) for l in o.lins], f(o.lin.weight)]
+        assert len(entries) == len(G_NAMES) + len(I_NAMES) * self.num_blocks + len(O_NAMES) * (self.num_blocks + 1)
+        flat, offs, pos = [], [], 0
+        for ent in entries:
+            pos = (pos + 63) // 64 * 64  # 256-byte alignment of every matrix
+            offs.append(pos)
+            for t_ in (ent if isinstance(ent, list) else [ent]):
+                flat.append((pos, t_.reshape(-1)))
+                pos += t_.numel()
+        buf = torch.zeros(pos + 64, dtype=torch.float32)
+        for p0, t_ in flat:
+            buf[p0:p0 + t_.numel()] = t_.to(torch.float32).cpu()
+        return buf.to(device), offs
+
+    def _scale_mean(self) -> Tuple[float, float]:
+        if self.scaler and self.do_postprocessing:
+            return float(self.scaler["scale_"]), float(self.scaler["mean_"])
+        return 1.0, 0.0
+
+    # ---- forward ------------------------------------------------------------------------------------------------------------------------------
+    def forward(self, data):
+        """data.z [N], data.pos [N,3], data.batch [N] (sorted) -> (energy [B], forces [N,3])   (dimenetplusplus.py:93-113)."""
+        if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("nabladft_b200 DimeNetPlusPlusPotential is inference-only (training needs a second-order pass through the "
+                                      "forces): call .eval() / torch.no_grad()")
+        energy, forces, _ = self.run(data.z, data.pos, data.batch)
+        return energy, forces
+
+    def run(self, z, pos, batch):
+        """-> (energy [B], forces [N,3], graph embeddings [B, node_latent_dim])."""
+        if not pos.is_cuda:
+            raise NablaB200Error("DimeNetPlusPlusPotential runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
+        runner = self._get_runner()
+        self._sync_weights(runner, pos.device)
+        return runner.run(*self.batch_args(z, pos, batch))
+
+    def _get_runner(self) -> "DimeNetRunner":
+        if self._runner is None:
+            from . import _lib
+
+            self._runner = DimeNetRunner(bind(_lib.load()))
+        return self._runner
+
+    def _sync_weights(self, runner: "DimeNetRunner", device) -> None:
+        key = (id(runner), str(device), self._scale_mean()) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+        if key != self._export_key:
+            runner.set_weights(self, device)
+            self._export_key = key
+
+    @staticmethod
+    def batch_args(z, pos, batch):
+        if batch.numel() and bool((batch[1:] < batch[:-1]).any()):
+            raise NablaB200Error("DimeNetPlusPlusPotential: `batch` must be sorted (atoms of a molecule contiguous), as PyG collation produces it")
+        n_mol = int(batch[-1].item()) + 1 if batch.numel() else 0
+        counts = torch.bincount(batch, minlength=n_mol)
+        mol_ptr = torch.zeros(n_mol + 1, dtype=torch.int32, device=pos.device)
+        mol_ptr[1:] = torch.cumsum(counts, 0)
+        return z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr, n_mol
+
+
+class DimeNetRunner:
+    """Host driver of `nb200_dimenet_*`: owns the engine handle, the exported weights, the graph buffer and the workspace."""
+
+    def __init__(self, lib):
+        self.lib = lib
+        h = c_void_p()
+        check(lib.nb200_engine_create(byref(h)), "nb200_engine_create")
+        self._h = h
+        self._w = None
+        self._keep = None
+        self._graph_buf = self._ws = None
+        self.last_counts: Dict[str, int] = {}
+
+    def __del__(self):
+        try:
+            if self._h:
+                self.lib.nb200_engine_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def _stream(self):
+        return c_void_p(torch.cuda.current_stream().cuda_stream)
+
+    def set_weights(self, model: DimeNetPlusPlusPotential, device):
+        buf, offs = model.export(device)
+        off_arr = (c_int64 * len(offs))(*offs)
+        scale, mean = model._scale_mean()
+        w = DimeNetWeights(model.num_blocks, model.node_latent_dim, 256, 64, 8, 256, 7, 6, 1, 2, 3, 5, model.max_num_neighbors, model.cutoff,
+                           scale, mean, buf.data_ptr(), ctypes.cast(off_arr, POINTER(c_int64)))
+        self._w, self._keep = w, (buf, off_arr)
+
+    def _buffer(self, attr: str, nbytes: int, device):
+        cur = getattr(self, attr)
+        if cur is None or cur.numel() < nbytes or cur.device != device:
+            setattr(self, attr, None)  # free the old buffer before the larger one is allocated
+            cur = torch.empty(int(nbytes * 1.25) + 256, dtype=torch.uint8, device=device)
+            setattr(self, attr, cur)
+        return cur
+
+    def run(self, z, pos, mol_ptr, n_mol: int):
+        """Two-phase call: graph (one synchronisation for the counts), workspace, energies / forces / graph embeddings."""
+        if self._w is None:
+            raise NablaB200Error("DimeNetRunner.run before set_weights")
+        lib, n, dev = self.lib, int(z.shape[0]), pos.device
+        if n == 0 or n_mol == 0:
+            raise NablaB200Error("DimeNetPlusPlusPotential: empty batch")
+        s = self._stream()
+        gbytes = lib.nb200_dimenet_graph_bytes(byref(self._w), n)
+        if gbytes < 0:
+            check(int(gbytes), "nb200_dimenet_graph_bytes")
+        gbuf = self._buffer("_graph_buf", gbytes, dev)
+        counts = (c_int64 * N_COUNTS)()
+        check(lib.nb200_dimenet_graph_count(byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(), gbuf.numel(),
+                                            counts, s), "nb200_dimenet_graph_count")
+        self.last_counts = {"edges": int(counts[0]), "triplets": int(counts[1])}
+        wbytes = lib.nb200_dimenet_workspace_bytes(byref(self._w), n_mol, n, counts)
+        if wbytes < 0:
+            check(int(wbytes), "nb200_dimenet_workspace_bytes")
+        ws = self._buffer("_ws", wbytes, dev)
+        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+        forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        emb = torch.empty(n_mol, self._w.node_latent_dim, dtype=torch.float32, device=dev)
+        check(lib.nb200_dimenet_energy_forces(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(),
+                                              gbuf.numel(), counts, ws.data_ptr(), ws.numel(), energy.data_ptr(), forces.data_ptr(), emb.data_ptr(), s),
+              "nb200_dimenet_energy_forces")
+        return energy, forces, emb

@@ -22,6 +22,7 @@ SWAPS = {
     "painn-oc": [("nablaDFT.painn_pyg.PaiNN", "nabladft_b200.painn_oc.PaiNN")],
     "qhnet": [("nablaDFT.qhnet.QHNet", "nabladft_b200.qhnet.QHNet")],
     "gemnet-oc": [("nablaDFT.gemnet_oc.GemNetOC", "nabladft_b200.gemnet_oc.GemNetOC")],
+    "dimenetplusplus": [("nablaDFT.dimenetplusplus.DimeNetPlusPlusPotential", "nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential")],
 }
 SWAPS["schnet"] = [(a.replace("representation.PaiNN", "representation.SchNet"), b.replace("spk.PaiNN", "spk.SchNet")) for a, b in SWAPS["painn"]]
 
