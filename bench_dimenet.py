@@ -4,6 +4,11 @@ synthetic molecules and on tiled fixture molecules, graph sizes, the engine's pe
 kernels), GEMM FLOP/s from shapes over GEMM kernel time, the CPU float64 oracle on a bounded sample, and the card it ran on.  One JSON line.
 
     python bench_dimenet.py --batch 256 [--steps 5 --warmup 2 --oracle-mols 2]
+    python bench_dimenet.py --train [--batch 256 --steps 5 --warmup 2]
+
+--train: one training step (forward, L1(E) + L1(F), backward through nb200_dimenet_train_grads, Adam lr 1e-4 as the yaml has it) on the same
+synthetic batch: ms per step (CUDA events, warm-up excluded), molecules/s, the per-category split of the gradient call (weight-gradient
+reductions are counted as force_assembly there: that call assembles no forces) and its workspace bytes.
 """
 import argparse
 import json
@@ -38,6 +43,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--oracle-mols", type=int, default=2, help="molecules the CPU float64 oracle runs (its time is scaled to the batch)")
+    ap.add_argument("--train", action="store_true", help="time a training step instead of the energy + forces call")
     args = ap.parse_args()
     import ctypes
 
@@ -82,6 +88,8 @@ def main():
     runner = net._get_runner()
     s = synth_batch(0, args.batch)
     synth = batch_of(s["z"], s["pos"], s["mol_ptr"])
+    if args.train:
+        return train_main(args, net, runner, synth, s)
     ms_synth = timed(synth)
     counts = dict(runner.last_counts)
     n_atoms = int(len(s["z"]))
@@ -127,6 +135,79 @@ def main():
         "oracle_cpu_float64": {"molecules": k, "s_per_molecule": round(oracle_s_per_mol, 3),
                                "speedup_vs_oracle": round(oracle_s_per_mol * args.batch / (ms_synth / 1e3), 1)},
         "card": card, "steps": args.steps, "warmup": args.warmup,
+    }
+    print(json.dumps(out))
+
+
+def card_name() -> str:
+    import torch
+
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
+                              timeout=30).stdout.strip().splitlines()[torch.cuda.current_device()]
+    except Exception as exc:  # noqa: BLE001
+        return f"{torch.cuda.get_device_name()} (power limit unknown: {exc})"
+
+
+def train_main(args, net, runner, synth, s):
+    import ctypes
+
+    import torch
+
+    from nabladft_b200.dimenetplusplus import DimeNetEnergyFn
+
+    gen = torch.Generator().manual_seed(0)
+    e_t = (torch.randn(args.batch, generator=gen) - 40.0).cuda()
+    f_t = (0.1 * torch.randn(len(s["z"]), 3, generator=gen)).cuda()
+    opt = torch.optim.Adam(net.parameters(), lr=1e-4)
+    net.train()
+
+    def step():
+        opt.zero_grad(set_to_none=True)
+        e, f = net(synth)
+        loss = (e - e_t).abs().mean() + (f - f_t).abs().mean()
+        loss.backward()
+        opt.step()
+
+    for _ in range(args.warmup):
+        step()
+    torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(args.steps):
+        step()
+    b.record()
+    torch.cuda.synchronize()
+    ms = a.elapsed_time(b) / args.steps
+    counts = dict(runner.last_counts)
+    # per-category split of the gradient call alone (nb200_dimenet_train_grads)
+    lib = runner.lib
+    z, pos, mol_ptr, n_mol = net.batch_args(synth.z, synth.pos, synth.batch)
+    flat, offs = net._export_impl(detach=True)
+    runner.bind(net, flat, offs)
+    se, sf = torch.ones(n_mol, device="cuda"), torch.ones(len(s["z"]), 3, device="cuda")
+    runner.train_grads(z, pos, mol_ptr, n_mol, se, sf)
+    torch.cuda.synchronize()
+    c0, c1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    lib.nb200_engine_set_timing(runner._h, 1)
+    c0.record()
+    runner.train_grads(z, pos, mol_ptr, n_mol, se, sf)
+    c1.record()
+    torch.cuda.synchronize()
+    ms_cat = (ctypes.c_float * 16)()
+    n_cat = (ctypes.c_int32 * 16)()
+    lib.nb200_engine_read_timings(runner._h, ms_cat, n_cat, 16)
+    lib.nb200_engine_set_timing(runner._h, 0)
+    names = list(CATS)
+    names[CATS.index("force_assembly")] = "weight_gradients"
+    split = {names[i]: round(ms_cat[i], 3) for i in range(len(CATS))}
+    cnt = (ctypes.c_int64 * 4)(counts["edges"], counts["triplets"], 0, 0)
+    ws = lib.nb200_dimenet_train_workspace_bytes(ctypes.byref(runner._w), n_mol, len(s["z"]), cnt)
+    out = {
+        "metric": "dimenet_train_step_molecules_per_s", "value": round(args.batch / (ms / 1e3), 2), "batch": args.batch, "ms_per_step": round(ms, 3),
+        "atoms": int(len(s["z"])), "edges": counts["edges"], "triplets": counts["triplets"],
+        "train_grads_call_ms_timed": round(c0.elapsed_time(c1), 3), "train_grads_ms_by_category": split, "train_workspace_bytes": int(ws),
+        "peak_memory_bytes": int(torch.cuda.max_memory_allocated()), "card": card_name(), "steps": args.steps, "warmup": args.warmup,
     }
     print(json.dumps(out))
 

@@ -550,8 +550,9 @@ int nb200_gemnet_oc_debug_h(const void* workspace, const nb200_gemnet_oc_weights
  * DimeNet++ energy + conservative forces, config/model/dimenetplusplus.yaml: DimeNetPlusPlusPotential
  * (nablaDFT/dimenetplusplus/dimenetplusplus.py:22-113) around torch_geometric.nn.models.DimeNetPlusPlus (2.4.0).
  * energy[m] = scale * y_m + mean, forces = -dy/dpos of the UNSCALED prediction y (dimenetplusplus.py:97-112); scale = 1, mean = 0
- * without postprocessing.  Inference only: a reverse pass through output blocks, interaction blocks, the triplet aggregation and the
- * bases, no parameter gradients; sums are gathers (no atomics), so two calls on the same input are bitwise equal (DESIGN.md 3.15).
+ * without postprocessing.  nb200_dimenet_energy_forces runs a reverse pass through output blocks, interaction blocks, the triplet
+ * aggregation and the bases; its sums are gathers (no atomics), so two calls on the same input are bitwise equal (DESIGN.md 3.15).
+ * nb200_dimenet_train_grads gives the parameter gradients of an energy and force loss.
  * Supported: hidden 256, int_emb 64, basis_emb 8, out_emb 256, num_spherical 7, num_radial 6, before / after skip 1 / 2, 3 output
  * layers, envelope exponent 5, 1 <= num_blocks <= 16, 2 <= node_latent_dim (= out_channels) <= 64, 1 <= max_neighbors <= 64;
  * anything else is NB200_EUNSUPPORTED.
@@ -614,6 +615,20 @@ int64_t nb200_dimenet_workspace_bytes(const nb200_dimenet_weights* w, int32_t n_
 int nb200_dimenet_energy_forces(nb200_engine* eng, const nb200_dimenet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
                                 int32_t n_mol, int32_t n_atoms, void* graph_buf, int64_t graph_bytes, const int64_t* counts_host,
                                 void* workspace, int64_t workspace_bytes, float* energy, float* forces, float* graph_emb, void* stream);
+/* Training (DESIGN.md 3.15.1): bytes of the workspace of nb200_dimenet_train_grads (the inference workspace plus the tangent arrays). */
+int64_t nb200_dimenet_train_workspace_bytes(const nb200_dimenet_weights* w, int32_t n_mol, int32_t n_atoms, const int64_t* counts_host);
+/* Parameter gradients of a loss L(E, F) (same z, pos, mol_ptr, graph buffer and counts as phase 1): given the seeds
+ * seed_energy[n_mol] = dL/dE and seed_forces[n_atoms,3] = dL/dF (either may be NULL), writes
+ *   grads = sum_m seed_energy[m] scale dy_m/dw + sum_i seed_forces[i] . dF_i/dw
+ * into `grads`, a buffer with the layout and offsets of the weight buffer (zeroed first, up to the end of the last entry).  Entries y does not
+ * read (ZEROS, NORMS, SBF1, SBF2) stay zero; the folded entries (I_RBF, I_SBF, EMB_TI, EMB_TJ) get the gradient w.r.t. the folded matrix.
+ * One call recomputes the forward, runs the unit-seed reverse pass and, with seed_forces, its tangent along seed_forces (forward-over-
+ * reverse).  Weight-gradient sums use atomics: two calls agree to rounding, not bitwise.  NB200_EINVAL for a NULL pointer (seeds excepted),
+ * a short workspace or graph buffer; NB200_EUNSUPPORTED for a configuration outside the list above. */
+int nb200_dimenet_train_grads(nb200_engine* eng, const nb200_dimenet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
+                              int32_t n_mol, int32_t n_atoms, void* graph_buf, int64_t graph_bytes, const int64_t* counts_host,
+                              void* workspace, int64_t workspace_bytes, const float* seed_energy, const float* seed_forces, float* grads,
+                              void* stream);
 /* Test entry point, not a supported API: the spherical radial basis env(x) N_ln j_l(z_ln x), x = dist / cutoff, and its derivative
  * with respect to dist, [n, 42] each, as the engine evaluates them in fp32. */
 int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, const float* dist, int32_t n, float* rbs, float* drbs, void* stream);

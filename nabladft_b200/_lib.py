@@ -182,6 +182,9 @@ SIGNATURES = {
     "nb200_dimenet_workspace_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32, c_int32, POINTER(c_int64)]),
     "nb200_dimenet_energy_forces": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
                                               POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_dimenet_train_workspace_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32, c_int32, POINTER(c_int64)]),
+    "nb200_dimenet_train_grads": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
+                                            POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_dimenet_debug_sbf_radial": (c_int32, [POINTER(DimeNetWeights), c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
 }
 

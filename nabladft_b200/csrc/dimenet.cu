@@ -821,3 +821,5 @@ extern "C" int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, co
     const Ctx c{e, (cudaStream_t)stream, w};
     return pfor(e, c.s, CAT_FILTER, (int64_t)n * NSR, RbsK{dist, c.G(NB200_DPP_G_ZEROS), c.G(NB200_DPP_G_NORMS), 1.0f / w->cutoff, rbs, drbs});
 }
+
+#include "dimenet_train.inc"

@@ -9,9 +9,11 @@ runs in `libnabla_b200.so` (`csrc/dimenet.cu`, C ABI `nb200_dimenet_*` in includ
 export into the flat buffer the C ABI takes (lin_rbf2 . lin_rbf1 and lin_sbf2 . lin_sbf1 folded, the embedding's atom thirds turned into
 per-element tables).
 
-Supported: the shipped sizes, with 1 <= dimenet_num_blocks <= 16, 2 <= node_latent_dim <= 64 and dimenet_max_num_neighbors <= 64; anything else
-raises at construction.  Inference only: in training mode with autograd the forward raises NotImplementedError (the reference's force loss
-needs a second-order pass).  No CPU fallback.
+Training: in training mode with autograd the forward goes through `DimeNetEnergyFn`, whose backward is `nb200_dimenet_train_grads` (the
+parameter gradients of energy and force losses, the force term by forward-over-reverse, DESIGN.md 3.15.1); the export is then differentiable,
+so autograd carries the flat-buffer gradient back to every reference-named parameter.  Supported: the shipped sizes, with
+1 <= dimenet_num_blocks <= 16, 2 <= node_latent_dim <= 64 and dimenet_max_num_neighbors <= 64; anything else raises at construction.  No CPU
+fallback: CPU tensors raise NablaB200Error in eval mode and NotImplementedError in training mode.
 """
 import ctypes
 from ctypes import POINTER, byref, c_int64, c_void_p
@@ -159,13 +161,20 @@ class DimeNetPlusPlusPotential(nn.Module):
 
     # ---- export: reference-named tensors -> flat buffer (include/nabla_b200.h NB200_DPP_*) ---------------------------------------------------
     def export(self, device) -> Tuple[torch.Tensor, List[int]]:
-        f = lambda t: t.detach().to(torch.float64)
+        buf, offs = self._export_impl(detach=True)
+        return buf.to(device), offs
+
+    def _export_impl(self, detach: bool) -> Tuple[torch.Tensor, List[int]]:
+        """The flat float32 buffer on the parameters' device, folds in float64.  detach=False keeps the graph, so a gradient w.r.t. the
+        buffer (nb200_dimenet_train_grads) reaches every reference-named parameter, the folded lin_rbf1/2, lin_sbf1/2 and emb included."""
+        f = (lambda t: t.detach().to(torch.float64)) if detach else (lambda t: t.to(torch.float64))
         net, H = self.net, 256
+        dev = net.rbf.freq.device
         z, norms = sbf_radial_constants()
         W = f(net.emb.lin.weight)
         emb = f(net.emb.emb.weight)
         head = [f(t) for m in (0, 2, 4, 6) for t in (self.regr_or_cls_nn[m].weight, self.regr_or_cls_nn[m].bias)]
-        entries: List = [f(net.rbf.freq), torch.from_numpy(z).reshape(-1), torch.from_numpy(norms).reshape(-1),
+        entries: List = [f(net.rbf.freq), torch.from_numpy(z).reshape(-1).to(dev), torch.from_numpy(norms).reshape(-1).to(dev),
                          emb @ W[:, :H].t() + f(net.emb.lin.bias), emb @ W[:, H:2 * H].t(), f(net.emb.lin_rbf.weight), f(net.emb.lin_rbf.bias),
                          W[:, 2 * H:]] + head
         for b in net.interaction_blocks:
@@ -177,17 +186,18 @@ class DimeNetPlusPlusPotential(nn.Module):
         for o in net.output_blocks:
             entries += [f(o.lin_rbf.weight), f(o.lin_up.weight), [f(l.weight) for l in o.lins], [f(l.bias) for l in o.lins], f(o.lin.weight)]
         assert len(entries) == len(G_NAMES) + len(I_NAMES) * self.num_blocks + len(O_NAMES) * (self.num_blocks + 1)
-        flat, offs, pos = [], [], 0
+        pieces, offs, pos = [], [], 0
         for ent in entries:
-            pos = (pos + 63) // 64 * 64  # 256-byte alignment of every matrix
-            offs.append(pos)
+            start = (pos + 63) // 64 * 64  # 256-byte alignment of every matrix
+            if start > pos:
+                pieces.append(torch.zeros(start - pos, dtype=torch.float32, device=dev))
+            offs.append(start)
+            pos = start
             for t_ in (ent if isinstance(ent, list) else [ent]):
-                flat.append((pos, t_.reshape(-1)))
+                pieces.append(t_.reshape(-1).to(torch.float32))
                 pos += t_.numel()
-        buf = torch.zeros(pos + 64, dtype=torch.float32)
-        for p0, t_ in flat:
-            buf[p0:p0 + t_.numel()] = t_.to(torch.float32).cpu()
-        return buf.to(device), offs
+        pieces.append(torch.zeros(64, dtype=torch.float32, device=dev))
+        return torch.cat(pieces), offs
 
     def _scale_mean(self) -> Tuple[float, float]:
         if self.scaler and self.do_postprocessing:
@@ -196,10 +206,17 @@ class DimeNetPlusPlusPotential(nn.Module):
 
     # ---- forward ------------------------------------------------------------------------------------------------------------------------------
     def forward(self, data):
-        """data.z [N], data.pos [N,3], data.batch [N] (sorted) -> (energy [B], forces [N,3])   (dimenetplusplus.py:93-113)."""
+        """data.z [N], data.pos [N,3], data.batch [N] (sorted) -> (energy [B], forces [N,3])   (dimenetplusplus.py:93-113).  In training mode
+        with autograd the outputs are differentiable w.r.t. every parameter (DimeNetEnergyFn), forces included: what the reference gets from
+        create_graph=True.  They are bitwise equal to the eval-mode outputs."""
         if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("nabladft_b200 DimeNetPlusPlusPotential is inference-only (training needs a second-order pass through the "
-                                      "forces): call .eval() / torch.no_grad()")
+            if not data.pos.is_cuda:
+                raise NotImplementedError("nabladft_b200 DimeNetPlusPlusPotential trains on CUDA tensors only (sm_90a engine; there is no CPU path)")
+            runner = self._get_runner()
+            flat, offs = self._export_impl(detach=False)
+            self._export_key = None  # the runner now holds this step's buffer; the next eval call exports again
+            z, pos, mol_ptr, n_mol = self.batch_args(data.z, data.pos, data.batch)
+            return DimeNetEnergyFn.apply(flat, self, runner, offs, z, pos, mol_ptr, n_mol)
         energy, forces, _ = self.run(data.z, data.pos, data.batch)
         return energy, forces
 
@@ -260,7 +277,10 @@ class DimeNetRunner:
         return c_void_p(torch.cuda.current_stream().cuda_stream)
 
     def set_weights(self, model: DimeNetPlusPlusPotential, device):
-        buf, offs = model.export(device)
+        self.bind(model, *model.export(device))
+
+    def bind(self, model: DimeNetPlusPlusPotential, buf: torch.Tensor, offs: List[int]):
+        """Use `buf` (a flat float32 buffer in the layout of `model.export`, kept alive here) as the weights."""
         off_arr = (c_int64 * len(offs))(*offs)
         scale, mean = model._scale_mean()
         w = DimeNetWeights(model.num_blocks, model.node_latent_dim, 256, 64, 8, 256, 7, 6, 1, 2, 3, 5, model.max_num_neighbors, model.cutoff,
@@ -280,17 +300,8 @@ class DimeNetRunner:
         if self._w is None:
             raise NablaB200Error("DimeNetRunner.run before set_weights")
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        if n == 0 or n_mol == 0:
-            raise NablaB200Error("DimeNetPlusPlusPotential: empty batch")
         s = self._stream()
-        gbytes = lib.nb200_dimenet_graph_bytes(byref(self._w), n)
-        if gbytes < 0:
-            check(int(gbytes), "nb200_dimenet_graph_bytes")
-        gbuf = self._buffer("_graph_buf", gbytes, dev)
-        counts = (c_int64 * N_COUNTS)()
-        check(lib.nb200_dimenet_graph_count(byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(), gbuf.numel(),
-                                            counts, s), "nb200_dimenet_graph_count")
-        self.last_counts = {"edges": int(counts[0]), "triplets": int(counts[1])}
+        gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
         wbytes = lib.nb200_dimenet_workspace_bytes(byref(self._w), n_mol, n, counts)
         if wbytes < 0:
             check(int(wbytes), "nb200_dimenet_workspace_bytes")
@@ -302,3 +313,63 @@ class DimeNetRunner:
                                               gbuf.numel(), counts, ws.data_ptr(), ws.numel(), energy.data_ptr(), forces.data_ptr(), emb.data_ptr(), s),
               "nb200_dimenet_energy_forces")
         return energy, forces, emb
+
+    def _graph(self, z, pos, mol_ptr, n_mol: int):
+        lib, n = self.lib, int(z.shape[0])
+        if n == 0 or n_mol == 0:
+            raise NablaB200Error("DimeNetPlusPlusPotential: empty batch")
+        gbytes = lib.nb200_dimenet_graph_bytes(byref(self._w), n)
+        if gbytes < 0:
+            check(int(gbytes), "nb200_dimenet_graph_bytes")
+        gbuf = self._buffer("_graph_buf", gbytes, pos.device)
+        counts = (c_int64 * N_COUNTS)()
+        check(lib.nb200_dimenet_graph_count(byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(), gbuf.numel(),
+                                            counts, self._stream()), "nb200_dimenet_graph_count")
+        self.last_counts = {"edges": int(counts[0]), "triplets": int(counts[1])}
+        return gbuf, counts
+
+    def train_grads(self, z, pos, mol_ptr, n_mol: int, seed_energy: Optional[torch.Tensor], seed_forces: Optional[torch.Tensor]) -> torch.Tensor:
+        """d(sum_m seed_energy[m] E_m + sum_i seed_forces[i] . F_i)/d(flat weight buffer), in the buffer's layout (nb200_dimenet_train_grads).
+        Either seed may be None.  Builds the graph again (one synchronisation for the counts), so it does not depend on an earlier call."""
+        if self._w is None:
+            raise NablaB200Error("DimeNetRunner.train_grads before set_weights / bind")
+        lib, n, dev = self.lib, int(z.shape[0]), pos.device
+        gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
+        wbytes = lib.nb200_dimenet_train_workspace_bytes(byref(self._w), n_mol, n, counts)
+        if wbytes < 0:
+            check(int(wbytes), "nb200_dimenet_train_workspace_bytes")
+        ws = self._buffer("_ws", wbytes, dev)
+        buf = self._keep[0]
+        grads = torch.zeros_like(buf)  # the call writes up to the end of the last entry
+        seeds = [None if t is None else t.detach().to(device=dev, dtype=torch.float32).contiguous() for t in (seed_energy, seed_forces)]
+        if seeds[0] is not None and seeds[0].shape != (n_mol,):
+            raise NablaB200Error(f"seed_energy: expected shape ({n_mol},), got {tuple(seeds[0].shape)}")
+        if seeds[1] is not None and seeds[1].shape != (n, 3):
+            raise NablaB200Error(f"seed_forces: expected shape ({n}, 3), got {tuple(seeds[1].shape)}")
+        ptr = [0 if t is None else t.data_ptr() for t in seeds]
+        check(lib.nb200_dimenet_train_grads(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(),
+                                            gbuf.numel(), counts, ws.data_ptr(), ws.numel(), ptr[0] or None, ptr[1] or None, grads.data_ptr(),
+                                            self._stream()), "nb200_dimenet_train_grads")
+        return grads
+
+
+class DimeNetEnergyFn(torch.autograd.Function):
+    """(flat weights) -> (energy [B], forces [N,3]) through nb200_dimenet_energy_forces; backward = nb200_dimenet_train_grads with the
+    incoming gradients as seeds (the force term by forward-over-reverse, DESIGN.md 3.15.1).  Once differentiable; pos gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, flat, model, runner, offs, z, pos, mol_ptr, n_mol):
+        runner.bind(model, flat.detach(), offs)
+        energy, forces, _ = runner.run(z, pos, mol_ptr, n_mol)
+        ctx.runner, ctx.w, ctx.keep, ctx.n_mol = runner, runner._w, runner._keep, n_mol
+        ctx.save_for_backward(z, pos, mol_ptr)
+        return energy, forces
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_energy, g_forces):
+        z, pos, mol_ptr = ctx.saved_tensors
+        runner = ctx.runner
+        runner._w, runner._keep = ctx.w, ctx.keep
+        grads = runner.train_grads(z, pos, mol_ptr, ctx.n_mol, g_energy, g_forces)
+        return grads, None, None, None, None, None, None, None
