@@ -1,7 +1,7 @@
-"""Throughput of exact Hessians (nb200_painn_hvp, nb200_schnet_hvp) on the config-2 batch: 256 synthetic conformations (synth.py), one JSON
-line.
+"""Throughput of exact Hessians (nb200_painn_hvp, nb200_schnet_hvp, nb200_dimenet_hvp) on the config-2 batch: 256 synthetic conformations
+(synth.py), one JSON line.
 
-    python bench_hessian.py [--model painn|painn-oc|schnet] [--max-dir D] [--repeats R]
+    python bench_hessian.py [--model painn|painn-oc|schnet|dimenetplusplus] [--max-dir D] [--repeats R] [--batch B]
 
 Reports Hessians / s and HVP directions / s for the whole batch (3 n_max shared directions, chunks of --max-dir), peak device memory, ms per
 direction split into the tangent forward and the backward (CUDA events around the engine's launch categories), and the same Hessians by
@@ -9,6 +9,11 @@ batched central finite differences of the inference engine (nb200_painn_energy_f
 direction, step 1e-3 A) with their deviation from the analytic ones.  For SchNet the per-direction split is also given per launch category
 (marginal ms per direction of each, from the engine's CUDA-event timing of an n_dir call minus a one-direction call).  Card name and power
 limit come from the same run.  Writes nothing into the tree.
+
+--model dimenetplusplus (config/model/dimenetplusplus.yaml sizes, the tests' weights, synth_batch(0, B) as bench_dimenet.py): one analytic
+pass over the 3 n_max shared directions (its cost per direction is about that of a training gradient call, so it is not repeated), the
+per-direction and once-per-call costs from one- and --probe-direction calls, and the same Hessians by central differences with two
+nb200_dimenet_energy_forces calls per direction.
 """
 import argparse
 import ctypes
@@ -33,11 +38,15 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="painn", choices=["painn", "painn-oc", "schnet"])
+    ap.add_argument("--model", default="painn", choices=["painn", "painn-oc", "schnet", "dimenetplusplus"])
     ap.add_argument("--max-dir", type=int, default=None)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--fd-step", type=float, default=1e-3)
+    ap.add_argument("--batch", type=int, default=256, help="molecules (dimenetplusplus only; the other models use the config-2 batch)")
+    ap.add_argument("--probe-directions", type=int, default=8, help="directions of the call the per-direction cost is taken from (dimenetplusplus)")
     args = ap.parse_args()
+    if args.model == "dimenetplusplus":
+        return dimenet_main(args)
 
     import torch
 
@@ -144,6 +153,103 @@ def main():
         rec["ms_per_direction_by_category"] = split
         rec["edges"] = edges
     print(json.dumps(rec))
+
+
+def dimenet_main(args):
+    import os
+    import sys
+
+    import torch
+    import yaml
+
+    root = os.path.dirname(os.path.abspath(__file__))
+    sys.path.insert(0, os.path.join(root, "tests", "golden"))
+    from make_golden_dimenet import load_test_weights
+
+    from nabladft_b200 import vibrations as vib
+    from nabladft_b200.dimenetplusplus import DimeNetPlusPlusPotential
+    from nabladft_b200.synth import synth_batch
+    from oracle.dimenet import DimeNetPlusPlusPotentialOracle
+
+    dev = torch.device("cuda:0")
+    cfg = yaml.safe_load(open(os.path.join(root, "config", "model", "dimenetplusplus-b200.yaml")))["net"]
+    cfg.pop("_target_")
+    ora = load_test_weights(DimeNetPlusPlusPotentialOracle(**cfg).double().eval())
+    model = DimeNetPlusPlusPotential(**cfg).eval()
+    model.load_state_dict({k: v.float() for k, v in ora.state_dict().items()}, strict=True)
+    model = model.to(dev)
+
+    class D:
+        pass
+
+    b = synth_batch(0, args.batch)
+    batch = D()
+    batch.z = torch.from_numpy(b["z"]).long().to(dev)
+    batch.pos = torch.from_numpy(b["pos"]).to(dev)
+    batch.batch = torch.from_numpy(b["batch"]).to(dev)
+    runner, zi, posf, mol_ptr, n_mol = vib._engine_inputs(model, batch)
+    ptr = mol_ptr.cpu().tolist()
+    n_max = max(q - p for p, q in zip(ptr[:-1], ptr[1:]))
+    n_dir = 3 * n_max
+    v = vib.shared_directions(ptr, 0, n_dir, dev)
+    k = max(2, min(args.probe_directions, n_dir))
+
+    def timed(vv):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        runner.run_hvp(zi, posf, mol_ptr, n_mol, vv, with_forces=False)
+        torch.cuda.synchronize()
+        return time.perf_counter() - t0
+
+    timed(v[:1])  # workspace allocation
+    torch.cuda.reset_peak_memory_stats(dev)
+    t1 = timed(v[:1])
+    tk = timed(v[:k])
+    per_dir = (tk - t1) / (k - 1)
+    # analytic Hessians of the whole batch, once
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    hs = vib.hessians(model, batch, args.max_dir)
+    torch.cuda.synchronize()
+    t_an = time.perf_counter() - t0
+    peak = torch.cuda.max_memory_allocated(dev)
+    counts = dict(runner.last_counts)
+    ws = runner.lib.nb200_dimenet_hvp_workspace_bytes(ctypes.byref(runner._w), n_mol, zi.numel(),
+                                                      (ctypes.c_int64 * 4)(counts["edges"], counts["triplets"], 0, 0))
+
+    # finite differences: two energy-and-forces calls per shared direction
+    h = args.fd_step
+    runner.run(zi, posf, mol_ptr, n_mol)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    cols = []
+    for d in range(n_dir):
+        dv = v[d] * h
+        fp = runner.run(zi, (posf + dv).contiguous(), mol_ptr, n_mol)[1]
+        fm = runner.run(zi, (posf - dv).contiguous(), mol_ptr, n_mol)[1]
+        cols.append(-(fp - fm) / (2 * h))
+    torch.cuda.synchronize()
+    t_fd = time.perf_counter() - t0
+    hv_fd = torch.stack(cols)
+    fd = vib.hessians_from_hvp(lambda vv: hv_fd[:vv.shape[0]], ptr)
+    devs = [float((a - c).abs().max() / a.abs().max()) for a, c in zip(hs, fd)]
+    # a molecule of more than max_neighbors + 1 atoms can have truncated candidate lists (radius_graph keeps the first K + 1 in index
+    # order); a step that moves a pair across the cutoff then changes the edge set and the forces jump, so only the others are smooth
+    kcap = model.max_num_neighbors + 1
+    smooth = [d for d, p0, p1 in zip(devs, ptr[:-1], ptr[1:]) if p1 - p0 <= kcap]
+
+    name, limit = card()
+    print(json.dumps({
+        "metric": "dimenet_hessians", "model": args.model, "batch": n_mol, "atoms": int(zi.numel()), "edges": counts["edges"],
+        "triplets": counts["triplets"], "n_max": n_max, "directions": n_dir,
+        "hessians_per_s": n_mol / t_an, "directions_per_s": n_dir / t_an, "ms_per_batch": 1e3 * t_an, "ms_per_direction": 1e3 * t_an / n_dir,
+        "ms_once_per_call": 1e3 * (t1 - per_dir), "ms_per_direction_marginal": 1e3 * per_dir, "probe_directions": k,
+        "peak_mem_gb": peak / 1e9, "hvp_workspace_gb": ws / 1e9,
+        "fd_ms_per_batch": 1e3 * t_fd, "fd_ms_per_direction": 1e3 * t_fd / n_dir, "fd_hessians_per_s": n_mol / t_fd, "fd_step_A": h,
+        "fd_max_rel_dev": max(devs), "fd_median_rel_dev": float(np.median(devs)),
+        "fd_max_rel_dev_untruncated": max(smooth) if smooth else None, "untruncated_molecules": len(smooth), "analytic_speedup_vs_fd": t_fd / t_an, "max_asymmetry": hs.max_asymmetry,
+        "card": name, "power_limit": limit,
+    }))
 
 
 if __name__ == "__main__":

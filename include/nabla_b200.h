@@ -552,7 +552,7 @@ int nb200_gemnet_oc_debug_h(const void* workspace, const nb200_gemnet_oc_weights
  * energy[m] = scale * y_m + mean, forces = -dy/dpos of the UNSCALED prediction y (dimenetplusplus.py:97-112); scale = 1, mean = 0
  * without postprocessing.  nb200_dimenet_energy_forces runs a reverse pass through output blocks, interaction blocks, the triplet
  * aggregation and the bases; its sums are gathers (no atomics), so two calls on the same input are bitwise equal (DESIGN.md 3.15).
- * nb200_dimenet_train_grads gives the parameter gradients of an energy and force loss.
+ * nb200_dimenet_train_grads gives the parameter gradients of an energy and force loss, nb200_dimenet_hvp Hessian-vector products.
  * Supported: hidden 256, int_emb 64, basis_emb 8, out_emb 256, num_spherical 7, num_radial 6, before / after skip 1 / 2, 3 output
  * layers, envelope exponent 5, 1 <= num_blocks <= 16, 2 <= node_latent_dim (= out_channels) <= 64, 1 <= max_neighbors <= 64;
  * anything else is NB200_EUNSUPPORTED.
@@ -632,6 +632,21 @@ int nb200_dimenet_train_grads(nb200_engine* eng, const nb200_dimenet_weights* w,
 /* Test entry point, not a supported API: the spherical radial basis env(x) N_ln j_l(z_ln x), x = dist / cutoff, and its derivative
  * with respect to dist, [n, 42] each, as the engine evaluates them in fp32. */
 int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, const float* dist, int32_t n, float* rbs, float* drbs, void* stream);
+/* Hessian-vector products (csrc/dimenet_hvp.inc, DESIGN.md 3.15.2): for each of n_dir position-space directions v[d] ([n_atoms,3], Angstrom)
+ *   hv[d] = -(dF/dR) v[d] = (d^2 y / dR dR) v[d]   in Ha/A, y the UNSCALED prediction (the forces' y; the scaler touches the energy only),
+ * exact (forward-over-reverse, no finite step), fp32.  Same z, pos, mol_ptr, graph buffer and counts as phase 1.  energy[n_mol] (scaled)
+ * and forces[n_atoms,3] (NULL => not written) are bitwise those of nb200_dimenet_energy_forces.  The primal pass runs once per call, the
+ * directions one after another, so the workspace does not depend on n_dir.  No atomics: bitwise repeatable and independent of how the
+ * directions are split into calls.  NB200_EINVAL (nothing launched) for a NULL required pointer, n_dir < 1, counts above the graph capacity,
+ * or a short graph buffer or workspace; NB200_EUNSUPPORTED for a configuration outside the list above. */
+int64_t nb200_dimenet_hvp_workspace_bytes(const nb200_dimenet_weights* w, int32_t n_mol, int32_t n_atoms, const int64_t* counts_host);
+int nb200_dimenet_hvp(nb200_engine* eng, const nb200_dimenet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
+                      int32_t n_mol, int32_t n_atoms, void* graph_buf, int64_t graph_bytes, const int64_t* counts_host,
+                      void* workspace, int64_t workspace_bytes, int32_t n_dir, const float* v, float* energy, float* forces,
+                      float* hv, void* stream);
+/* Test entry point, not a supported API: the second distance derivatives of the radial bases, d2rbs [n, 42] of env(x) N_ln j_l(z_ln x) and
+ * d2rbf [n, 6] of env(x) sin(freq_n x), x = dist / cutoff, as the Hessian-vector pass evaluates them in fp32. */
+int nb200_dimenet_debug_sbf_radial_d2(const nb200_dimenet_weights* w, const float* dist, int32_t n, float* d2rbs, float* d2rbf, void* stream);
 
 /* ----------------------------------------------------------------------------------------
  * PhiSNet Clebsch-Gordan mixing layers (SURVEY.md section 8 f4).  Features are component-major:

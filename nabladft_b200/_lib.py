@@ -186,6 +186,10 @@ SIGNATURES = {
     "nb200_dimenet_train_grads": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
                                             POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_dimenet_debug_sbf_radial": (c_int32, [POINTER(DimeNetWeights), c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
+    "nb200_dimenet_hvp_workspace_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32, c_int32, POINTER(c_int64)]),
+    "nb200_dimenet_hvp": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
+                                    POINTER(c_int64), c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_dimenet_debug_sbf_radial_d2": (c_int32, [POINTER(DimeNetWeights), c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

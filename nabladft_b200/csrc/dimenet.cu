@@ -709,6 +709,64 @@ bool sizes_ok(int32_t n_mol, int32_t n_atoms, int32_t max_neighbors) {
     return n_mol >= 1 && n_atoms >= 1 && (int64_t)n_atoms * (max_neighbors + 1) < 0x7fffffff;
 }
 
+// the energy-and-forces pass on a carved graph and workspace (arguments checked by the caller).  forces == nullptr: GeomBwdK and ForceK do not
+// run; grbf, grbs and gct are left holding dy/drbf, dy/drbs and dy/dcos either way
+int energy_forces_pass(const Ctx& c, const Work& wk, const Geo& q, const int32_t* z, const float* pos, const int32_t* mol_ptr, int32_t n_mol,
+                       int64_t T, float* energy, float* forces, float* graph_emb) {
+    nb200_engine* eng = c.e;
+    cudaStream_t s = c.s;
+    const nb200_dimenet_weights* w = c.w;
+    const GraphBuf& g = *q.g;
+    const int64_t E = q.E, n_atoms = q.n;
+    const int nb = w->num_blocks, L = w->node_latent_dim;
+    const int64_t EH = E * H;
+    const float inv_cut = 1.0f / w->cutoff;
+    // geometry and bases
+    NB_TRY(pfor(eng, s, CAT_FILTER, E, GeomK{pos, g.src, g.tgt, wk.V, wk.d}));
+    NB_TRY(pfor(eng, s, CAT_FILTER, E * NRAD, RbfK{wk.d, c.G(NB200_DPP_G_FREQ), inv_cut, wk.rbf}));
+    NB_TRY(pfor(eng, s, CAT_FILTER, E * NSR, RbsK{wk.d, c.G(NB200_DPP_G_ZEROS), c.G(NB200_DPP_G_NORMS), inv_cut, wk.rbs, wk.drbs}));
+    // embedding block
+    NB_TRY(pfor(eng, s, CAT_EMBED, EH, EmbRbfK{wk.rbf, c.G(NB200_DPP_G_EMB_RBF_W), c.G(NB200_DPP_G_EMB_RBF_B), wk.hr, wk.hra}));
+    NB_TRY(c.gemm(E, H, H, wk.hra, c.G(NB200_DPP_G_EMB_W3), 0, wk.epre, 0, nullptr, nullptr));
+    NB_TRY(pfor(eng, s, CAT_EMBED, EH, EmbAddK{z, g.src, g.tgt, c.G(NB200_DPP_G_EMB_TI), c.G(NB200_DPP_G_EMB_TJ), wk.epre, wk.X}));
+    // blocks
+    NB_TRY(output_fwd(c, wk, q, 0, wk.X));
+    for (int b = 0; b < nb; b++) {
+        NB_TRY(interaction_fwd(c, wk, q, b, wk.X + b * EH, wk.X + (b + 1) * EH));
+        NB_TRY(output_fwd(c, wk, q, b + 1, wk.X + (b + 1) * EH));
+    }
+    // regression head: energy and dy/d(graph embedding)
+    NB_TRY(pfor(eng, s, CAT_READOUT, n_mol, HeadK{mol_ptr, wk.P, L, c.G(NB200_DPP_G_HEAD_W0), c.G(NB200_DPP_G_HEAD_B0), c.G(NB200_DPP_G_HEAD_W1),
+                                                  c.G(NB200_DPP_G_HEAD_B1), c.G(NB200_DPP_G_HEAD_W2), c.G(NB200_DPP_G_HEAD_B2), c.G(NB200_DPP_G_HEAD_W3),
+                                                  c.G(NB200_DPP_G_HEAD_B3), w->scale, w->mean, graph_emb, wk.gG, energy}));
+    // reverse pass
+    NB_TRY(pfor(eng, s, CAT_READOUT, n_atoms * L, BcastK{g.mol_id, wk.gG, L, wk.gP}));
+    if (E > 0) {
+        NB_TRY(goc_memset(wk.grbf, 0, (size_t)E * NRAD * sizeof(float), s));
+        NB_TRY(goc_memset(wk.grbs, 0, (size_t)E * NSR * sizeof(float), s));
+        if (T > 0) NB_TRY(goc_memset(wk.gct, 0, (size_t)T * sizeof(float), s));
+    }
+    float* gx = wk.gX;
+    float* gprev = wk.gI;
+    NB_TRY(output_bwd(c, wk, q, nb, wk.X + nb * EH, gx, 0));
+    for (int b = nb - 1; b >= 0; b--) {
+        if (b != nb - 1) NB_TRY(interaction_fwd(c, wk, q, b, wk.X + b * EH, wk.out));  // the scratch holds block nb - 1 after the forward
+        NB_TRY(interaction_bwd(c, wk, q, b, gx, gprev));
+        NB_TRY(output_bwd(c, wk, q, b, wk.X + b * EH, gprev, 1));
+        float* t = gx; gx = gprev; gprev = t;
+    }
+    // embedding block reverse: gx = d/dx0
+    NB_TRY(pfor(eng, s, CAT_EMBED, EH, DActMulK{gx, wk.epre, wk.g1}));
+    NB_TRY(c.gemm(E, H, H, wk.g1, c.G(NB200_DPP_G_EMB_W3), 1, wk.g2, 0, nullptr, nullptr));
+    NB_TRY(pfor(eng, s, CAT_EMBED, EH, DActMulK{wk.g2, wk.hr, wk.g2}));
+    NB_TRY(pfor(eng, s, CAT_FILTER, E * NRAD, RbfBwdK{nullptr, wk.g2, nullptr, c.G(NB200_DPP_G_EMB_RBF_W), wk.grbf}));
+    if (!forces) return NB200_OK;
+    // geometry reverse and forces
+    NB_TRY(pfor(eng, s, CAT_FORCE, E, GeomBwdK{g.ptr, g.src, g.tgt, g.rev, g.optr, g.oeid, g.tptr, wk.V, wk.d, wk.rbf, c.G(NB200_DPP_G_FREQ), inv_cut,
+                                               wk.grbf, wk.drbs, wk.grbs, wk.gct, wk.gV}));
+    return pfor(eng, s, CAT_FORCE, 3 * n_atoms, ForceK{g.ptr, g.optr, g.oeid, wk.gV, forces});
+}
+
 }  // namespace
 
 extern "C" int64_t nb200_dimenet_graph_bytes(const nb200_dimenet_weights* w, int32_t n_atoms) {
@@ -760,54 +818,8 @@ extern "C" int nb200_dimenet_energy_forces(nb200_engine* eng, const nb200_dimene
     const GraphBuf g = carve_graph(graph_buf, n_atoms, kcap);
     const Work wk = carve_work(workspace, w->num_blocks, n_mol, n_atoms, E, T, w->node_latent_dim);
     const Ctx c{eng, (cudaStream_t)stream, w};
-    cudaStream_t s = c.s;
     const Geo q{&g, n_atoms, E};
-    const int nb = w->num_blocks, L = w->node_latent_dim;
-    const int64_t EH = E * H;
-    const float inv_cut = 1.0f / w->cutoff;
-    // geometry and bases
-    NB_TRY(pfor(eng, s, CAT_FILTER, E, GeomK{pos, g.src, g.tgt, wk.V, wk.d}));
-    NB_TRY(pfor(eng, s, CAT_FILTER, E * NRAD, RbfK{wk.d, c.G(NB200_DPP_G_FREQ), inv_cut, wk.rbf}));
-    NB_TRY(pfor(eng, s, CAT_FILTER, E * NSR, RbsK{wk.d, c.G(NB200_DPP_G_ZEROS), c.G(NB200_DPP_G_NORMS), inv_cut, wk.rbs, wk.drbs}));
-    // embedding block
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, EmbRbfK{wk.rbf, c.G(NB200_DPP_G_EMB_RBF_W), c.G(NB200_DPP_G_EMB_RBF_B), wk.hr, wk.hra}));
-    NB_TRY(c.gemm(E, H, H, wk.hra, c.G(NB200_DPP_G_EMB_W3), 0, wk.epre, 0, nullptr, nullptr));
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, EmbAddK{z, g.src, g.tgt, c.G(NB200_DPP_G_EMB_TI), c.G(NB200_DPP_G_EMB_TJ), wk.epre, wk.X}));
-    // blocks
-    NB_TRY(output_fwd(c, wk, q, 0, wk.X));
-    for (int b = 0; b < nb; b++) {
-        NB_TRY(interaction_fwd(c, wk, q, b, wk.X + b * EH, wk.X + (b + 1) * EH));
-        NB_TRY(output_fwd(c, wk, q, b + 1, wk.X + (b + 1) * EH));
-    }
-    // regression head: energy and dy/d(graph embedding)
-    NB_TRY(pfor(eng, s, CAT_READOUT, n_mol, HeadK{mol_ptr, wk.P, L, c.G(NB200_DPP_G_HEAD_W0), c.G(NB200_DPP_G_HEAD_B0), c.G(NB200_DPP_G_HEAD_W1),
-                                                  c.G(NB200_DPP_G_HEAD_B1), c.G(NB200_DPP_G_HEAD_W2), c.G(NB200_DPP_G_HEAD_B2), c.G(NB200_DPP_G_HEAD_W3),
-                                                  c.G(NB200_DPP_G_HEAD_B3), w->scale, w->mean, graph_emb, wk.gG, energy}));
-    // reverse pass
-    NB_TRY(pfor(eng, s, CAT_READOUT, (int64_t)n_atoms * L, BcastK{g.mol_id, wk.gG, L, wk.gP}));
-    if (E > 0) {
-        NB_TRY(goc_memset(wk.grbf, 0, (size_t)E * NRAD * sizeof(float), s));
-        NB_TRY(goc_memset(wk.grbs, 0, (size_t)E * NSR * sizeof(float), s));
-        if (T > 0) NB_TRY(goc_memset(wk.gct, 0, (size_t)T * sizeof(float), s));
-    }
-    float* gx = wk.gX;
-    float* gprev = wk.gI;
-    NB_TRY(output_bwd(c, wk, q, nb, wk.X + nb * EH, gx, 0));
-    for (int b = nb - 1; b >= 0; b--) {
-        if (b != nb - 1) NB_TRY(interaction_fwd(c, wk, q, b, wk.X + b * EH, wk.out));  // the scratch holds block nb - 1 after the forward
-        NB_TRY(interaction_bwd(c, wk, q, b, gx, gprev));
-        NB_TRY(output_bwd(c, wk, q, b, wk.X + b * EH, gprev, 1));
-        float* t = gx; gx = gprev; gprev = t;
-    }
-    // embedding block reverse: gx = d/dx0
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, DActMulK{gx, wk.epre, wk.g1}));
-    NB_TRY(c.gemm(E, H, H, wk.g1, c.G(NB200_DPP_G_EMB_W3), 1, wk.g2, 0, nullptr, nullptr));
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, DActMulK{wk.g2, wk.hr, wk.g2}));
-    NB_TRY(pfor(eng, s, CAT_FILTER, E * NRAD, RbfBwdK{nullptr, wk.g2, nullptr, c.G(NB200_DPP_G_EMB_RBF_W), wk.grbf}));
-    // geometry reverse and forces
-    NB_TRY(pfor(eng, s, CAT_FORCE, E, GeomBwdK{g.ptr, g.src, g.tgt, g.rev, g.optr, g.oeid, g.tptr, wk.V, wk.d, wk.rbf, c.G(NB200_DPP_G_FREQ), inv_cut,
-                                               wk.grbf, wk.drbs, wk.grbs, wk.gct, wk.gV}));
-    return pfor(eng, s, CAT_FORCE, 3 * (int64_t)n_atoms, ForceK{g.ptr, g.optr, g.oeid, wk.gV, forces});
+    return energy_forces_pass(c, wk, q, z, pos, mol_ptr, n_mol, T, energy, forces, graph_emb);
 }
 
 extern "C" int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, const float* dist, int32_t n, float* rbs, float* drbs, void* stream) {
@@ -823,3 +835,4 @@ extern "C" int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, co
 }
 
 #include "dimenet_train.inc"
+#include "dimenet_hvp.inc"

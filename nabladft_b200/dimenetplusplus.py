@@ -11,7 +11,8 @@ per-element tables).
 
 Training: in training mode with autograd the forward goes through `DimeNetEnergyFn`, whose backward is `nb200_dimenet_train_grads` (the
 parameter gradients of energy and force losses, the force term by forward-over-reverse, DESIGN.md 3.15.1); the export is then differentiable,
-so autograd carries the flat-buffer gradient back to every reference-named parameter.  Supported: the shipped sizes, with
+so autograd carries the flat-buffer gradient back to every reference-named parameter.  Hessians: `DimeNetRunner.run_hvp` (nb200_dimenet_hvp,
+DESIGN.md 3.15.2) gives exact Hessian-vector products of the unscaled prediction; `vibrations.hessians` / `normal_modes` take this model.  Supported: the shipped sizes, with
 1 <= dimenet_num_blocks <= 16, 2 <= node_latent_dim <= 64 and dimenet_max_num_neighbors <= 64; anything else raises at construction.  No CPU
 fallback: CPU tensors raise NablaB200Error in eval mode and NotImplementedError in training mode.
 """
@@ -351,6 +352,31 @@ class DimeNetRunner:
                                             gbuf.numel(), counts, ws.data_ptr(), ws.numel(), ptr[0] or None, ptr[1] or None, grads.data_ptr(),
                                             self._stream()), "nb200_dimenet_train_grads")
         return grads
+
+    def run_hvp(self, z, pos, mol_ptr, n_mol: int, v, with_forces: bool = True):
+        """Exact Hessian-vector products (nb200_dimenet_hvp): v [n_dir, N, 3] (or [N, 3]) fp32 in Angstrom.  Returns (energy [B], forces [N, 3]
+        or None, hv [n_dir, N, 3]) with hv = -(dF/dR) v in Ha/A -- the Hessian of the unscaled prediction, whose gradient the forces are --
+        and energy / forces bitwise those of `run`.  Builds the graph (one synchronisation for the counts), then one call."""
+        if self._w is None:
+            raise NablaB200Error("DimeNetRunner.run_hvp before set_weights / bind")
+        lib, n, dev = self.lib, int(z.shape[0]), pos.device
+        if v.dim() == 2:
+            v = v.unsqueeze(0)
+        if not (v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n, 3) and v.shape[0] >= 1 and v.device == dev):
+            raise NablaB200Error(f"run_hvp(): v must be a contiguous fp32 tensor [n_dir, {n}, 3] with n_dir >= 1 on {dev}")
+        n_dir = int(v.shape[0])
+        gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
+        wbytes = lib.nb200_dimenet_hvp_workspace_bytes(byref(self._w), n_mol, n, counts)
+        if wbytes < 0:
+            check(int(wbytes), "nb200_dimenet_hvp_workspace_bytes")
+        ws = self._buffer("_ws", wbytes, dev)
+        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+        forces = torch.empty(n, 3, dtype=torch.float32, device=dev) if with_forces else None
+        hv = torch.empty(n_dir, n, 3, dtype=torch.float32, device=dev)
+        check(lib.nb200_dimenet_hvp(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(), gbuf.numel(),
+                                    counts, ws.data_ptr(), ws.numel(), n_dir, v.data_ptr(), energy.data_ptr(),
+                                    None if forces is None else forces.data_ptr(), hv.data_ptr(), self._stream()), "nb200_dimenet_hvp")
+        return energy, forces, hv
 
 
 class DimeNetEnergyFn(torch.autograd.Function):

@@ -1,8 +1,9 @@
-"""Analytic Hessians and normal modes of the PaiNN and SchNet models on the GPU.
+"""Analytic Hessians and normal modes of the PaiNN, SchNet and DimeNet++ models on the GPU.
 
 The reference's `PYGAseInterface.compute_normal_modes` (nablaDFT/optimization/pyg_ase_interface.py) runs ASE `Vibrations`: central finite
 differences of the forces, one molecule at a time, 6N + 1 force calls per molecule with a 0.01 A step.  Here the engine computes exact
-Hessian-vector products H v = -(dF/dR) v (`PainnEngine.run_hvp`; DESIGN.md section 3.13 for PaiNN, 3.13.1 for SchNet), and since
+Hessian-vector products H v = -(dF/dR) v (`PainnEngine.run_hvp`, `DimeNetRunner.run_hvp`; DESIGN.md section 3.13 for PaiNN, 3.13.1 for
+SchNet, 3.15.2 for DimeNet++), and since
 molecules do not interact, ONE direction displaces atom k of every molecule of the batch at once: the Hessians of a whole batch take
 3 * n_max directions, n_max = the atom count of the largest molecule.
 
@@ -10,8 +11,9 @@ molecules do not interact, ONE direction displaces atom k of every molecule of t
     hessians(model, batch, max_dir=None)    -> per-molecule [3n, 3n] Hessians, Ha/A^2
     normal_modes(model, batch, masses=None) -> per-molecule eigenvalues, modes, wavenumbers (cm^-1) and ASE-style energies (meV)
 
-`model` is `spk.NeuralNetworkPotential` (PaiNN or SchNet representation; `batch` = its inputs dict) or `painn_oc.PaiNN` (`batch` has
-.z, .pos, .batch and optionally .ptr).  Everything runs in fp32 on the device except the diagonalisation (float64, `torch.linalg.eigh`).
+`model` is `spk.NeuralNetworkPotential` (PaiNN or SchNet representation; `batch` = its inputs dict), `painn_oc.PaiNN` (`batch` has
+.z, .pos, .batch and optionally .ptr) or `dimenetplusplus.DimeNetPlusPlusPotential` (`batch` has .z, .pos and a sorted .batch).  H is the
+Hessian of the energy the forces are the gradient of: for DimeNet++ that is the unscaled prediction (the scaler touches the energy only).  Everything runs in fp32 on the device except the diagonalisation (float64, `torch.linalg.eigh`).
 """
 import math
 from dataclasses import dataclass
@@ -41,8 +43,8 @@ MEV_PER_CM1 = 1e3 * PLANCK_JS * C_CM_PER_S / EV_J  # h c in meV cm
 
 # ---------------------------------------------------------------------------------------------------------------- model plumbing
 def _engine_inputs(model, batch):
-    """(engine, z int32, pos fp32, mol_ptr int32, n_mol) for either mirror, with the errors the mirrors raise."""
-    from . import painn_oc, spk
+    """(engine, z int32, pos fp32, mol_ptr int32, n_mol) for each mirror, with the errors the mirrors raise."""
+    from . import dimenetplusplus, painn_oc, spk
 
     if isinstance(model, spk.NeuralNetworkPotential):
         eng, z, pos, mol_ptr, n_mol = model._prepare(batch)  # raises on CPU inputs and periodic systems
@@ -61,7 +63,17 @@ def _engine_inputs(model, batch):
         else:
             mol_ptr, n_mol = mol_ptr_from_batch(batch.batch, getattr(batch, "num_graphs", None))
         return model.engine(), z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr.contiguous(), n_mol
-    raise NotImplementedError(f"Hessians need nabladft_b200.spk.NeuralNetworkPotential or nabladft_b200.painn_oc.PaiNN, not {type(model).__name__}")
+    if isinstance(model, dimenetplusplus.DimeNetPlusPlusPotential):
+        if not batch.pos.is_cuda:
+            raise NablaB200Error("DimeNetPlusPlusPotential runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
+        if model.training and torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters()):
+            raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
+        runner = model._get_runner()
+        model._sync_weights(runner, batch.pos.device)
+        z, pos, mol_ptr, n_mol = model.batch_args(batch.z, batch.pos, batch.batch)
+        return runner, z, pos, mol_ptr, n_mol
+    raise NotImplementedError("Hessians need nabladft_b200.spk.NeuralNetworkPotential, nabladft_b200.painn_oc.PaiNN or "
+                              f"nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential, not {type(model).__name__}")
 
 
 def hessian_vector_product(model, batch, v: torch.Tensor):
@@ -129,7 +141,8 @@ def hessians_from_hvp(hvp: Callable[[torch.Tensor], torch.Tensor], mol_ptr: Sequ
 
 
 def hessians(model, batch, max_dir: Optional[int] = None) -> Hessians:
-    """Exact per-molecule Hessians of the energy, [3n_m, 3n_m] in Ha/A^2 (symmetrised; see `Hessians`).  `max_dir` bounds the directions per
+    """Exact per-molecule Hessians of the energy whose gradient the forces are (for DimeNet++ the unscaled prediction), [3n_m, 3n_m] in
+    Ha/A^2 (symmetrised; see `Hessians`).  `max_dir` bounds the directions per
     engine call, hence the v and hv buffers (n_dir x N x 3 floats each); the engine workspace does not depend on it, and every call re-runs
     the primal forward once."""
     eng, z, pos, mol_ptr, n_mol = _engine_inputs(model, batch)
