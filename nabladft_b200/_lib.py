@@ -6,7 +6,9 @@ There is NO fallback: if the shared library is missing or a call fails, we raise
 """
 import ctypes
 import os
-from ctypes import c_double, POINTER, c_float, c_int32, c_int64, c_uint64, c_void_p
+from ctypes import c_double, POINTER, byref, c_float, c_int32, c_int64, c_uint64, c_void_p
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libnabla_b200.so")
@@ -199,6 +201,17 @@ class NablaB200Error(RuntimeError):
     pass
 
 
+def bind(lib, prefixes=None):
+    """Attach the prototypes of SIGNATURES to `lib`: all of them, or those of the symbols whose names start with one of `prefixes` plus the
+    engine handle's create / destroy (an emulation build of one engine exports only its own).  A declared symbol that `lib` does not export
+    raises AttributeError."""
+    for name, (res, args) in SIGNATURES.items():
+        if prefixes is None or name.startswith(tuple(prefixes)) or name in ("nb200_engine_create", "nb200_engine_destroy"):
+            fn = getattr(lib, name)
+            fn.restype, fn.argtypes = res, args
+    return lib
+
+
 def load():
     """Load libnabla_b200.so (once). Raises if it has not been built -- never falls back."""
     global _lib
@@ -209,12 +222,8 @@ def load():
             f"{LIB_PATH} is missing: build it with `python -m nabladft_b200.build` "
             "(nvcc, sm_90a). There is no CPU / eager fallback for this path."
         )
-    lib = ctypes.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
-        fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
-        fn.restype, fn.argtypes = res, args
-    _lib = lib
-    return lib
+    _lib = bind(ctypes.CDLL(LIB_PATH))
+    return _lib
 
 
 def check(rc: int, what: str):
@@ -233,6 +242,56 @@ def ptr(t):
 
 
 def current_stream():
-    import torch
-
     return c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+class EngineDriver:
+    """Host side of one `nb200_engine` handle, shared by the model drivers: the handle's lifecycle, the stream and device checks of their
+    calls (`_stream`, `_on_device`: what the emulation tests replace), size queries and the growth of the buffers they size."""
+
+    _ws = None  # the workspace every driver has (`_buffer("_ws", ...)` sizes it)
+    SLACK = 1.25  # a grown buffer holds this many times the bytes asked for (+ 256): headroom for the next, slightly larger batch
+
+    def __init__(self, lib=None):
+        """`lib`: a bound library exporting the C ABI (default: libnabla_b200.so)."""
+        self.lib = load() if lib is None else lib
+        h = c_void_p()
+        check(self.lib.nb200_engine_create(byref(h)), "nb200_engine_create")
+        self._h = h
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                self.lib.nb200_engine_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def _stream(self):
+        return current_stream()
+
+    def _on_device(self, t) -> bool:
+        return t.is_cuda
+
+    def _bytes(self, fn_name: str, *args) -> int:
+        """A size query of the C ABI; a negative return is its error code."""
+        n = getattr(self.lib, fn_name)(*args)
+        if n < 0:
+            check(int(n), fn_name)
+        return int(n)
+
+    def _buffer(self, attr: str, nbytes: int, device):
+        """The byte buffer `self.<attr>`, replaced by a larger one (the old one freed first) when it holds fewer than `nbytes` or sits on
+        another device."""
+        cur = getattr(self, attr, None)
+        if cur is None or cur.numel() < nbytes or cur.device != device:
+            setattr(self, attr, None)
+            cur = torch.empty(int(nbytes * self.SLACK) + 256, dtype=torch.uint8, device=device)
+            setattr(self, attr, cur)
+        return cur
+
+    def _check_seeds(self, seed, force_seed, n_mol: int, n_atoms: int, device) -> None:
+        """The loss seeds of a gradient call, dLoss/dE [n_mol] and dLoss/dF [n_atoms, 3]; either may be None."""
+        for t, n in ((seed, n_mol), (force_seed, 3 * n_atoms)):
+            if t is not None and not (t.device == device and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == n):
+                raise NablaB200Error("seeds must be contiguous fp32 tensors [n_mol] / [n_atoms, 3] on the batch's device")

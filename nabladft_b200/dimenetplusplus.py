@@ -17,15 +17,15 @@ DESIGN.md 3.15.2) gives exact Hessian-vector products of the unscaled prediction
 fallback: CPU tensors raise NablaB200Error in eval mode and NotImplementedError in training mode.
 """
 import ctypes
-from ctypes import POINTER, byref, c_int64, c_void_p
+from ctypes import POINTER, byref, c_int64
 from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
 from torch import nn
 
-from ._lib import SIGNATURES as _ALL_SIGNATURES
-from ._lib import DimeNetWeights, NablaB200Error, check
+from . import _lib
+from ._lib import DimeNetWeights, EngineDriver, NablaB200Error, check
 
 # ---- canonical layout: keep in step with the enums of include/nabla_b200.h -----------------------------------------------------------------
 G_NAMES = ["FREQ", "ZEROS", "NORMS", "EMB_TI", "EMB_TJ", "EMB_RBF_W", "EMB_RBF_B", "EMB_W3", "HEAD_W0", "HEAD_B0", "HEAD_W1", "HEAD_B1",
@@ -37,15 +37,10 @@ _FIXED = dict(dimenet_hidden_channels=256, dimenet_int_emb_size=64, dimenet_basi
               dimenet_num_spherical=7, dimenet_num_radial=6, dimenet_envelope_exponent=5, dimenet_num_before_skip=1, dimenet_num_after_skip=2,
               dimenet_num_output_layers=3)
 
-SIGNATURES = {k: v for k, v in _ALL_SIGNATURES.items() if k.startswith("nb200_dimenet_")}
-
 
 def bind(lib):
-    """Attach the DimeNet++ prototypes to a loaded library (libnabla_b200.so is bound by _lib.load(); this is for tests/emu)."""
-    for name, (res, args) in SIGNATURES.items():
-        fn = getattr(lib, name)
-        fn.restype, fn.argtypes = res, args
-    return lib
+    """The DimeNet++ prototypes on `lib`, e.g. an emulation build of csrc/dimenet.cu, which exports no other engine."""
+    return _lib.bind(lib, ["nb200_dimenet_"])
 
 
 def sbf_radial_constants(num_spherical: int = 7, num_radial: int = 6) -> Tuple[np.ndarray, np.ndarray]:
@@ -231,9 +226,7 @@ class DimeNetPlusPlusPotential(nn.Module):
 
     def _get_runner(self) -> "DimeNetRunner":
         if self._runner is None:
-            from . import _lib
-
-            self._runner = DimeNetRunner(bind(_lib.load()))
+            self._runner = DimeNetRunner()
         return self._runner
 
     def _sync_weights(self, runner: "DimeNetRunner", device) -> None:
@@ -253,29 +246,14 @@ class DimeNetPlusPlusPotential(nn.Module):
         return z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr, n_mol
 
 
-class DimeNetRunner:
+class DimeNetRunner(EngineDriver):
     """Host driver of `nb200_dimenet_*`: owns the engine handle, the exported weights, the graph buffer and the workspace."""
 
-    def __init__(self, lib):
-        self.lib = lib
-        h = c_void_p()
-        check(lib.nb200_engine_create(byref(h)), "nb200_engine_create")
-        self._h = h
+    def __init__(self, lib=None):
+        super().__init__(lib)
         self._w = None
         self._keep = None
-        self._graph_buf = self._ws = None
         self.last_counts: Dict[str, int] = {}
-
-    def __del__(self):
-        try:
-            if self._h:
-                self.lib.nb200_engine_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
-    def _stream(self):
-        return c_void_p(torch.cuda.current_stream().cuda_stream)
 
     def set_weights(self, model: DimeNetPlusPlusPotential, device):
         self.bind(model, *model.export(device))
@@ -288,14 +266,6 @@ class DimeNetRunner:
                            scale, mean, buf.data_ptr(), ctypes.cast(off_arr, POINTER(c_int64)))
         self._w, self._keep = w, (buf, off_arr)
 
-    def _buffer(self, attr: str, nbytes: int, device):
-        cur = getattr(self, attr)
-        if cur is None or cur.numel() < nbytes or cur.device != device:
-            setattr(self, attr, None)  # free the old buffer before the larger one is allocated
-            cur = torch.empty(int(nbytes * 1.25) + 256, dtype=torch.uint8, device=device)
-            setattr(self, attr, cur)
-        return cur
-
     def run(self, z, pos, mol_ptr, n_mol: int):
         """Two-phase call: graph (one synchronisation for the counts), workspace, energies / forces / graph embeddings."""
         if self._w is None:
@@ -303,10 +273,7 @@ class DimeNetRunner:
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
         s = self._stream()
         gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
-        wbytes = lib.nb200_dimenet_workspace_bytes(byref(self._w), n_mol, n, counts)
-        if wbytes < 0:
-            check(int(wbytes), "nb200_dimenet_workspace_bytes")
-        ws = self._buffer("_ws", wbytes, dev)
+        ws = self._buffer("_ws", self._bytes("nb200_dimenet_workspace_bytes", byref(self._w), n_mol, n, counts), dev)
         energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
         forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
         emb = torch.empty(n_mol, self._w.node_latent_dim, dtype=torch.float32, device=dev)
@@ -319,10 +286,7 @@ class DimeNetRunner:
         lib, n = self.lib, int(z.shape[0])
         if n == 0 or n_mol == 0:
             raise NablaB200Error("DimeNetPlusPlusPotential: empty batch")
-        gbytes = lib.nb200_dimenet_graph_bytes(byref(self._w), n)
-        if gbytes < 0:
-            check(int(gbytes), "nb200_dimenet_graph_bytes")
-        gbuf = self._buffer("_graph_buf", gbytes, pos.device)
+        gbuf = self._buffer("_graph_buf", self._bytes("nb200_dimenet_graph_bytes", byref(self._w), n), pos.device)
         counts = (c_int64 * N_COUNTS)()
         check(lib.nb200_dimenet_graph_count(byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(), gbuf.numel(),
                                             counts, self._stream()), "nb200_dimenet_graph_count")
@@ -335,18 +299,11 @@ class DimeNetRunner:
         if self._w is None:
             raise NablaB200Error("DimeNetRunner.train_grads before set_weights / bind")
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
-        wbytes = lib.nb200_dimenet_train_workspace_bytes(byref(self._w), n_mol, n, counts)
-        if wbytes < 0:
-            check(int(wbytes), "nb200_dimenet_train_workspace_bytes")
-        ws = self._buffer("_ws", wbytes, dev)
-        buf = self._keep[0]
-        grads = torch.zeros_like(buf)  # the call writes up to the end of the last entry
         seeds = [None if t is None else t.detach().to(device=dev, dtype=torch.float32).contiguous() for t in (seed_energy, seed_forces)]
-        if seeds[0] is not None and seeds[0].shape != (n_mol,):
-            raise NablaB200Error(f"seed_energy: expected shape ({n_mol},), got {tuple(seeds[0].shape)}")
-        if seeds[1] is not None and seeds[1].shape != (n, 3):
-            raise NablaB200Error(f"seed_forces: expected shape ({n}, 3), got {tuple(seeds[1].shape)}")
+        self._check_seeds(*seeds, n_mol, n, dev)
+        gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
+        ws = self._buffer("_ws", self._bytes("nb200_dimenet_train_workspace_bytes", byref(self._w), n_mol, n, counts), dev)
+        grads = torch.zeros_like(self._keep[0])  # the call writes up to the end of the last entry
         ptr = [0 if t is None else t.data_ptr() for t in seeds]
         check(lib.nb200_dimenet_train_grads(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(),
                                             gbuf.numel(), counts, ws.data_ptr(), ws.numel(), ptr[0] or None, ptr[1] or None, grads.data_ptr(),
@@ -366,10 +323,7 @@ class DimeNetRunner:
             raise NablaB200Error(f"run_hvp(): v must be a contiguous fp32 tensor [n_dir, {n}, 3] with n_dir >= 1 on {dev}")
         n_dir = int(v.shape[0])
         gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
-        wbytes = lib.nb200_dimenet_hvp_workspace_bytes(byref(self._w), n_mol, n, counts)
-        if wbytes < 0:
-            check(int(wbytes), "nb200_dimenet_hvp_workspace_bytes")
-        ws = self._buffer("_ws", wbytes, dev)
+        ws = self._buffer("_ws", self._bytes("nb200_dimenet_hvp_workspace_bytes", byref(self._w), n_mol, n, counts), dev)
         energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
         forces = torch.empty(n, 3, dtype=torch.float32, device=dev) if with_forces else None
         hv = torch.empty(n_dir, n, 3, dtype=torch.float32, device=dev)

@@ -4,13 +4,14 @@ Owns: the C engine object, the device workspace, the canonical weight export.
 The model classes (`painn_oc.PaiNN`, `spk.NeuralNetworkPotential`) only describe how their
 reference-named parameters map onto the canonical layout.
 """
-from ctypes import byref, c_int64, c_void_p
+from ctypes import byref
 from typing import Dict, Optional, Tuple
 
 import torch
 
 from . import _lib
-from ._lib import NablaB200Error, PainnWeights, SchnetWeights, check, current_stream, ptr
+from ._lib import EngineDriver, NablaB200Error, PainnWeights, SchnetWeights, check, ptr
+from .schnet_train import count_edges
 
 _KINDS = {
     "painn": (PainnWeights, "nb200_painn_workspace_bytes", "nb200_painn_energy_forces",
@@ -20,17 +21,15 @@ _KINDS = {
 }
 
 
-class PainnEngine:
+class PainnEngine(EngineDriver):
     """One engine per (module, device). Not thread-safe; one CUDA stream per call."""
 
+    SLACK = 1.05  # the capacity-sized workspace is the largest buffer of the project (the filter rows alone: ~3.5 GB per bench.py step)
+
     def __init__(self, kind: str = "painn", lib=None):
-        """`lib`: a bound library exporting the C ABI (default: libnabla_b200.so)."""
+        super().__init__(lib)
         self.kind = kind
         self._wtype, self._ws_fn, self._run_fn, self._wkeys = _KINDS[kind]
-        self.lib = _lib.load() if lib is None else lib
-        h = c_void_p()
-        check(self.lib.nb200_engine_create(byref(h)), "nb200_engine_create")
-        self._h = h
         self._ws: Optional[torch.Tensor] = None
         self._status: Optional[torch.Tensor] = None
         self._weights = None
@@ -47,14 +46,6 @@ class PainnEngine:
         self._kept_serial = 0
         self._kept_args = None
         self.edge_storage = "f32"
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                self.lib.nb200_engine_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def set_edge_storage(self, kind: str) -> None:
         """'f32' (default) or 'bf16': storage of the per-edge arrays of the TRAINING calls (`nb200_engine_set_edge_storage`)."""
@@ -82,15 +73,46 @@ class PainnEngine:
         self._wkey = key
 
     # ------------------------------------------------------------------ run
-    def _ensure_ws(self, n_mol: int, n_atoms: int, e_cap: int, with_forces: bool, device):
-        need = getattr(self.lib, self._ws_fn)(byref(self._weights), n_mol, n_atoms, e_cap, int(with_forces))
-        if need < 0:
-            check(int(need), self._ws_fn)
-        if self._ws is None or self._ws.numel() < need or self._ws.device != device:
-            self._ws = None  # release before growing
-            self._ws = torch.empty(int(need * 1.05) + 256, dtype=torch.uint8, device=device)
+    def _workspace(self, fn_name: str, *args, device) -> torch.Tensor:
+        """The workspace sized by `fn_name(weights, *args)`, and the device status word of the calls."""
         if self._status is None or self._status.device != device:
             self._status = torch.zeros(4, dtype=torch.int32, device=device)
+        return self._buffer("_ws", self._bytes(fn_name, byref(self._weights), *args), device)
+
+    def _cap(self, n_atoms: int, validated: bool = False) -> int:
+        """Edge capacity of the next launch (never below the current one): the first-batch guess, or, once a checked launch has measured
+        the edges per atom, 25 % + `e_cap_slack` above that."""
+        want = int(1.25 * self._validated_ratio * n_atoms) + self.e_cap_slack if validated else n_atoms * self.edges_per_atom_guess
+        return max(self.e_cap, want)
+
+    def _regrow(self, call):
+        """Synchronous: `call()` launches with `_cap` and fills the status word; on NB200_ECAPACITY the capacity grows to the reported
+        edge count and the call runs once more.  -> (what `call` returned, status on the host)."""
+        for _ in range(2):
+            out = call()
+            st = self._status.cpu()
+            if int(st[1]) == -4:
+                self.e_cap = int(int(st[0]) * 1.1) + 1024
+                continue
+            self.raise_on_status(st)
+            return out, st
+        raise NablaB200Error("edge capacity regrow failed")
+
+    def _defer_status(self, n_atoms: int) -> None:
+        """Queue the status word of the launch just enqueued for `check_pending`: a pinned host copy behind the results, and an event."""
+        host = torch.empty(5, dtype=torch.int32, pin_memory=True)
+        host[4] = n_atoms
+        host[:4].copy_(self._status, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._pending.append((host, ev))
+
+    def _first_run(self, z, pos, mol_ptr, n_mol, with_forces):
+        """The synchronous `run` of an engine's first batch, which sizes the capacity of the asynchronous launches after it."""
+        energy, forces, st = self.run(z, pos, mol_ptr, n_mol, with_forces)
+        self._validated_ratio = float(int(st[0])) / max(1, z.shape[0])
+        self.e_cap = max(self.e_cap, int(1.25 * int(st[0])) + 1024)
+        return energy, forces
 
     def launch(self, z: torch.Tensor, pos: torch.Tensor, mol_ptr: torch.Tensor, n_mol: int, with_forces: bool = True,
                e_cap: Optional[int] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor], torch.Tensor]:
@@ -100,19 +122,17 @@ class PainnEngine:
         if self._weights is None:
             raise NablaB200Error("set_weights() first")
         n_atoms = z.shape[0]
-        if not (z.is_cuda and z.dtype == torch.int32 and pos.dtype == torch.float32 and mol_ptr.dtype == torch.int32):
+        if not (self._on_device(z) and z.dtype == torch.int32 and pos.dtype == torch.float32 and mol_ptr.dtype == torch.int32):
             raise NablaB200Error("launch(): need CUDA int32 z / mol_ptr and fp32 pos")
-        if e_cap is None:
-            e_cap = max(self.e_cap, n_atoms * self.edges_per_atom_guess)
-        self.e_cap = e_cap
+        self.e_cap = e_cap = self._cap(n_atoms) if e_cap is None else e_cap
         self._kept_token = 0  # this launch overwrites the workspace a kept training forward lives in
-        self._ensure_ws(n_mol, n_atoms, e_cap, with_forces, z.device)
+        ws = self._workspace(self._ws_fn, n_mol, n_atoms, e_cap, int(with_forces), device=z.device)
         energy = torch.empty(n_mol, dtype=torch.float32, device=z.device)
         forces = torch.empty(n_atoms, 3, dtype=torch.float32, device=z.device) if with_forces else None
         status = self._status
         rc = getattr(self.lib, self._run_fn)(
             self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap,
-            ptr(self._ws), self._ws.numel(), ptr(energy), ptr(forces), ptr(status), current_stream())
+            ptr(ws), ws.numel(), ptr(energy), ptr(forces), ptr(status), self._stream())
         check(rc, self._run_fn)
         return energy, forces, status
 
@@ -127,6 +147,15 @@ class PainnEngine:
     # ------------------------------------------------------------------ training
     GRAD_KEYS = ("emb", "w_rbf", "b_rbf", "A1", "c1", "A2", "c2", "U", "B1", "d1", "B2", "d2", "R1", "e1", "R2", "e2")
 
+    def _grad_struct(self):
+        """Fresh gradient tensors shaped like the exported weights, and the weight struct of the gradient calls that points at them
+        (rbf_offsets: the weights' own)."""
+        grads = {k: torch.empty_like(self._keep[k]) for k in self.GRAD_KEYS}
+        gw = self._wtype()
+        for k in self._wkeys:
+            setattr(gw, k, (grads[k] if k in grads else self._keep[k]).data_ptr())
+        return grads, gw
+
     def run_train(self, z, pos, mol_ptr, n_mol, seed: Optional[torch.Tensor], force_seed: Optional[torch.Tensor] = None):
         """One training step of the PaiNN engine in one call (`nb200_painn_energy_forces_grads`: the fused forward of
         `run_train_forward`, then the backward of `run_train_backward`): energy, true forces and
@@ -140,51 +169,30 @@ class PainnEngine:
         n_atoms = z.shape[0]
         dev = z.device
         self._kept_token = 0
-        grads = {k: torch.empty_like(self._keep[k]) for k in self.GRAD_KEYS}
-        gw = self._wtype()
-        for k in self._wkeys:
-            setattr(gw, k, grads[k].data_ptr() if k in grads else self._keep[k].data_ptr())
-        if seed is not None and not (seed.is_cuda and seed.dtype == torch.float32 and seed.is_contiguous() and seed.numel() == n_mol):
-            raise NablaB200Error("run_train(): seed must be a contiguous fp32 CUDA tensor [n_mol]")
-        if force_seed is not None and not (force_seed.is_cuda and force_seed.dtype == torch.float32 and force_seed.is_contiguous()
-                                           and force_seed.numel() == 3 * n_atoms):
-            raise NablaB200Error("run_train(): force_seed must be a contiguous fp32 CUDA tensor [n_atoms, 3]")
+        grads, gw = self._grad_struct()
+        self._check_seeds(seed, force_seed, n_mol, n_atoms, dev)
         validated = self._validated_ratio > 0.0  # a checked launch has sized the edge capacity: no host sync in this call then
-        for _ in range(2):
-            e_cap = max(self.e_cap, int(1.25 * self._validated_ratio * n_atoms) + self.e_cap_slack) if validated else max(self.e_cap, n_atoms * self.edges_per_atom_guess)
-            self.e_cap = e_cap
-            need = self.lib.nb200_painn_train_workspace_bytes(byref(self._weights), n_mol, n_atoms, e_cap, int(force_seed is not None))
-            if need < 0:
-                check(int(need), "nb200_painn_train_workspace_bytes")
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                self._ws = None
-                self._ws = torch.empty(int(need * 1.05) + 256, dtype=torch.uint8, device=dev)
-            if self._status is None or self._status.device != dev:
-                self._status = torch.zeros(4, dtype=torch.int32, device=dev)
+
+        def call():
+            self.e_cap = e_cap = self._cap(n_atoms, validated)
+            ws = self._workspace("nb200_painn_train_workspace_bytes", n_mol, n_atoms, e_cap, int(force_seed is not None), device=dev)
             energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
             forces = torch.empty(n_atoms, 3, dtype=torch.float32, device=dev)
             rc = self.lib.nb200_painn_energy_forces_grads(
-                self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(self._ws), self._ws.numel(),
-                ptr(seed), ptr(force_seed), byref(gw), ptr(energy), ptr(forces), ptr(self._status), current_stream())
+                self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(ws), ws.numel(),
+                ptr(seed), ptr(force_seed), byref(gw), ptr(energy), ptr(forces), ptr(self._status), self._stream())
             check(rc, "nb200_painn_energy_forces_grads")
-            if validated:
-                # deferred status check (as run_async): a failed launch has NaN energies / forces, and its gradients came from an empty graph;
-                # the next call (or check_pending(wait=True)) raises
-                host = torch.empty(5, dtype=torch.int32, pin_memory=True)
-                host[4] = n_atoms
-                host[:4].copy_(self._status, non_blocking=True)
-                ev = torch.cuda.Event()
-                ev.record()
-                self._pending.append((host, ev))
-                return energy, forces, grads
-            st = self._status.cpu()
-            if int(st[1]) == -4:
-                self.e_cap = int(int(st[0]) * 1.1) + 1024
-                continue
-            self.raise_on_status(st)
+            return energy, forces
+
+        if validated:
+            # deferred status check (as run_async): a failed launch has NaN energies / forces, and its gradients came from an empty graph;
+            # the next call (or check_pending(wait=True)) raises
+            energy, forces = call()
+            self._defer_status(n_atoms)
+        else:
+            (energy, forces), st = self._regrow(call)
             self._validated_ratio = max(self._validated_ratio, float(int(st[0])) / max(1, n_atoms))
-            return energy, forces, grads
-        raise NablaB200Error("edge capacity regrow failed")
+        return energy, forces, grads
 
     # ------------------------------------------------------------------ training step in two calls (forward kept for the backward)
     def run_train_forward(self, z, pos, mol_ptr, n_mol, with_force_seed: bool = True):
@@ -197,33 +205,18 @@ class PainnEngine:
         self.check_pending()
         n_atoms, dev = z.shape[0], z.device
         if self._validated_ratio == 0.0:
-            _, _, st = self.run(z, pos, mol_ptr, n_mol, True)
-            self._validated_ratio = float(int(st[0])) / max(1, n_atoms)
-            self.e_cap = max(self.e_cap, int(1.25 * int(st[0])) + 1024)
-        e_cap = max(self.e_cap, int(1.25 * self._validated_ratio * n_atoms) + self.e_cap_slack)
-        self.e_cap = e_cap
-        need = self.lib.nb200_painn_train_workspace_bytes(byref(self._weights), n_mol, n_atoms, e_cap, int(with_force_seed))
-        if need < 0:
-            check(int(need), "nb200_painn_train_workspace_bytes")
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = None
-            self._ws = torch.empty(int(need * 1.05) + 256, dtype=torch.uint8, device=dev)
-        if self._status is None or self._status.device != dev:
-            self._status = torch.zeros(4, dtype=torch.int32, device=dev)
+            self._first_run(z, pos, mol_ptr, n_mol, True)
+        self.e_cap = e_cap = self._cap(n_atoms, validated=True)
+        ws = self._workspace("nb200_painn_train_workspace_bytes", n_mol, n_atoms, e_cap, int(with_force_seed), device=dev)
         energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
         forces = torch.empty(n_atoms, 3, dtype=torch.float32, device=dev)
-        rc = self.lib.nb200_painn_train_forward(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(self._ws),
-                                                self._ws.numel(), int(with_force_seed), ptr(energy), ptr(forces), ptr(self._status), current_stream())
+        rc = self.lib.nb200_painn_train_forward(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(ws),
+                                                ws.numel(), int(with_force_seed), ptr(energy), ptr(forces), ptr(self._status), self._stream())
         check(rc, "nb200_painn_train_forward")
-        host = torch.empty(5, dtype=torch.int32, pin_memory=True)
-        host[4] = n_atoms
-        host[:4].copy_(self._status, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._pending.append((host, ev))
+        self._defer_status(n_atoms)
         self._kept_serial += 1
         self._kept_token = self._kept_serial
-        self._kept_args = (n_mol, n_atoms, e_cap, int(with_force_seed), self._ws.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        self._kept_args = (n_mol, n_atoms, e_cap, int(with_force_seed), ws.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
         return energy, forces, self._kept_token
 
     def kept(self, token: int) -> bool:
@@ -238,29 +231,15 @@ class PainnEngine:
             raise NablaB200Error("run_train_backward(): workspace or stream changed since the forward")
         if force_seed is not None and not wfs:
             raise NablaB200Error("run_train_backward(): the forward was run without room for the force-seed tangent pass")
-        if seed is not None and not (seed.is_cuda and seed.dtype == torch.float32 and seed.is_contiguous() and seed.numel() == n_mol):
-            raise NablaB200Error("run_train_backward(): seed must be a contiguous fp32 CUDA tensor [n_mol]")
-        if force_seed is not None and not (force_seed.is_cuda and force_seed.dtype == torch.float32 and force_seed.is_contiguous()
-                                           and force_seed.numel() == 3 * n_atoms):
-            raise NablaB200Error("run_train_backward(): force_seed must be a contiguous fp32 CUDA tensor [n_atoms, 3]")
-        grads = {k: torch.empty_like(self._keep[k]) for k in self.GRAD_KEYS}
-        gw = self._wtype()
-        for k in self._wkeys:
-            setattr(gw, k, grads[k].data_ptr() if k in grads else self._keep[k].data_ptr())
+        self._check_seeds(seed, force_seed, n_mol, n_atoms, z.device)
+        grads, gw = self._grad_struct()
         rc = self.lib.nb200_painn_train_backward(self._h, byref(self._weights), ptr(z), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(self._ws), self._ws.numel(),
-                                                 wfs, ptr(seed), ptr(force_seed), byref(gw), ptr(self._status), current_stream())
+                                                 wfs, ptr(seed), ptr(force_seed), byref(gw), ptr(self._status), self._stream())
         check(rc, "nb200_painn_train_backward")
         self._kept_token = 0  # the backward reuses transient buffers; a second backward of the same forward recomputes
         return grads
 
     # ------------------------------------------------------------------ Hessian-vector products
-    # device check and stream of the calls below: tests/test_schnet_hvp_emu.py runs the same host code on CPU tensors against the emulation build
-    def _on_device(self, t: torch.Tensor) -> bool:
-        return t.is_cuda
-
-    def _stream(self):
-        return current_stream()
-
     def run_hvp(self, z, pos, mol_ptr, n_mol, v, with_forces: bool = True):
         """Exact Hessian-vector products of the energy (`nb200_painn_hvp`, `nb200_schnet_hvp`): v [n_dir, n_atoms, 3] (or [n_atoms, 3]) fp32
         CUDA, in Angstrom.  Returns (energy [B], forces [N, 3] or None, hv [n_dir, N, 3] = H v in Ha/A).  Synchronous like `run`: the PaiNN
@@ -281,52 +260,29 @@ class PainnEngine:
         self._kept_token = 0  # this call overwrites the workspace a kept training forward lives in
         if self.kind == "schnet":
             return self._run_schnet_hvp(z, pos, mol_ptr, n_mol, v, with_forces)
-        for _ in range(2):
-            e_cap = max(self.e_cap, n_atoms * self.edges_per_atom_guess)
-            self.e_cap = e_cap
-            need = self.lib.nb200_painn_hvp_workspace_bytes(byref(self._weights), n_mol, n_atoms, e_cap, n_dir)
-            if need < 0:
-                check(int(need), "nb200_painn_hvp_workspace_bytes")
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                self._ws = None
-                self._ws = torch.empty(int(need * 1.05) + 256, dtype=torch.uint8, device=dev)
-            if self._status is None or self._status.device != dev:
-                self._status = torch.zeros(4, dtype=torch.int32, device=dev)
+
+        def call():
+            self.e_cap = e_cap = self._cap(n_atoms)
+            ws = self._workspace("nb200_painn_hvp_workspace_bytes", n_mol, n_atoms, e_cap, n_dir, device=dev)
             energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
             forces = torch.empty(n_atoms, 3, dtype=torch.float32, device=dev) if with_forces else None
             hv = torch.empty(n_dir, n_atoms, 3, dtype=torch.float32, device=dev)
-            rc = self.lib.nb200_painn_hvp(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(self._ws),
-                                          self._ws.numel(), n_dir, ptr(v), ptr(energy), ptr(forces), ptr(hv), ptr(self._status), current_stream())
+            rc = self.lib.nb200_painn_hvp(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, e_cap, ptr(ws),
+                                          ws.numel(), n_dir, ptr(v), ptr(energy), ptr(forces), ptr(hv), ptr(self._status), self._stream())
             check(rc, "nb200_painn_hvp")
-            st = self._status.cpu()
-            if int(st[1]) == -4:
-                self.e_cap = int(int(st[0]) * 1.1) + 1024
-                continue
-            self.raise_on_status(st)
             return energy, forces, hv
-        raise NablaB200Error("edge capacity regrow failed")
+
+        return self._regrow(call)[0]
 
     def _run_schnet_hvp(self, z, pos, mol_ptr, n_mol, v, with_forces):
         """`nb200_schnet_train_count` (exact edge count, one host sync), then `nb200_schnet_hvp` on the engine's weights."""
-        lib, n_atoms, dev, n_dir = self.lib, z.shape[0], z.device, v.shape[0]
-        s = self._stream()
-        row_ptr = torch.empty(n_atoms + 1, dtype=torch.int32, device=dev)
-        scratch = torch.empty(2 * n_atoms, dtype=torch.int32, device=dev)
-        n_edges = c_int64(0)
-        check(lib.nb200_schnet_train_count(byref(self._weights), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, ptr(row_ptr), ptr(scratch), byref(n_edges), s),
-              "nb200_schnet_train_count")
-        need = lib.nb200_schnet_hvp_workspace_bytes(byref(self._weights), n_mol, n_atoms, n_edges.value)
-        if need < 0:
-            check(int(need), "nb200_schnet_hvp_workspace_bytes")
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = None
-            self._ws = torch.empty(int(need * 1.05) + 256, dtype=torch.uint8, device=dev)
+        n_atoms, dev, n_dir = z.shape[0], z.device, v.shape[0]
+        row_ptr, n_edges, ws = count_edges(self, self._weights, pos, mol_ptr, n_mol, "nb200_schnet_hvp_workspace_bytes")
         energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
         forces = torch.empty(n_atoms, 3, dtype=torch.float32, device=dev) if with_forces else None
         hv = torch.empty(n_dir, n_atoms, 3, dtype=torch.float32, device=dev)
-        check(lib.nb200_schnet_hvp(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, ptr(row_ptr), n_edges.value,
-                                   ptr(self._ws), self._ws.numel(), n_dir, ptr(v), ptr(energy), ptr(forces), ptr(hv), s), "nb200_schnet_hvp")
-        self.last_edges = int(n_edges.value)
+        check(self.lib.nb200_schnet_hvp(self._h, byref(self._weights), ptr(z), ptr(pos), ptr(mol_ptr), n_mol, n_atoms, ptr(row_ptr), n_edges,
+                                        ptr(ws), ws.numel(), n_dir, ptr(v), ptr(energy), ptr(forces), ptr(hv), self._stream()), "nb200_schnet_hvp")
         return energy, forces, hv
 
     # ------------------------------------------------------------------ asynchronous inference (the reference-facing forward())
@@ -359,18 +315,9 @@ class PainnEngine:
         self.check_pending()
         n_atoms = z.shape[0]
         if self._validated_ratio == 0.0:
-            energy, forces, st = self.run(z, pos, mol_ptr, n_mol, with_forces)
-            self._validated_ratio = float(int(st[0])) / max(1, n_atoms)
-            self.e_cap = max(self.e_cap, int(1.25 * int(st[0])) + 1024)
-            return energy, forces
-        e_cap = max(self.e_cap, int(1.25 * self._validated_ratio * n_atoms) + self.e_cap_slack)
-        energy, forces, status = self.launch(z, pos, mol_ptr, n_mol, with_forces, e_cap=e_cap)
-        host = torch.empty(5, dtype=torch.int32, pin_memory=True)
-        host[4] = n_atoms
-        host[:4].copy_(status, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._pending.append((host, ev))
+            return self._first_run(z, pos, mol_ptr, n_mol, with_forces)
+        energy, forces, _ = self.launch(z, pos, mol_ptr, n_mol, with_forces, e_cap=self._cap(n_atoms, validated=True))
+        self._defer_status(n_atoms)
         return energy, forces
 
     def clone_for_stream(self) -> "PainnEngine":
@@ -385,15 +332,8 @@ class PainnEngine:
     def run(self, z, pos, mol_ptr, n_mol, with_forces=True):
         """Synchronous convenience: launch, check the device status, regrow the edge capacity once
         if the guess was too small (the only host<->device sync of the whole path)."""
-        for _ in range(2):
-            energy, forces, status = self.launch(z, pos, mol_ptr, n_mol, with_forces)
-            st = status.cpu()
-            if int(st[1]) == -4:  # capacity: regrow to the reported edge count and retry
-                self.e_cap = int(int(st[0]) * 1.1) + 1024
-                continue
-            self.raise_on_status(st)
-            return energy, forces, st
-        raise NablaB200Error("edge capacity regrow failed")
+        (energy, forces, _), st = self._regrow(lambda: self.launch(z, pos, mol_ptr, n_mol, with_forces))
+        return energy, forces, st
 
 
 def mol_ptr_from_batch(batch: torch.Tensor, n_mol: Optional[int] = None) -> Tuple[torch.Tensor, int]:

@@ -20,14 +20,14 @@ STATUS (round 1): every kernel has been checked against the oracle through the h
 import ctypes
 import math
 import re
-from ctypes import POINTER, byref, c_float, c_int32, c_int64, c_void_p
+from ctypes import POINTER, byref, c_float, c_int32, c_int64
 from typing import Dict, List, Optional, Tuple
 
 import torch
 from torch import nn
 
-from ._lib import SIGNATURES as _ALL_SIGNATURES
-from ._lib import GemNetOCWeights, NablaB200Error, check
+from . import _lib
+from ._lib import EngineDriver, GemNetOCWeights, NablaB200Error, check
 
 # ---- canonical layout: keep in step with the enums of include/nabla_b200.h (tests/test_host.py compares the names) -------------------
 G_NAMES = ["RBF_OFFSET", "EMB", "CAT_MAIN", "CAT_AE", "CAT_Q", "CAT_A2A", "EDGE_EMB", "OUT_E0", "OUT_E_RES", "OUT_ENERGY", "OUT_F0", "OUT_F_RES",
@@ -41,17 +41,12 @@ SO_NAMES = ["SUM", "RBF_F"]
 C_NAMES = ["A2A", "MAIN", "AE", "Q", "TIN"]
 N_COUNTS = 8
 LD_MAIN = 1920
-
-
-SIGNATURES = {k: v for k, v in _ALL_SIGNATURES.items() if k.startswith("nb200_gemnet_oc_")}
+SIGNATURES = {k: v for k, v in _lib.SIGNATURES.items() if k.startswith("nb200_gemnet_oc_")}
 
 
 def bind(lib):
-    """Attach the GemNet-OC prototypes to a loaded library (libnabla_b200.so is bound by _lib.load(); this is for tests/emu)."""
-    for name, (res, args) in SIGNATURES.items():
-        fn = getattr(lib, name)
-        fn.restype, fn.argtypes = res, args
-    return lib
+    """The GemNet-OC prototypes on `lib`, e.g. an emulation build of csrc/gemnet_oc.cu, which exports no other engine."""
+    return _lib.bind(lib, ["nb200_gemnet_oc_"])
 
 
 # ---- parameter holders with the reference's attribute names ----------------------------------------------------------------------------
@@ -382,9 +377,7 @@ class GemNetOC(nn.Module):
 
     def _get_runner(self) -> "GemNetOCRunner":
         if self._runner is None:
-            from . import _lib
-
-            self._runner = GemNetOCRunner(bind(_lib.load()))
+            self._runner = GemNetOCRunner()
         return self._runner
 
     def _sync_weights(self, runner: "GemNetOCRunner", device) -> None:
@@ -428,31 +421,15 @@ class GemNetOC(nn.Module):
         return runner.run(z, pos, mol_ptr, n_mol, max_atoms)
 
 
-class GemNetOCRunner:
-    """Host driver of `nb200_gemnet_oc_*`: owns the engine handle, the exported weights, the graph buffer and the workspace.
-    `lib` is the bound shared library (libnabla_b200.so via `_lib.load()`)."""
+class GemNetOCRunner(EngineDriver):
+    """Host driver of `nb200_gemnet_oc_*`: owns the engine handle, the exported weights, the graph buffers and the workspaces."""
 
-    def __init__(self, lib):
-        self.lib = lib
-        h = c_void_p()
-        check(lib.nb200_engine_create(byref(h)), "nb200_engine_create")
-        self._h = h
+    def __init__(self, lib=None):
+        super().__init__(lib)
         self._w = None
         self._keep = None
-        self._graph_buf = self._ws = self._train_ws = self._train_graph_buf = None
         self._status = None
         self.last_counts: Dict[str, int] = {}
-
-    def __del__(self):
-        try:
-            if self._h:
-                self.lib.nb200_engine_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
-    def _stream(self):
-        return c_void_p(torch.cuda.current_stream().cuda_stream)
 
     def set_weights(self, model: GemNetOC, device):
         self.set_weights_from(model, *model.export(device))
@@ -464,12 +441,15 @@ class GemNetOCRunner:
                             buf.data_ptr(), ctypes.cast(off_arr, POINTER(c_int64)), ctypes.cast(sc_arr, POINTER(c_float)))
         self._w, self._keep = w, (buf, off_arr, sc_arr)
 
-    def _buffer(self, attr: str, nbytes: int, device):
-        cur = getattr(self, attr)
-        if cur is None or cur.numel() < nbytes or cur.device != device:
-            cur = torch.empty(int(nbytes * 1.25) + 256, dtype=torch.uint8, device=device)
-            setattr(self, attr, cur)
-        return cur
+    def _graph(self, pos, mol_ptr, n_mol: int, max_atoms_per_mol: int, attr: str = "_graph_buf"):
+        """Phase one of a two-phase call: the four graphs in the buffer `self.<attr>` and their counts (one synchronisation)."""
+        n = int(pos.shape[0])
+        gbuf = self._buffer(attr, self._bytes("nb200_gemnet_oc_graph_bytes", n, max_atoms_per_mol), pos.device)
+        counts = (c_int64 * N_COUNTS)()
+        check(self.lib.nb200_gemnet_oc_graph_count(byref(self._w), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol, gbuf.data_ptr(),
+                                                   gbuf.numel(), counts, self._stream()), "nb200_gemnet_oc_graph_count")
+        self.last_counts = {k: int(counts[i]) for i, k in enumerate(C_NAMES)}
+        return gbuf, counts
 
     def run_train(self, z, pos, mol_ptr, n_mol: int, max_atoms_per_mol: int, seed_energy=None, seed_forces=None, keep: bool = False):
         """nb200_gemnet_oc_energy_forces_grads with the weights bound by set_weights_from.
@@ -480,25 +460,12 @@ class GemNetOCRunner:
         if self._w is None:
             raise NablaB200Error("GemNetOCRunner.run_train before set_weights")
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        s = self._stream()
+        self._check_seeds(seed_energy, seed_forces, n_mol, n, dev)
         buf = self._keep[0]
-        gbytes = lib.nb200_gemnet_oc_graph_bytes(n, max_atoms_per_mol)
-        if gbytes < 0:
-            check(int(gbytes), "nb200_gemnet_oc_graph_bytes")
-        gbuf = self._buffer("_train_graph_buf", gbytes, dev)
-        counts = (c_int64 * N_COUNTS)()
-        check(lib.nb200_gemnet_oc_graph_count(byref(self._w), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol, gbuf.data_ptr(),
-                                              gbuf.numel(), counts, s), "nb200_gemnet_oc_graph_count")
-        self.last_counts = {k: int(counts[i]) for i, k in enumerate(C_NAMES)}
-        wbytes = lib.nb200_gemnet_oc_train_workspace_bytes(byref(self._w), n_mol, n, counts)
-        if wbytes < 0:
-            check(int(wbytes), "nb200_gemnet_oc_train_workspace_bytes")
-        ws = self._buffer("_train_ws", wbytes, dev)
+        gbuf, counts = self._graph(pos, mol_ptr, n_mol, max_atoms_per_mol, "_train_graph_buf")
+        ws = self._buffer("_train_ws", self._bytes("nb200_gemnet_oc_train_workspace_bytes", byref(self._w), n_mol, n, counts), dev)
         energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
         forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        for t_, shape in ((seed_energy, n_mol), (seed_forces, 3 * n)):
-            if t_ is not None and not (t_.dtype == torch.float32 and t_.is_contiguous() and t_.numel() == shape and t_.device == dev):
-                raise NablaB200Error("run_train(): seeds must be contiguous fp32 tensors [n_mol] / [n_atoms, 3] on the batch's device")
         seeded = seed_energy is not None or seed_forces is not None
         grads = torch.empty_like(buf) if (seeded or keep) else None
         token = c_int64(0)
@@ -506,7 +473,7 @@ class GemNetOCRunner:
             self._h, byref(self._w), buf.numel(), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol, gbuf.data_ptr(), gbuf.numel(),
             counts, ws.data_ptr(), ws.numel(), seed_energy.data_ptr() if seed_energy is not None else None,
             seed_forces.data_ptr() if seed_forces is not None else None, grads.data_ptr() if grads is not None else None, energy.data_ptr(), forces.data_ptr(),
-            byref(token) if (keep and not seeded) else None, s), "nb200_gemnet_oc_energy_forces_grads")
+            byref(token) if (keep and not seeded) else None, self._stream()), "nb200_gemnet_oc_energy_forces_grads")
         if keep and not seeded:
             return energy, forces, (int(token.value), grads)
         return energy, forces, grads
@@ -526,18 +493,8 @@ class GemNetOCRunner:
             raise NablaB200Error("GemNetOCRunner.run before set_weights")
         lib, n = self.lib, int(z.shape[0])
         s = self._stream()
-        gbytes = lib.nb200_gemnet_oc_graph_bytes(n, max_atoms_per_mol)
-        if gbytes < 0:
-            check(int(gbytes), "nb200_gemnet_oc_graph_bytes")
-        gbuf = self._buffer("_graph_buf", gbytes, pos.device)
-        counts = (c_int64 * N_COUNTS)()
-        check(lib.nb200_gemnet_oc_graph_count(byref(self._w), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol, gbuf.data_ptr(),
-                                              gbuf.numel(), counts, s), "nb200_gemnet_oc_graph_count")
-        self.last_counts = {k: int(counts[i]) for i, k in enumerate(C_NAMES)}
-        wbytes = lib.nb200_gemnet_oc_workspace_bytes(byref(self._w), n_mol, n, counts)
-        if wbytes < 0:
-            check(int(wbytes), "nb200_gemnet_oc_workspace_bytes")
-        ws = self._buffer("_ws", wbytes, pos.device)
+        gbuf, counts = self._graph(pos, mol_ptr, n_mol, max_atoms_per_mol)
+        ws = self._buffer("_ws", self._bytes("nb200_gemnet_oc_workspace_bytes", byref(self._w), n_mol, n, counts), pos.device)
         energy = torch.empty(n_mol, dtype=torch.float32, device=pos.device)
         forces = torch.empty(n, 3, dtype=torch.float32, device=pos.device)
         check(lib.nb200_gemnet_oc_energy_forces(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol,
@@ -566,14 +523,9 @@ class GemNetOCRunner:
         if self._w is None:
             raise NablaB200Error("GemNetOCRunner.launch before set_weights")
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        gbytes = lib.nb200_gemnet_oc_graph_bytes(n, max_atoms_per_mol)
-        if gbytes < 0:
-            check(int(gbytes), "nb200_gemnet_oc_graph_bytes")
-        wbytes = lib.nb200_gemnet_oc_workspace_bytes(byref(self._w), n_mol, n, bounds)
-        if wbytes < 0:
-            check(int(wbytes), "nb200_gemnet_oc_workspace_bytes")
-        self.last_workspace_bytes = int(wbytes)
-        gbuf, ws = self._buffer("_graph_buf", gbytes, dev), self._buffer("_ws", wbytes, dev)
+        gbytes = self._bytes("nb200_gemnet_oc_graph_bytes", n, max_atoms_per_mol)
+        self.last_workspace_bytes = self._bytes("nb200_gemnet_oc_workspace_bytes", byref(self._w), n_mol, n, bounds)
+        gbuf, ws = self._buffer("_graph_buf", gbytes, dev), self._buffer("_ws", self.last_workspace_bytes, dev)
         if self._status is None or self._status.device != dev:
             self._status = torch.zeros(N_COUNTS, dtype=torch.int32, device=dev)
         energy = torch.empty(n_mol, dtype=torch.float32, device=dev)

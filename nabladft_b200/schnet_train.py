@@ -13,37 +13,35 @@ inference engine (csrc/schnet.cu).
 STATUS (round 1): first correct path, verified against the oracle's autograd under host emulation (tests/test_schnet_train_emu.py); not yet run
 on a device.  No CPU fallback: the product entry (`spk.NeuralNetworkPotential.forward`) accepts CUDA tensors only.
 """
-from ctypes import byref, c_int64, c_void_p
+from ctypes import byref, c_int64
 from typing import Dict, List, Optional
 
 import torch
 
-from ._lib import NablaB200Error, SchnetWeights, check
+from ._lib import EngineDriver, NablaB200Error, SchnetWeights, check
 
 GRAD_KEYS = ("emb", "w_f1", "b_f1", "W_f2", "b_f2", "I1", "P1", "p1", "P2", "p2", "R1", "e1", "R2", "e2")
 SCALAR_KEYS = ("n_layers", "n_feat", "n_rbf", "n_elem", "z_offset", "cutoff", "rbf_coeff", "energy_shift_per_atom")
 
 
-class SchnetTrainRunner:
-    """Host driver of `nb200_schnet_train_count` / `_workspace_bytes` / `nb200_schnet_energy_grads`; `lib` = bound libnabla_b200.so."""
+def count_edges(driver: EngineDriver, w: SchnetWeights, pos, mol_ptr, n_mol: int, ws_fn: str, *ws_args):
+    """The exact-count step of the SchNet training and Hessian calls: `nb200_schnet_train_count` (one host sync) builds the CSR row pointer
+    of the batch's graph in the driver's count buffer and returns its edge count, which sizes the workspace `ws_fn(w, n_mol, n_atoms, n_edges,
+    *ws_args)`.  -> (row_ptr, n_edges, workspace)."""
+    n, dev = int(pos.shape[0]), pos.device
+    off = (4 * (n + 1) + 255) // 256 * 256  # row_ptr [N + 1] int32, then scratch [2 N] int32 on its own 256-byte boundary
+    buf = driver._buffer("_count_buf", off + 8 * n, dev)
+    row_ptr, scratch = buf[:4 * (n + 1)].view(torch.int32), buf[off:off + 8 * n].view(torch.int32)
+    n_edges = c_int64(0)
+    check(driver.lib.nb200_schnet_train_count(byref(w), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, row_ptr.data_ptr(), scratch.data_ptr(),
+                                              byref(n_edges), driver._stream()), "nb200_schnet_train_count")
+    driver.last_edges = int(n_edges.value)
+    ws = driver._buffer("_ws", driver._bytes(ws_fn, byref(w), n_mol, n, n_edges.value, *ws_args), dev)
+    return row_ptr, n_edges.value, ws
 
-    def __init__(self, lib):
-        self.lib = lib
-        h = c_void_p()
-        check(lib.nb200_engine_create(byref(h)), "nb200_engine_create")
-        self._h = h
-        self._ws = None
 
-    def __del__(self):
-        try:
-            if self._h:
-                self.lib.nb200_engine_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
-    def _stream(self):
-        return c_void_p(torch.cuda.current_stream().cuda_stream)
+class SchnetTrainRunner(EngineDriver):
+    """Host driver of `nb200_schnet_train_count` / `_workspace_bytes` / `nb200_schnet_energy_grads`."""
 
     @staticmethod
     def _struct(tensors: Dict[str, torch.Tensor], scalars: Dict) -> SchnetWeights:
@@ -62,33 +60,18 @@ class SchnetTrainRunner:
         """-> (energy [B], grads or None).  grads: dict of fresh tensors shaped like the canonical weights,
         d(sum_m seed_m E_m + sum_i force_seed_i . F_i)/d(weight)."""
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        s = self._stream()
+        self._check_seeds(seed, force_seed, n_mol, n, dev)
         w = self._struct(tensors, scalars)
-        row_ptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
-        scratch = torch.empty(2 * n, dtype=torch.int32, device=dev)
-        n_edges = c_int64(0)
-        check(lib.nb200_schnet_train_count(byref(w), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, row_ptr.data_ptr(), scratch.data_ptr(), byref(n_edges), s),
-              "nb200_schnet_train_count")
-        need = lib.nb200_schnet_train_workspace_bytes(byref(w), n_mol, n, n_edges.value, int(force_seed is not None))
-        if need < 0:
-            check(int(need), "nb200_schnet_train_workspace_bytes")
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = None
-            self._ws = torch.empty(int(need * 1.1) + 256, dtype=torch.uint8, device=dev)
+        row_ptr, n_edges, ws = count_edges(self, w, pos, mol_ptr, n_mol, "nb200_schnet_train_workspace_bytes", int(force_seed is not None))
         energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
         grads = gw = None
-        if seed is not None and not (seed.dtype == torch.float32 and seed.is_contiguous() and seed.numel() == n_mol and seed.device == dev):
-            raise NablaB200Error("energy_grads(): seed must be a contiguous fp32 tensor [n_mol] on the batch's device")
-        if force_seed is not None and not (force_seed.dtype == torch.float32 and force_seed.is_contiguous() and force_seed.numel() == 3 * n
-                                           and force_seed.device == dev):
-            raise NablaB200Error("energy_grads(): force_seed must be a contiguous fp32 tensor [n_atoms, 3] on the batch's device")
         if seed is not None or force_seed is not None:
             grads = {k: torch.empty_like(tensors[k]) for k in GRAD_KEYS}
             gw = self._struct({**grads, "rbf_offsets": tensors["rbf_offsets"]}, scalars)
-        check(lib.nb200_schnet_energy_grads(self._h, byref(w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, row_ptr.data_ptr(), n_edges.value,
-                                            self._ws.data_ptr(), self._ws.numel(), seed.data_ptr() if seed is not None else None,
-                                            force_seed.data_ptr() if force_seed is not None else None, byref(gw) if gw is not None else None, energy.data_ptr(), s), "nb200_schnet_energy_grads")
-        self.last_edges = int(n_edges.value)
+        check(lib.nb200_schnet_energy_grads(self._h, byref(w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, row_ptr.data_ptr(), n_edges,
+                                            ws.data_ptr(), ws.numel(), seed.data_ptr() if seed is not None else None,
+                                            force_seed.data_ptr() if force_seed is not None else None, byref(gw) if gw is not None else None,
+                                            energy.data_ptr(), self._stream()), "nb200_schnet_energy_grads")
         return energy, grads
 
 

@@ -324,10 +324,9 @@ class NeuralNetworkPotential(nn.Module):
 
             if self._kind == "schnet":
                 if self._schnet_runner is None:
-                    from . import _lib as _l
                     from .schnet_train import SchnetTrainRunner
 
-                    self._schnet_runner = SchnetTrainRunner(_l.load())
+                    self._schnet_runner = SchnetTrainRunner()
                 return self._train_schnet_with(self._schnet_runner, eng, z, pos, mol_ptr, n_mol)
             if not self._forces:
                 raise NotImplementedError("training PaiNN through the CUDA path needs the Forces output module (config/model/painn.yaml)")

@@ -23,38 +23,12 @@ REL = 1e-4  # of max |H_ref| (of max |hv_ref| for single directions): the criter
 
 @pytest.fixture(scope="module")
 def emu():
-    from build_emu import build
+    from emu_driver import load, poisoned
 
-    from nabladft_b200.dimenetplusplus import DimeNetRunner, bind
+    from nabladft_b200.dimenetplusplus import DimeNetRunner
 
-    lib = ctypes.CDLL(build(name="dimenet"))
-    lib.nb200_engine_create.restype, lib.nb200_engine_create.argtypes = ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p)]
-    lib.nb200_engine_destroy.restype, lib.nb200_engine_destroy.argtypes = ctypes.c_int32, [ctypes.c_void_p]
-    lib.nb200_emu_check_guards.restype = ctypes.c_int32
-    bind(lib)
-
-    class EmuRunner(DimeNetRunner):  # host pointers, no streams
-        def _stream(self):
-            return None
-
-        def _buffer(self, attr, nbytes, device):
-            buf = super()._buffer(attr, nbytes, device)
-            buf.fill_(255)  # a kernel reading what it never wrote sees NaN floats / -1 indices
-            return buf
-
-        def _checked(self, call, *a, **kw):  # the registry is emptied while the buffers it points into are alive
-            lib.nb200_emu_check_guards()
-            out = call(*a, **kw)
-            checked = lib.nb200_emu_check_guards()
-            assert checked < 0, f"{checked} guard zones behind workspace arrays were overwritten" if checked > 0 else "no guard zones registered"
-            return out
-
-        def run_hvp(self, *a, **kw):
-            return self._checked(super().run_hvp, *a, **kw)
-
-        def run(self, *a, **kw):
-            return self._checked(super().run, *a, **kw)
-
+    lib = load("dimenet", ["nb200_dimenet_"])
+    EmuRunner = poisoned(DimeNetRunner, checked=["run_hvp", "run"])
     return lambda: EmuRunner(lib), lib
 
 

@@ -22,32 +22,12 @@ REL = 1e-4  # of max |g_ref| of each tensor
 
 @pytest.fixture(scope="module")
 def emu():
-    from build_emu import build
+    from emu_driver import load, poisoned
 
-    from nabladft_b200.dimenetplusplus import DimeNetRunner, bind
+    from nabladft_b200.dimenetplusplus import DimeNetRunner
 
-    lib = ctypes.CDLL(build(name="dimenet"))
-    lib.nb200_engine_create.restype, lib.nb200_engine_create.argtypes = ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p)]
-    lib.nb200_engine_destroy.restype, lib.nb200_engine_destroy.argtypes = ctypes.c_int32, [ctypes.c_void_p]
-    lib.nb200_emu_check_guards.restype = ctypes.c_int32
-    bind(lib)
-
-    class EmuRunner(DimeNetRunner):  # host pointers, no streams
-        def _stream(self):
-            return None
-
-        def _buffer(self, attr, nbytes, device):
-            buf = super()._buffer(attr, nbytes, device)
-            buf.fill_(255)  # a kernel reading what it never wrote sees NaN floats / -1 indices
-            return buf
-
-        def train_grads(self, *a, **kw):
-            lib.nb200_emu_check_guards()
-            out = super().train_grads(*a, **kw)
-            checked = lib.nb200_emu_check_guards()
-            assert checked < 0, f"{checked} guard zones behind workspace arrays were overwritten" if checked > 0 else "no guard zones registered"
-            return out
-
+    lib = load("dimenet", ["nb200_dimenet_"])
+    EmuRunner = poisoned(DimeNetRunner, checked=["train_grads"])
     return lambda: EmuRunner(lib), lib
 
 

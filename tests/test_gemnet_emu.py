@@ -3,7 +3,6 @@ functors the GPU launches, run as loops, driven through the SAME C ABI and the S
 two-phase graph/workspace protocol), compared with the pinned oracle (oracle/gemnet_oc.py) and the golden outputs of the reference's own
 classes.  This validates index logic, bases, weight layout and scale folding without a GPU; it says nothing about launch configuration or the
 tensor-core GEMM, which only `-m gpu` covers.  The emulation library is test infrastructure -- the package never loads it."""
-import ctypes
 import os
 import sys
 
@@ -18,39 +17,12 @@ sys.path.insert(0, os.path.join(HERE, "emu"))
 
 @pytest.fixture(scope="module")
 def emu():
-    from build_emu import build
+    from emu_driver import load, poisoned
 
-    from nabladft_b200.gemnet_oc import GemNetOCRunner, bind
+    from nabladft_b200.gemnet_oc import GemNetOCRunner
 
-    lib = ctypes.CDLL(build())
-    lib.nb200_engine_create.restype, lib.nb200_engine_create.argtypes = ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p)]
-    lib.nb200_engine_destroy.restype, lib.nb200_engine_destroy.argtypes = ctypes.c_int32, [ctypes.c_void_p]
-    bind(lib)
-
-    class EmuRunner(GemNetOCRunner):  # the emulation build takes host pointers and has no streams
-        def _stream(self):
-            return None
-
-        def _buffer(self, attr, nbytes, device):
-            # device memory comes back uninitialised; fresh CPU pages are zero.  Poison every (re)used buffer with 0xFF bytes (NaN floats,
-            # -1 indices) so that a kernel reading something it never wrote shows up here and not only on the GPU
-            buf = super()._buffer(attr, nbytes, device)
-            buf.fill_(255)
-            return buf
-
-        def _checked(self, out):
-            checked = lib.nb200_emu_check_guards()  # > 0: a kernel wrote past the end of one of its workspace arrays
-            assert checked < 0, f"{checked} guard zones behind workspace arrays were overwritten" if checked > 0 else "no guard zones were registered"
-            return out
-
-        def run(self, *a, **kw):
-            lib.nb200_emu_check_guards()  # forget zones registered by direct C-ABI calls of other tests (their buffers are gone)
-            return self._checked(super().run(*a, **kw))
-
-        def run_train(self, *a, **kw):
-            lib.nb200_emu_check_guards()
-            return self._checked(super().run_train(*a, **kw))
-
+    lib = load("gemnet_oc", ["nb200_gemnet_oc_"])
+    EmuRunner = poisoned(GemNetOCRunner, checked=["run", "run_train"])
     return lambda: EmuRunner(lib)
 
 

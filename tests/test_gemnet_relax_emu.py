@@ -2,7 +2,6 @@
 the engine source (tests/emu): bounds against real counts on adversarial geometries, bitwise agreement with the two-phase call, dead rows,
 the error path of a bound that is too small, and the relaxation loop against the float64 oracle.  Workspaces are poisoned before every call
 and the guard zones behind every workspace array are checked after it.  The device run of the same code is tests/test_gpu_gemnet_relax.py."""
-import ctypes
 import os
 import sys
 from ctypes import byref, c_int32, c_int64
@@ -18,41 +17,13 @@ from test_gemnet_emu import _models  # noqa: E402
 
 
 @pytest.fixture(scope="module")
-def emu_lib():
-    from build_emu import build
+def runner():
+    from emu_driver import load, poisoned
 
-    from nabladft_b200.gemnet_oc import bind
-
-    lib = ctypes.CDLL(build())
-    lib.nb200_engine_create.restype, lib.nb200_engine_create.argtypes = ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p)]
-    lib.nb200_engine_destroy.restype, lib.nb200_engine_destroy.argtypes = ctypes.c_int32, [ctypes.c_void_p]
-    return bind(lib)
-
-
-@pytest.fixture(scope="module")
-def runner(emu_lib):
     from nabladft_b200.gemnet_oc import GemNetOCRunner
 
-    class EmuRunner(GemNetOCRunner):  # host pointers, no streams; every (re)used buffer is filled with `fill` bytes before the call
-        fill = 255
-
-        def _stream(self):
-            return None
-
-        def _buffer(self, attr, nbytes, device):
-            buf = super()._buffer(attr, nbytes, device)
-            buf.fill_(self.fill)
-            return buf
-
-        def guarded(self, fn, *a, **kw):
-            self.lib.nb200_emu_check_guards()  # forget zones of earlier calls
-            out = fn(*a, **kw)
-            checked = self.lib.nb200_emu_check_guards()
-            assert checked < 0, f"{checked} guard zones behind workspace arrays were overwritten" if checked > 0 else "no guard zones were registered"
-            return out
-
     net, _ = _models(True)
-    r = EmuRunner(emu_lib)
+    r = poisoned(GemNetOCRunner)(load("gemnet_oc", ["nb200_gemnet_oc_"]))
     r.set_weights(net, torch.device("cpu"))
     return r
 
@@ -260,10 +231,9 @@ def test_engine_adapter_host_logic(runner):
 
 def test_c_abi_argument_checks_of_the_async_entry_and_exported_symbols(runner):
     from nabladft_b200 import _lib
-    from nabladft_b200.gemnet_oc import SIGNATURES
 
     for name in ("nb200_gemnet_oc_count_bounds", "nb200_gemnet_oc_energy_forces_async"):
-        assert name in SIGNATURES and hasattr(runner.lib, name) and hasattr(_lib.load(), name)
+        assert name in _lib.SIGNATURES and hasattr(runner.lib, name) and hasattr(_lib.load(), name)
     hdr = open(os.path.join(HERE, "..", "include", "nabla_b200.h")).read()
     assert "int nb200_gemnet_oc_count_bounds(" in hdr and "int nb200_gemnet_oc_energy_forces_async(" in hdr
     real = _lib.load()  # the pure host function of the CUDA library agrees with the emulation build

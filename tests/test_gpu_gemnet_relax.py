@@ -12,6 +12,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+sys.path.insert(0, os.path.join(HERE, "emu"))
 from test_gemnet_emu import _models  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -49,18 +50,11 @@ def model():
 
 @pytest.fixture()
 def runner(model):
-    from nabladft_b200 import _lib
-    from nabladft_b200.gemnet_oc import GemNetOCRunner, bind
+    from emu_driver import poisoned
 
-    class PoisonRunner(GemNetOCRunner):  # every (re)used buffer is filled with `fill` bytes before the call
-        fill = 255
+    from nabladft_b200.gemnet_oc import GemNetOCRunner
 
-        def _buffer(self, attr, nbytes, device):
-            buf = super()._buffer(attr, nbytes, device)
-            buf.fill_(self.fill)
-            return buf
-
-    r = PoisonRunner(bind(_lib.load()))
+    r = poisoned(GemNetOCRunner, emulated=False)()  # every (re)used buffer is filled with `fill` bytes before the call
     r.set_weights(model[0], torch.device(DEV))
     return r
 

@@ -288,10 +288,7 @@ def test_two_call_training_c_abi_argument_checks():
     assert lib.nb200_painn_train_forward(h, byref(w), _lib.ptr(zz), _lib.ptr(pp), _lib.ptr(mp), n_mol, n_atoms, e_cap, _lib.ptr(ws), 1024, 1,
                                          _lib.ptr(en), _lib.ptr(fo), _lib.ptr(st), _lib.current_stream()) == EINVAL
     # backward with a force seed although the workspace was sized without the tangent pass
-    grads = {k: torch.empty_like(eng._keep[k]) for k in eng.GRAD_KEYS}
-    gw = eng._wtype()
-    for k in eng._wkeys:
-        setattr(gw, k, grads[k].data_ptr() if k in grads else eng._keep[k].data_ptr())
+    grads, gw = eng._grad_struct()
     seed = torch.ones(n_mol, device=dev())
     assert lib.nb200_painn_train_backward(h, byref(w), _lib.ptr(zz), _lib.ptr(mp), n_mol, n_atoms, e_cap, _lib.ptr(ws), ws.numel(), 0, _lib.ptr(seed),
                                           _lib.ptr(fo), byref(gw), _lib.ptr(st), _lib.current_stream()) == EINVAL

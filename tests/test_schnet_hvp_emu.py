@@ -2,7 +2,6 @@
 through the product's own host code (`PainnEngine.run_hvp`, `vibrations.hessians_from_hvp`) against the float64 double backward of the oracle
 (oracle/spk.py).  As tests/test_schnet_train_emu.py: this validates the arithmetic and the host plumbing, not the launch configuration; every
 call poisons the reused workspace and checks the guard zones behind its sub-buffers."""
-import ctypes
 import os
 import sys
 
@@ -19,18 +18,9 @@ N_INTERACTIONS = 3
 
 @pytest.fixture(scope="module")
 def lib():
-    from build_emu import build
+    from emu_driver import load
 
-    from nabladft_b200 import _lib
-
-    lib = ctypes.CDLL(build(name="schnet_train"))
-    lib.nb200_engine_create.restype, lib.nb200_engine_create.argtypes = ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p)]
-    lib.nb200_engine_destroy.restype, lib.nb200_engine_destroy.argtypes = ctypes.c_int32, [ctypes.c_void_p]
-    for name, (res, args) in _lib.SIGNATURES.items():
-        if name.startswith(("nb200_schnet_train", "nb200_schnet_hvp")):
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-    return lib
+    return load("schnet_train", ["nb200_schnet_train", "nb200_schnet_hvp"])
 
 
 @pytest.fixture(scope="module")
@@ -55,27 +45,13 @@ def models():
 @pytest.fixture(scope="module")
 def engine(lib, models):
     """The product's SchNet engine on the emulation library: host tensors, no streams."""
+    from emu_driver import poisoned
+
     from nabladft_b200.engine import PainnEngine
     from nabladft_b200.schnet_train import SchnetTrainRunner
 
-    class EmuEngine(PainnEngine):
-        def _on_device(self, t):
-            return True
-
-        def _stream(self):
-            return None
-
-        def _run_schnet_hvp(self, *a, **kw):
-            if self._ws is not None:
-                self._ws.fill_(255)  # poison the reused workspace (NaN floats, -1 indices): device memory is never zero for free
-            lib.nb200_emu_check_guards()  # forget stale zones
-            out = super()._run_schnet_hvp(*a, **kw)
-            checked = lib.nb200_emu_check_guards()  # > 0: a kernel wrote past the end of one of its workspace arrays
-            assert checked < 0, f"{checked} guard zones behind workspace arrays were overwritten" if checked > 0 else "no guard zones were registered"
-            return out
-
     m, _ = models
-    eng = EmuEngine("schnet", lib=lib)
+    eng = poisoned(PainnEngine, checked=["run_hvp"])("schnet", lib=lib)
     tensors, scalars = m._export_schnet(postprocess=True)
     eng._weights, eng._keep = SchnetTrainRunner._struct(tensors, scalars), tensors  # set_weights() takes CUDA tensors only
     return eng

@@ -2,7 +2,6 @@
 by the product's own host code (`spk.NeuralNetworkPotential._train_schnet_with`, `schnet_train.SchnetEnergyFn`), against the autograd of the
 oracle (oracle/spk.py) in float64 for EVERY schnetpack-named parameter.  Same caveat as tests/test_gemnet_emu.py: this validates the arithmetic
 and the autograd plumbing, not the launch configuration; the emulation library is test infrastructure and is never loaded by the package."""
-import ctypes
 import os
 import sys
 
@@ -18,33 +17,12 @@ from helpers import load_fixture, load_golden_weights  # noqa: E402
 
 @pytest.fixture(scope="module")
 def runner():
-    from build_emu import build
+    from emu_driver import load, poisoned
 
-    from nabladft_b200 import _lib
     from nabladft_b200.schnet_train import SchnetTrainRunner
 
-    lib = ctypes.CDLL(build(name="schnet_train"))
-    lib.nb200_engine_create.restype, lib.nb200_engine_create.argtypes = ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p)]
-    lib.nb200_engine_destroy.restype, lib.nb200_engine_destroy.argtypes = ctypes.c_int32, [ctypes.c_void_p]
-    for name, (res, args) in _lib.SIGNATURES.items():
-        if name.startswith("nb200_schnet_train") or name == "nb200_schnet_energy_grads":
-            fn = getattr(lib, name)
-            fn.restype, fn.argtypes = res, args
-
-    class EmuRunner(SchnetTrainRunner):  # host pointers, no streams
-        def _stream(self):
-            return None
-
-        def energy_grads(self, *a, **kw):
-            if self._ws is not None:
-                self._ws.fill_(255)  # poison the reused workspace (NaN floats, -1 indices): device memory is never zero for free
-            lib.nb200_emu_check_guards()  # forget stale zones
-            out = super().energy_grads(*a, **kw)
-            checked = lib.nb200_emu_check_guards()  # > 0: a kernel wrote past the end of one of its workspace arrays
-            assert checked < 0, f"{checked} guard zones behind workspace arrays were overwritten" if checked > 0 else "no guard zones were registered"
-            return out
-
-    return EmuRunner(lib)
+    lib = load("schnet_train", ["nb200_schnet_train", "nb200_schnet_energy_grads"])
+    return poisoned(SchnetTrainRunner, checked=["energy_grads"])(lib)
 
 
 def _models(with_forces: bool, n_interactions=6):
