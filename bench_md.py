@@ -5,7 +5,10 @@
 per thermostat, the integrator's and the engine's kernel time per step (torch.profiler, separate run), host synchronisations per chunk and, with
 `--batch1`, the same at one molecule.  `--host-loop` times the shape of the reference's ASE loop on the same engine: per step a D2H copy of
 the forces, a numpy velocity-Verlet step and an H2D copy of the positions.  Secondary benchmark (the headline is bench.py); prints one
-JSON line with the card's name and power limit."""
+JSON line with the card's name and power limit.  `--model dimenetplusplus` runs DimeNet++ (config/model/dimenetplusplus.yaml, seeded
+test weights) at batch 32 and 256: the device loop (asynchronous forward sized by per-batch bounds) against the same loop with the two-phase
+forward, which waits for the counts, at every step, plus one forward of each at the start geometry, the counts over their bounds at the start
+and at the end, and the workspace sizes."""
 import argparse
 import json
 import os
@@ -169,6 +172,47 @@ def host_loop(calc, atoms, steps, warmup):
     return {"steps_per_s": rate, "molecule_steps_per_s": rate * len(atoms), "ms_per_step": 1e3 / rate, "host_syncs_per_step": 1}
 
 
+def dimenet_main(args):
+    import numpy as np
+    import torch
+
+    from bench_opt import dimenet_forward_compare, dimenet_model, dimenet_sync_calculator
+    from nabladft_b200.md import BatchwiseMD
+    from nabladft_b200.optimization import PyGBatchwiseCalculator, SimpleAtoms
+    from nabladft_b200.synth import synth_batch
+
+    dev = torch.device("cuda:0")
+    net = dimenet_model(dev)
+    out = {"metric": "MD steps/sec (DimeNet++ E+F + one integrator launch, B molecules per step), NVE", "steps": args.steps,
+           "check_every": args.check_every, "time_step_fs": 0.5, "card": card(), "data": "synthetic, seeded test weights",
+           "timing": "host wall clock around BatchwiseMD.run_md ending in a device synchronise; arms alternated", "batches": []}
+    for batch in args.batches:
+        b = synth_batch(1, batch)
+        p = b["mol_ptr"]
+        atoms = [SimpleAtoms(b["pos"][p[i]:p[i + 1]].astype(np.float64), b["z"][p[i]:p[i + 1]]) for i in range(batch)]
+        arms = {"device_loop": PyGBatchwiseCalculator(net, device=dev, energy_unit="Hartree", position_unit="Ang"),
+                "sync_forward_per_step": dimenet_sync_calculator()(net, device=dev, energy_unit="Hartree", position_unit="Ang")}
+        row = {"batch": batch, "atoms": int(p[-1]), "start_geometry": dimenet_forward_compare(arms["device_loop"], atoms)}
+        for k, calc in arms.items():
+            md = BatchwiseMD(calc, atoms, seed=0, check_every=args.check_every)
+            md.init_md("bench", time_step=0.5, temp_init=300, interval=10 ** 9)
+            md.run_md(args.warmup)
+            torch.cuda.synchronize()
+            syncs0 = md.host_syncs
+            t0 = time.perf_counter()
+            md.run_md(args.steps)
+            torch.cuda.synchronize()
+            dt = time.perf_counter() - t0
+            row[k] = {"ms_per_step": dt / args.steps * 1e3, "steps_per_s": args.steps / dt, "molecule_steps_per_s": args.steps * batch / dt,
+                      "host_syncs_of_the_loop": md.host_syncs - syncs0, "host_syncs_inside_each_forward": 0 if k == "device_loop" else 1}
+            if k == "device_loop":
+                st = md._eng.runner._status.cpu().tolist()
+                bnd = md._eng.bounds
+                row["count_over_bound_at_the_end"] = {"edges": round(st[0] / max(1, bnd["edges"]), 4), "triplets": round(st[4] / max(1, bnd["triplets"]), 4)}
+        out["batches"].append(row)
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=256)
@@ -177,7 +221,11 @@ def main():
     ap.add_argument("--check-every", type=int, default=50)
     ap.add_argument("--host-loop", action="store_true")
     ap.add_argument("--batch1", action="store_true", help="also time one molecule (the first of the batch)")
+    ap.add_argument("--model", choices=["painn", "dimenetplusplus"], default="painn")
+    ap.add_argument("--batches", type=int, nargs="+", default=[32, 256], help="dimenetplusplus: batch sizes to run")
     args = ap.parse_args()
+    if args.model == "dimenetplusplus":
+        return dimenet_main(args)
     import numpy as np
     import torch
 

@@ -8,8 +8,11 @@ Secondary benchmark (the driver's headline is bench.py); prints one JSON line.
 `--model gemnet-oc` relaxes with GemNet-OC (reference job config/gemnet-oc_optim.yaml) at batch 32 and 256 and alternates two arms in one
 process: the device loop (asynchronous forward sized by per-batch upper bounds, one host look per `check_every` steps) and the same loop with
 the synchronous two-phase forward (`GemNetOCRunner.run`, which waits for the edge counts) at every step.  It also reports the host
-synchronisations of a run, real count / bound of the five edge counts, the workspace size, and the card's name and power limit."""
+synchronisations of a run, real count / bound of the five edge counts, the workspace size, and the card's name and power limit.
+`--model dimenetplusplus` does the same for DimeNet++ (config/model/dimenetplusplus.yaml, seeded test weights), and also times one
+asynchronous against one two-phase forward at the start geometry with CUDA events."""
 import argparse
+from ctypes import c_int64
 import json
 import os
 import sys
@@ -106,11 +109,144 @@ def gemnet_main(args):
     print(json.dumps(out))
 
 
+def card_and_power():
+    import subprocess
+
+    import torch
+
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30)
+        name, power = (v.strip() for v in q.stdout.strip().split(","))
+    except Exception as exc:  # noqa: BLE001
+        name, power = torch.cuda.get_device_name(0), f"unavailable ({exc})"
+    return name, power
+
+
+def dimenet_model(dev, postprocessing=True):
+    """DimeNet++ of config/model/dimenetplusplus-b200.yaml with the seeded test weights (tests/golden/make_golden_dimenet.py)."""
+    import torch
+    import yaml
+    from make_golden_dimenet import load_test_weights
+
+    from nabladft_b200.dimenetplusplus import DimeNetPlusPlusPotential
+
+    cfg = yaml.safe_load(open(os.path.join(ROOT, "config", "model", "dimenetplusplus-b200.yaml")))["net"]
+    cfg.pop("_target_")
+    cfg["do_postprocessing"] = postprocessing
+    net = DimeNetPlusPlusPotential(**cfg).eval()
+    load_test_weights(net, torch.float32)
+    return net.to(dev)
+
+
+def dimenet_sync_calculator():
+    """A `PyGBatchwiseCalculator` whose engine runs the two-phase forward (`DimeNetRunner.run`, which waits for the edge and triplet counts)
+    at every step: the comparison arm of the device loops."""
+    import torch
+
+    from nabladft_b200.dimenetplusplus import DimeNetEngine
+    from nabladft_b200.optimization import PyGBatchwiseCalculator
+
+    class SyncEngine(DimeNetEngine):
+        def launch(self, z, pos, mol_ptr, n_mol, e_cap=None):
+            energy, forces, _ = self.runner.run(z, pos, mol_ptr, n_mol)
+            return energy, forces, torch.zeros(8, dtype=torch.int32, device=pos.device)
+
+    class SyncCalculator(PyGBatchwiseCalculator):
+        def engine(self):
+            if getattr(self, "_sync_engine", None) is None:
+                self._sync_engine = SyncEngine(self.model, self.model._get_runner())
+            return self._sync_engine
+
+    return SyncCalculator
+
+
+def dimenet_forward_compare(calc, atoms, n=10):
+    """One asynchronous forward against one two-phase forward at the start geometry (CUDA events around n calls each, alternated in three
+    rounds, the best round), the counts against the bounds and both workspaces."""
+    from ctypes import byref
+
+    import torch
+
+    eng = calc.engine()
+    z, pos, mol_ptr, sizes = calc.pack(atoms)
+    pos = pos.float().contiguous()
+    _, _, st = eng.run(z, pos, mol_ptr, len(sizes))
+    r = eng.runner
+    r.run(z, pos, mol_ptr, len(sizes))
+    counts = (c_int64 * 4)(r.last_counts["edges"], r.last_counts["triplets"], 0, 0)
+    ws_exact = r._bytes("nb200_dimenet_workspace_bytes", byref(r._w), len(sizes), int(z.shape[0]), counts)
+    arms = {"async": lambda: eng.launch(z, pos, mol_ptr, len(sizes)), "two_phase": lambda: r.run(z, pos, mol_ptr, len(sizes))}
+    best = {k: float("inf") for k in arms}
+    for _ in range(3):
+        for k, fn in arms.items():
+            fn()
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            for _ in range(n):
+                fn()
+            b.record()
+            b.synchronize()
+            best[k] = min(best[k], a.elapsed_time(b) / n)
+    return {"ms_per_async_forward": round(best["async"], 3), "ms_per_two_phase_forward": round(best["two_phase"], 3),
+            "edges": int(st[0]), "triplet_slots": int(st[4]), "bounds": eng.bounds,
+            "count_over_bound": {"edges": round(int(st[0]) / max(1, eng.bounds["edges"]), 4),
+                                 "triplets": round(int(st[4]) / max(1, eng.bounds["triplets"]), 4)},
+            "workspace_bytes_async": r.last_workspace_bytes, "workspace_bytes_two_phase": ws_exact}
+
+
+def dimenet_main(args):
+    import numpy as np
+    import torch
+
+    from nabladft_b200.optimization import ASEBatchwiseLBFGS, PyGBatchwiseCalculator, SimpleAtoms
+    from nabladft_b200.synth import synth_batch
+
+    dev = torch.device("cuda:0")
+    net = dimenet_model(dev)
+    name, power = card_and_power()
+    out = {"metric": "L-BFGS steps/sec (DimeNet++ E+F + batched L-BFGS, B molecules per step)", "card": name, "power_limit": power, "steps": args.steps,
+           "check_every": args.check_every, "memory": args.memory, "dtype": "f32 model / f64 positions", "data": "synthetic, seeded test weights",
+           "timing": "host wall clock around ASEBatchwiseLBFGS.run ending in a device synchronise; arms alternated, best of the repeats", "batches": []}
+    for batch in args.batches:
+        b = synth_batch(1, batch)
+        ptr = b["mol_ptr"]
+        atoms = [SimpleAtoms(b["pos"][ptr[m]:ptr[m + 1]], b["z"][ptr[m]:ptr[m + 1]]) for m in range(batch)]
+        arms = {"device_loop": PyGBatchwiseCalculator(net, device=dev, energy_unit="Hartree", position_unit="Ang"),
+                "sync_forward_per_step": dimenet_sync_calculator()(net, device=dev, energy_unit="Hartree", position_unit="Ang")}
+        row = {"batch": batch, "atoms": int(ptr[-1]), "start_geometry": dimenet_forward_compare(arms["device_loop"], atoms)}
+        opts = {k: ASEBatchwiseLBFGS(c, logfile=None, memory=args.memory, check_every=args.check_every) for k, c in arms.items()}
+        times = {k: [] for k in arms}
+        for k, o in opts.items():
+            o.run(atoms, fmax=1e-9, steps=3)  # warm-up
+        torch.cuda.synchronize()
+        for _ in range(args.repeats):
+            for k, o in opts.items():
+                o.initialize()
+                t0 = time.perf_counter()
+                o.run(atoms, fmax=1e-9, steps=args.steps)
+                torch.cuda.synchronize()
+                times[k].append(time.perf_counter() - t0)
+                if k == "device_loop":
+                    last = arms[k].engine().runner._status.cpu().tolist()
+        eng = arms["device_loop"].engine()
+        row["count_over_bound_at_the_final_geometry"] = {"edges": round(last[0] / max(1, eng.bounds["edges"]), 4),
+                                                          "triplets": round(last[4] / max(1, eng.bounds["triplets"]), 4)}
+        row["final_results_bitwise_equal_between_arms"] = bool(all(np.array_equal(arms["device_loop"].results[k], arms["sync_forward_per_step"].results[k])
+                                                                   for k in ("energy", "forces")))
+        for k, o in opts.items():
+            dt = min(times[k])
+            row[k] = {"steps_per_s": o.nsteps / dt, "molecule_steps_per_s": o.nsteps * batch / dt, "ms_per_step": dt / o.nsteps * 1e3,
+                      "all_runs_s": [round(t, 4) for t in times[k]], "host_syncs_of_the_loop": o.host_syncs,
+                      "host_syncs_inside_each_forward": 0 if k == "device_loop" else 1}
+        out["batches"].append(row)
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["painn", "gemnet-oc"], default="painn")
-    ap.add_argument("--batches", type=int, nargs="+", default=[32, 256], help="gemnet-oc: batch sizes to run")
-    ap.add_argument("--repeats", type=int, default=2, help="gemnet-oc: timed runs of each arm (alternated)")
+    ap.add_argument("--model", choices=["painn", "gemnet-oc", "dimenetplusplus"], default="painn")
+    ap.add_argument("--batches", type=int, nargs="+", default=[32, 256], help="gemnet-oc, dimenetplusplus: batch sizes to run")
+    ap.add_argument("--repeats", type=int, default=2, help="gemnet-oc, dimenetplusplus: timed runs of each arm (alternated)")
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--memory", type=int, default=100)
@@ -121,6 +257,8 @@ def main():
     args = ap.parse_args()
     if args.model == "gemnet-oc":
         return gemnet_main(args)
+    if args.model == "dimenetplusplus":
+        return dimenet_main(args)
     import numpy as np
     import torch
 

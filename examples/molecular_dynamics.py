@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Relax a batch of fixture molecules with the batched L-BFGS, equilibrate them with Langevin dynamics at 300 K, then run NVE and print
 each molecule's temperature and total-energy drift: the reference's `init_md` / `run_md` (PYGAseInterface, ASE dynamics of one molecule)
-for a whole batch on the GPU."""
+for a whole batch on the GPU.  `--model painn` (default: spk PaiNN) or `--model dimenetplusplus` (config/model/dimenetplusplus.yaml, run
+without postprocessing so that the logged total energy is the one the forces conserve, DESIGN.md 3.15.3)."""
 import argparse
 import os
 import sys
@@ -14,33 +15,48 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 from helpers import load_fixture, load_golden_weights  # noqa: E402
+from make_golden_dimenet import load_test_weights  # noqa: E402
 
 from nabladft_b200 import spk  # noqa: E402
 from nabladft_b200.md import BatchwiseMD  # noqa: E402
-from nabladft_b200.optimization import ASEBatchwiseLBFGS, SimpleAtoms, SpkBatchwiseCalculator  # noqa: E402
+from nabladft_b200.optimization import ASEBatchwiseLBFGS, PyGBatchwiseCalculator, SimpleAtoms, SpkBatchwiseCalculator  # noqa: E402
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--mols", type=int, nargs="+", default=[0, 3, 26, 99])
-    ap.add_argument("--weights", help="state dict of the spk PaiNN model (default: the seeded test weights)")
+    ap.add_argument("--model", choices=["painn", "dimenetplusplus"], default="painn")
+    ap.add_argument("--weights", help="state dict of the model (default: the seeded test weights)")
     ap.add_argument("--nvt-steps", type=int, default=2000)
     ap.add_argument("--nve-steps", type=int, default=2000)
     ap.add_argument("--workdir", help="write {name}_{i}.log (and .traj with ASE) here")
     a = ap.parse_args()
-    model = spk.NeuralNetworkPotential(
-        representation=spk.PaiNN(n_atom_basis=128, n_interactions=3, radial_basis=spk.GaussianRBF(n_rbf=100, cutoff=5.0),
-                                 cutoff_fn=spk.CosineCutoff(cutoff=5.0)),
-        input_modules=[spk.PairwiseDistances()], output_modules=[spk.Atomwise(n_in=128, output_key="energy"), spk.Forces()])
+    if a.model == "dimenetplusplus":
+        import yaml
+
+        from nabladft_b200.dimenetplusplus import DimeNetPlusPlusPotential
+
+        cfg = yaml.safe_load(open(os.path.join(ROOT, "config", "model", "dimenetplusplus-b200.yaml")))["net"]
+        cfg.pop("_target_")
+        cfg["do_postprocessing"] = False
+        model = DimeNetPlusPlusPotential(**cfg)
+    else:
+        model = spk.NeuralNetworkPotential(
+            representation=spk.PaiNN(n_atom_basis=128, n_interactions=3, radial_basis=spk.GaussianRBF(n_rbf=100, cutoff=5.0),
+                                     cutoff_fn=spk.CosineCutoff(cutoff=5.0)),
+            input_modules=[spk.PairwiseDistances()], output_modules=[spk.Atomwise(n_in=128, output_key="energy"), spk.Forces()])
     if a.weights:
         model.load_state_dict(torch.load(a.weights, map_location="cpu"), strict=True)
+    elif a.model == "dimenetplusplus":
+        load_test_weights(model, torch.float32)
     else:
         load_golden_weights(model, torch.float32)
     z, pos, batch = load_fixture(a.mols)
     sizes = torch.bincount(batch).tolist()
     off = np.concatenate([[0], np.cumsum(sizes)])
     atoms = [SimpleAtoms(pos[off[i]:off[i + 1]].numpy(), z[off[i]:off[i + 1]].numpy()) for i in range(len(sizes))]
-    calc = SpkBatchwiseCalculator(model, device="cuda:0", energy_unit="Hartree", position_unit="Ang")
+    calculator = PyGBatchwiseCalculator if a.model == "dimenetplusplus" else SpkBatchwiseCalculator
+    calc = calculator(model, device="cuda:0", energy_unit="Hartree", position_unit="Ang")
     opt = ASEBatchwiseLBFGS(calc, logfile=None)
     print(f"relaxation converged: {opt.run(atoms, fmax=1e-3, steps=1000)} after {opt.nsteps} steps")
 

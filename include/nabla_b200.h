@@ -190,6 +190,11 @@ int nb200_engine_set_node_backend(nb200_engine* eng, int32_t backend);
 int nb200_gemm_tf32x3(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B,
                       int32_t ldb, int32_t trans_b, float* C, int32_t ldc, int32_t accumulate,
                       const float* bias, float* act, void* stream);
+/* Test entry point: nb200_gemm_tf32x3 with the row count in device memory.  M is an upper bound: it sizes the grid and picks the kernel
+ * (the same choice as nb200_gemm_tf32x3 with that M); rows at or beyond min(M, *m_dev) are neither computed nor written.  m_dev == NULL:
+ * exactly nb200_gemm_tf32x3. */
+int nb200_gemm_tf32x3_rows(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb, int32_t trans_b,
+                           float* C, int32_t ldc, int32_t accumulate, const float* bias, float* act, const int32_t* m_dev, void* stream);
 /* Weight / bias gradient of a Linear layer (torch autograd: grad_weight = grad_out^T @ input, grad_bias = grad_out.sum(0); every
  * nn.Linear of nablaDFT/painn_pyg/painn.py), ACCUMULATED into dW / dbias:
  *   dW[out,in] += alpha * ( (c o G0)^T X0 + G1^T X1 ),   dbias[out] += bias_alpha * colsum(c o G0)
@@ -615,6 +620,23 @@ int64_t nb200_dimenet_workspace_bytes(const nb200_dimenet_weights* w, int32_t n_
 int nb200_dimenet_energy_forces(nb200_engine* eng, const nb200_dimenet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
                                 int32_t n_mol, int32_t n_atoms, void* graph_buf, int64_t graph_bytes, const int64_t* counts_host,
                                 void* workspace, int64_t workspace_bytes, float* energy, float* forces, float* graph_emb, void* stream);
+/* Asynchronous form for loops that must not wait for the host (relaxation, molecular dynamics): graph phase and energy-and-forces pass in
+ * ONE enqueue, no stream synchronisation, no device-to-host copy (DESIGN.md 3.15.3).
+ *   nb200_dimenet_count_bounds: pure host function; mol_ptr_host[n_mol + 1] -> bounds[NB200_DPP_C_COUNT] = {edges, triplet slots, 0, 0},
+ *   upper bounds that hold for every geometry of molecules of these sizes.  NB200_EINVAL for a mol_ptr that does not start at 0 or does not
+ *   increase, or a bound beyond int32.
+ *   nb200_dimenet_energy_forces_async: graph_bytes >= nb200_dimenet_graph_bytes(w, n_atoms), workspace_bytes >=
+ *   nb200_dimenet_workspace_bytes(w, n_mol, n_atoms, bounds).  Edge rows and GEMMs are sized by the bounds and stop at the counts, which stay
+ *   on the device; `status` is a device int32[8] rewritten by every call:
+ *     {edges, error code, max in-degree, atoms without a neighbour, triplet slots, 0, 0, 0}   (words 0-3 as nb200_painn_energy_forces)
+ *   Error codes in status[1]: NB200_ECAPACITY a count exceeds its bound, NB200_EINVAL z outside [0, 94] or a non-finite coordinate; both
+ *   are found before any edge or triplet row is written, nothing is written past a bound, and every energy and force of the call is NaN.
+ *   An atom without neighbours and a batch without edges are not errors.  Energies and forces are those of the two-phase form. */
+int nb200_dimenet_count_bounds(const nb200_dimenet_weights* w, const int32_t* mol_ptr_host, int32_t n_mol, int64_t* bounds);
+int nb200_dimenet_energy_forces_async(nb200_engine* eng, const nb200_dimenet_weights* w, const int32_t* z, const float* pos,
+                                      const int32_t* mol_ptr, int32_t n_mol, int32_t n_atoms, void* graph_buf, int64_t graph_bytes,
+                                      const int64_t* bounds, void* workspace, int64_t workspace_bytes, float* energy, float* forces,
+                                      int32_t* status, void* stream);
 /* Training (DESIGN.md 3.15.1): bytes of the workspace of nb200_dimenet_train_grads (the inference workspace plus the tangent arrays). */
 int64_t nb200_dimenet_train_workspace_bytes(const nb200_dimenet_weights* w, int32_t n_mol, int32_t n_atoms, const int64_t* counts_host);
 /* Parameter gradients of a loss L(E, F) (same z, pos, mol_ptr, graph buffer and counts as phase 1): given the seeds

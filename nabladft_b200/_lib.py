@@ -113,6 +113,8 @@ SIGNATURES = {
                             + [c_void_p] * 3 + [c_int32, c_int32] + [c_void_p] * 4 + [c_int32, c_void_p, c_void_p]),
     "nb200_gemm_tf32x3": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_int32,
                                     c_int32, c_void_p, c_void_p, c_void_p]),
+    "nb200_gemm_tf32x3_rows": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_int32,
+                                         c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_linear_wgrad": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32, c_float,
                                      c_void_p, c_float, c_void_p, c_int32, c_void_p]),
     "nb200_qh_expand_rows": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
@@ -184,6 +186,9 @@ SIGNATURES = {
     "nb200_dimenet_workspace_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32, c_int32, POINTER(c_int64)]),
     "nb200_dimenet_energy_forces": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
                                               POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_dimenet_count_bounds": (c_int32, [POINTER(DimeNetWeights), POINTER(c_int32), c_int32, POINTER(c_int64)]),
+    "nb200_dimenet_energy_forces_async": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
+                                                    c_int64, POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_dimenet_train_workspace_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32, c_int32, POINTER(c_int64)]),
     "nb200_dimenet_train_grads": (c_int32, [c_void_p, POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
                                             POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -137,8 +137,10 @@ __device__ __forceinline__ float actf_(float x, int kind) {
 // derivative w.r.t. the pre-activation: silu' or ssp' (= sigmoid)
 __device__ __forceinline__ float dactf_(float x, int kind) { return kind == NB_ACT_SSP ? sigmoidf_(x) : dsiluf_(x); }
 
+// m_dev (optional): the row count in device memory; M (an upper bound) still sizes the grid and picks the kernel, rows at or beyond
+// min(M, *m_dev) are neither computed nor written.  nullptr: exactly M rows.
 int nb_gemm_tf32x3_ex(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-                      const float* bias, float* act, int act_kind, cudaStream_t s);
+                      const float* bias, float* act, int act_kind, cudaStream_t s, const int32_t* m_dev = nullptr);
 int nb_bin_sort(const float* geom, const int32_t* status, float xscale, float inv_dx, int n_bins, int32_t* scratch, cudaStream_t s,
                 const int32_t* rev = nullptr);
 int nb_painn_filter_ex(const float* geom, const int32_t* status, int32_t e_stride, const float* w_rbf, const float* b_rbf, int32_t n_layers,
@@ -152,7 +154,7 @@ int nb_painn_msg_bwd_ex(const float* xh, const float* xh_bias, const float* mu, 
 bool nb_gemm_ps_wanted(int M, int N, int K);
 size_t nb_gemm_ps_ws_bytes(int N, int K);
 int nb_gemm_ps(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-               const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s);
+               const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, const int32_t* m_dev = nullptr);
 // epilogue forms of the pre-split-weight GEMM: 0 C = o (+ optional activation copy), 1 C = act(o) (Dense + activation, no pre-activation kept),
 // 2 C = (C + act(o)) * alpha (tail of a residual layer: C holds the layer input x)
 enum { NB_EPI_PLAIN = 0, NB_EPI_ACT = 1, NB_EPI_RESIDUAL = 2 };

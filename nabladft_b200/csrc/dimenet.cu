@@ -13,6 +13,10 @@
 // gather in a fixed order (no atomics), so two calls are bitwise equal.  Dense layers run on the wgmma 3xTF32 GEMM when the shape tiles
 // (every [E,256] and [E,64] layer), else on the functor GEMM.  Every kernel is a functor launched through pfor() (gemnet_pf.cuh), so the same
 // source builds for host emulation (tests/emu, name="dimenet").
+//
+// Two entries share the energy-and-forces pass (DESIGN.md 3.15.3): the two-phase call sizes every edge extent by the exact count it read back
+// from the graph phase; the asynchronous call sizes them by upper bounds that follow from the molecule sizes (nb200_dimenet_count_bounds),
+// leaves the counts on the device, and every edge-row launch and GEMM stops at the device count (Ext, gemnet_pf.cuh).
 #include "gemnet_pf.cuh"
 
 namespace {
@@ -159,6 +163,45 @@ struct TcntK {  // triplets of edge j -> i: edges into j except i -> j
 struct TotK {
     const int32_t* a; const int32_t* b; const int32_t* c; int32_t* tot;
     GD void operator()(int64_t) const { tot[0] = *a; tot[1] = *b; tot[2] = *c; }
+};
+// status words of the asynchronous call (include/nabla_b200.h): 1 error, 2 largest in-degree, 3 atoms without a source
+struct StatusAtomK {
+    const int32_t* bad; const int32_t* deg; int32_t* status;
+    GD void operator()(int64_t a) const {
+        if (bad[a]) atomicMin(status + 1, (int32_t)NB200_EINVAL);  // z outside [0, 94] or a non-finite coordinate (NbrK)
+        atomicMax(status + 2, deg[a]);
+        if (deg[a] == 0) atomicAdd(status + 3, 1);
+    }
+};
+struct StatusCountsK {  // one thread, after StatusAtomK: 0 edges, 4 triplet slots, both against their bounds
+    const int32_t* n_edges; const int32_t* n_slots; int32_t e_bound, t_bound; int32_t* status;
+    GD void operator()(int64_t) const {
+        const int32_t E = *n_edges, T = *n_slots;
+        status[0] = E;
+        status[4] = T;
+        if (status[1] == 0 && (E < 0 || E > e_bound || T < 0 || T > t_bound)) status[1] = NB200_ECAPACITY;  // < 0: int32 overflow of the scan
+    }
+};
+// after an error every CSR row (by target and by source) is empty and the device edge count is 0: no later kernel reaches an edge row
+struct ClearOnErrorK {
+    const int32_t* status; int32_t* ptr; int32_t* optr; int64_t n1;
+    GD void operator()(int64_t i) const {
+        if (status[1] == 0) return;
+        if (i < n1) ptr[i] = 0; else optr[i - n1] = 0;
+    }
+};
+GD float quiet_nan() {
+    const uint32_t u = 0x7fc00000u;
+    float x;
+    memcpy(&x, &u, 4);
+    return x;
+}
+struct NanOnErrorK {
+    const int32_t* status; float* energy; int64_t n_mol; float* forces;
+    GD void operator()(int64_t i) const {
+        if (status[1] == 0) return;
+        if (i < n_mol) energy[i] = quiet_nan(); else forces[i - n_mol] = quiet_nan();
+    }
 };
 
 // ------------------------------------------------------------------ bases
@@ -565,6 +608,16 @@ int config_rc(const nb200_dimenet_weights* w) {
     return NB200_OK;
 }
 
+#ifdef NB_EMU
+// host emulation of nb_gemm_tf32x3_ex with a device row count: the "device" count is readable here, so the emulated library GEMM
+// (goc_tc_gemm_ex) runs over min(M, *m_dev) rows and the rows beyond are not written
+inline int emu_gemm_rows(nb200_engine* e, cudaStream_t s, int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans, float* C,
+                         int ldc, int acc, const float* bias, const int32_t* m_dev) {
+    const int64_t rows = ext_rows(M, m_dev);
+    return rows > 0 ? goc_tc_gemm_ex(e, s, (int)rows, N, K, A, lda, B, ldb, trans, C, ldc, acc, bias) : NB200_OK;
+}
+#endif
+
 struct Ctx {
     nb200_engine* e; cudaStream_t s; const nb200_dimenet_weights* w;
     const float* G(int idx) const { return w->w + w->off_host[idx]; }
@@ -572,86 +625,90 @@ struct Ctx {
     const float* O(int blk, int idx) const {
         return w->w + w->off_host[NB200_DPP_G_COUNT + w->num_blocks * NB200_DPP_I_COUNT + blk * NB200_DPP_O_COUNT + idx];
     }
-    // C[M, N] (ldc = N) = (acc ? C : 0) + A[M, K] op(B) (+ bias); act != nullptr: act = silu(C) (C keeps the pre-activation)
-    int gemm(int64_t M, int N, int K, const float* A, const float* B, int trans, float* C, int acc, const float* bias, float* act) const {
+    // C[M, N] (ldc = N) = (acc ? C : 0) + A[M, K] op(B) (+ bias); act != nullptr: act = silu(C) (C keeps the pre-activation).
+    // Mx.dev set: Mx.n is the bound (grid, kernel choice), rows at or beyond the device count are neither computed nor written.
+    int gemm(Ext Mx, int N, int K, const float* A, const float* B, int trans, float* C, int acc, const float* bias, float* act) const {
+        const int64_t M = Mx.n;
         if (M <= 0) return NB200_OK;
         if (M > 0x7fffffff) return NB200_EUNSUPPORTED;
         const int ldb = trans ? N : K;
 #ifndef NB_EMU
         if (goc_tc_ok(N, K, K, ldb, N)) {
             Scope sc(e, s, CAT_GEMM, 1);
-            return nb_gemm_tf32x3_ex((int)M, N, K, A, K, B, ldb, trans, C, N, acc, bias, act, NB_ACT_SILU, s);
+            return nb_gemm_tf32x3_ex((int)M, N, K, A, K, B, ldb, trans, C, N, acc, bias, act, NB_ACT_SILU, s, Mx.dev);
         }
 #else
         if (goc_tc_ok(N, K, K, ldb, N)) {
-            NB_TRY(goc_tc_gemm_ex(e, s, (int)M, N, K, A, K, B, ldb, trans, C, N, acc, bias));
-            return act ? pfor(e, s, CAT_NODE, M * N, ActK{C, act}) : NB200_OK;
+            NB_TRY(emu_gemm_rows(e, s, (int)M, N, K, A, K, B, ldb, trans, C, N, acc, bias, Mx.dev));
+            return act ? pfor(e, s, CAT_NODE, Mx, N, ActK{C, act}) : NB200_OK;
         }
 #endif
-        NB_TRY(pfor(e, s, CAT_GEMM, M * N, GemmK{A, K, B, ldb, trans, C, N, N, K, acc, bias}));
-        return act ? pfor(e, s, CAT_NODE, M * N, ActK{C, act}) : NB200_OK;
+        NB_TRY(pfor(e, s, CAT_GEMM, Mx, N, GemmK{A, K, B, ldb, trans, C, N, N, K, acc, bias}));
+        return act ? pfor(e, s, CAT_NODE, Mx, N, ActK{C, act}) : NB200_OK;
     }
     // ResidualLayer: out = in + silu(W2 silu(W1 in + b1) + b2); keeps q1, q2 (pre-activations); tmp holds silu(q1)
-    int res_fwd(int64_t E, const float* in, int r, int blk, float* q1, float* q2, float* tmp, float* out) const {
+    int res_fwd(Ext E, const float* in, int r, int blk, float* q1, float* q2, float* tmp, float* out) const {
         const float* W = I(blk, NB200_DPP_I_RES_W) + (int64_t)2 * r * H * H;
         const float* b = I(blk, NB200_DPP_I_RES_B) + (int64_t)2 * r * H;
         NB_TRY(gemm(E, H, H, in, W, 0, q1, 0, b, tmp));
         NB_TRY(gemm(E, H, H, tmp, W + (int64_t)H * H, 0, q2, 0, b + H, nullptr));
-        return pfor(e, s, CAT_NODE, E * H, AddActK{in, q2, out});
+        return pfor(e, s, CAT_NODE, E, H, AddActK{in, q2, out});
     }
     // its reverse: gin = gout + ((gout * silu'(q2)) W2 * silu'(q1)) W1
-    int res_bwd(int64_t E, const float* gout, int r, int blk, const float* q1, const float* q2, float* t1, float* t2, float* gin) const {
+    int res_bwd(Ext E, const float* gout, int r, int blk, const float* q1, const float* q2, float* t1, float* t2, float* gin) const {
         const float* W = I(blk, NB200_DPP_I_RES_W) + (int64_t)2 * r * H * H;
-        NB_TRY(pfor(e, s, CAT_NODE, E * H, DActMulK{gout, q2, t1}));
+        NB_TRY(pfor(e, s, CAT_NODE, E, H, DActMulK{gout, q2, t1}));
         NB_TRY(gemm(E, H, H, t1, W + (int64_t)H * H, 1, t2, 0, nullptr, nullptr));
-        NB_TRY(pfor(e, s, CAT_NODE, E * H, DActMulK{t2, q1, t2}));
-        NB_TRY(goc_d2d(gin, gout, (size_t)E * H * sizeof(float), s));
+        NB_TRY(pfor(e, s, CAT_NODE, E, H, DActMulK{t2, q1, t2}));
+        NB_TRY(goc_d2d(gin, gout, (size_t)E.n * H * sizeof(float), s));  // whole extent: rows past the count are copied, never read
         return gemm(E, H, H, t2, W, 1, gin, 1, nullptr, nullptr);
     }
 };
 
+// E: the edge extent -- the exact count (Edev == nullptr), or the bound with the count in device memory at Edev (the asynchronous call)
 struct Geo {
-    const GraphBuf* g; int64_t n, E;
+    const GraphBuf* g; int64_t n, E; const int32_t* Edev = nullptr;
+    Ext e() const { return Ext(E, Edev); }
 };
 
 int interaction_fwd(const Ctx& c, const Work& w, const Geo& q, int blk, const float* x, float* out) {
-    const int64_t E = q.E;
+    const Ext E = q.e();
     const GraphBuf& g = *q.g;
     NB_TRY(c.gemm(E, H, H, x, c.I(blk, NB200_DPP_I_JI_W), 0, w.a, 0, c.I(blk, NB200_DPP_I_JI_B), w.h0));
     NB_TRY(c.gemm(E, H, H, x, c.I(blk, NB200_DPP_I_KJ_W), 0, w.bk, 0, c.I(blk, NB200_DPP_I_KJ_B), w.xk));
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * H, MulRbfK{w.xk, w.rbf, c.I(blk, NB200_DPP_I_RBF), w.t}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, H, MulRbfK{w.xk, w.rbf, c.I(blk, NB200_DPP_I_RBF), w.t}));
     NB_TRY(c.gemm(E, IE, H, w.t, c.I(blk, NB200_DPP_I_DOWN), 0, w.dpre, 0, nullptr, w.xd));
-    NB_TRY(pfor(c.e, c.s, CAT_MSG_FWD, E * IE, TripFwdK{g.ptr, g.src, g.tgt, w.V, w.d, w.rbs, c.I(blk, NB200_DPP_I_SBF), w.xd, w.agg}));
+    NB_TRY(pfor(c.e, c.s, CAT_MSG_FWD, E, IE, TripFwdK{g.ptr, g.src, g.tgt, w.V, w.d, w.rbs, c.I(blk, NB200_DPP_I_SBF), w.xd, w.agg}));
     NB_TRY(c.gemm(E, H, IE, w.agg, c.I(blk, NB200_DPP_I_UP), 0, w.upre, 0, nullptr, nullptr));
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * H, AddActK{w.h0, w.upre, w.h0}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, H, AddActK{w.h0, w.upre, w.h0}));
     NB_TRY(c.res_fwd(E, w.h0, 0, blk, w.q1[0], w.q2[0], w.t, w.h1));
     NB_TRY(c.gemm(E, H, H, w.h1, c.I(blk, NB200_DPP_I_LIN_W), 0, w.lpre, 0, c.I(blk, NB200_DPP_I_LIN_B), nullptr));
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * H, LinOutK{w.lpre, x, w.h2}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, H, LinOutK{w.lpre, x, w.h2}));
     NB_TRY(c.res_fwd(E, w.h2, 1, blk, w.q1[1], w.q2[1], w.t, w.h3));
     return c.res_fwd(E, w.h3, 2, blk, w.q1[2], w.q2[2], w.t, out);
 }
 
 // reverse of interaction block `blk` whose forward state is in the scratch: gO = dE/d(output) -> gI = dE/d(input), grbf / grbs / gct accumulate
 int interaction_bwd(const Ctx& c, const Work& w, const Geo& q, int blk, const float* gO, float* gI) {
-    const int64_t E = q.E;
+    const Ext E = q.e();
     const GraphBuf& g = *q.g;
     NB_TRY(c.res_bwd(E, gO, 2, blk, w.q1[2], w.q2[2], w.g2, w.g3, w.g1));   // g1 = d/dh3
     NB_TRY(c.res_bwd(E, w.g1, 1, blk, w.q1[1], w.q2[1], w.g2, w.g3, gI));   // gI = d/dh2 (the skip: d/dx starts here)
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * H, DActMulK{gI, w.lpre, w.g2}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, H, DActMulK{gI, w.lpre, w.g2}));
     NB_TRY(c.gemm(E, H, H, w.g2, c.I(blk, NB200_DPP_I_LIN_W), 1, w.g3, 0, nullptr, nullptr));  // d/dh1
     float* gh0 = w.t;  // the forward's t is not read by the reverse pass
     NB_TRY(c.res_bwd(E, w.g3, 0, blk, w.q1[0], w.q2[0], w.g1, w.g2, gh0));  // d/dh0 = d/dx_ji = d/dx_kj(up)
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * H, DActMulK{gh0, w.a, w.g1}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, H, DActMulK{gh0, w.a, w.g1}));
     NB_TRY(c.gemm(E, H, H, w.g1, c.I(blk, NB200_DPP_I_JI_W), 1, gI, 1, nullptr, nullptr));
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * H, DActMulK{gh0, w.upre, w.g2}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, H, DActMulK{gh0, w.upre, w.g2}));
     NB_TRY(c.gemm(E, IE, H, w.g2, c.I(blk, NB200_DPP_I_UP), 1, w.g64a, 0, nullptr, nullptr));  // d/dagg
-    NB_TRY(pfor(c.e, c.s, CAT_MSG_BWD, E * IE, TripBwdXK{g.ptr, g.src, g.tgt, g.optr, g.oeid, w.V, w.d, w.rbs, c.I(blk, NB200_DPP_I_SBF), w.g64a, w.g64b}));
-    NB_TRY(pfor(c.e, c.s, CAT_MSG_BWD, E, TripBwdGK{g.ptr, g.src, g.tgt, g.rev, g.optr, g.oeid, g.tptr, w.V, w.d, w.rbs, c.I(blk, NB200_DPP_I_SBF1),
+    NB_TRY(pfor(c.e, c.s, CAT_MSG_BWD, E, IE, TripBwdXK{g.ptr, g.src, g.tgt, g.optr, g.oeid, w.V, w.d, w.rbs, c.I(blk, NB200_DPP_I_SBF), w.g64a, w.g64b}));
+    NB_TRY(pfor(c.e, c.s, CAT_MSG_BWD, E, 1, TripBwdGK{g.ptr, g.src, g.tgt, g.rev, g.optr, g.oeid, g.tptr, w.V, w.d, w.rbs, c.I(blk, NB200_DPP_I_SBF1),
                                                    c.I(blk, NB200_DPP_I_SBF2), w.g64a, w.xd, w.grbs, w.gct}));
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * IE, DActMulK{w.g64b, w.dpre, w.g64b}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, IE, DActMulK{w.g64b, w.dpre, w.g64b}));
     NB_TRY(c.gemm(E, H, IE, w.g64b, c.I(blk, NB200_DPP_I_DOWN), 1, w.g3, 0, nullptr, nullptr));  // d/dt
-    NB_TRY(pfor(c.e, c.s, CAT_FILTER, E * NRAD, RbfBwdK{nullptr, w.g3, w.xk, c.I(blk, NB200_DPP_I_RBF), w.grbf}));
-    NB_TRY(pfor(c.e, c.s, CAT_NODE, E * H, KjBwdK{w.g3, w.rbf, c.I(blk, NB200_DPP_I_RBF), w.bk, w.g1}));
+    NB_TRY(pfor(c.e, c.s, CAT_FILTER, E, NRAD, RbfBwdK{nullptr, w.g3, w.xk, c.I(blk, NB200_DPP_I_RBF), w.grbf}));
+    NB_TRY(pfor(c.e, c.s, CAT_NODE, E, H, KjBwdK{w.g3, w.rbf, c.I(blk, NB200_DPP_I_RBF), w.bk, w.g1}));
     return c.gemm(E, H, H, w.g1, c.I(blk, NB200_DPP_I_KJ_W), 1, gI, 1, nullptr, nullptr);
 }
 
@@ -683,8 +740,8 @@ int output_bwd(const Ctx& c, const Work& w, const Geo& q, int blk, const float* 
         float* t = cur; cur = nxt; nxt = t;
     }
     NB_TRY(c.gemm(n, H, OE, cur, c.O(blk, NB200_DPP_O_UP), 1, w.oA, 0, nullptr, nullptr));  // d/dA
-    NB_TRY(pfor(c.e, c.s, CAT_READOUT, q.E * H, OutBwdXK{q.g->tgt, w.rbf, c.O(blk, NB200_DPP_O_RBF), w.oA, gx, acc}));
-    return pfor(c.e, c.s, CAT_FILTER, q.E * NRAD, RbfBwdK{q.g->tgt, w.oA, x, c.O(blk, NB200_DPP_O_RBF), w.grbf});
+    NB_TRY(pfor(c.e, c.s, CAT_READOUT, q.e(), H, OutBwdXK{q.g->tgt, w.rbf, c.O(blk, NB200_DPP_O_RBF), w.oA, gx, acc}));
+    return pfor(c.e, c.s, CAT_FILTER, q.e(), NRAD, RbfBwdK{q.g->tgt, w.oA, x, c.O(blk, NB200_DPP_O_RBF), w.grbf});
 }
 
 int graph_phase(nb200_engine* e, cudaStream_t s, const nb200_dimenet_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
@@ -718,17 +775,18 @@ int energy_forces_pass(const Ctx& c, const Work& wk, const Geo& q, const int32_t
     const nb200_dimenet_weights* w = c.w;
     const GraphBuf& g = *q.g;
     const int64_t E = q.E, n_atoms = q.n;
+    const Ext Ex = q.e();  // every edge-row launch and GEMM stops at the device count when there is one
     const int nb = w->num_blocks, L = w->node_latent_dim;
     const int64_t EH = E * H;
     const float inv_cut = 1.0f / w->cutoff;
     // geometry and bases
-    NB_TRY(pfor(eng, s, CAT_FILTER, E, GeomK{pos, g.src, g.tgt, wk.V, wk.d}));
-    NB_TRY(pfor(eng, s, CAT_FILTER, E * NRAD, RbfK{wk.d, c.G(NB200_DPP_G_FREQ), inv_cut, wk.rbf}));
-    NB_TRY(pfor(eng, s, CAT_FILTER, E * NSR, RbsK{wk.d, c.G(NB200_DPP_G_ZEROS), c.G(NB200_DPP_G_NORMS), inv_cut, wk.rbs, wk.drbs}));
+    NB_TRY(pfor(eng, s, CAT_FILTER, Ex, 1, GeomK{pos, g.src, g.tgt, wk.V, wk.d}));
+    NB_TRY(pfor(eng, s, CAT_FILTER, Ex, NRAD, RbfK{wk.d, c.G(NB200_DPP_G_FREQ), inv_cut, wk.rbf}));
+    NB_TRY(pfor(eng, s, CAT_FILTER, Ex, NSR, RbsK{wk.d, c.G(NB200_DPP_G_ZEROS), c.G(NB200_DPP_G_NORMS), inv_cut, wk.rbs, wk.drbs}));
     // embedding block
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, EmbRbfK{wk.rbf, c.G(NB200_DPP_G_EMB_RBF_W), c.G(NB200_DPP_G_EMB_RBF_B), wk.hr, wk.hra}));
-    NB_TRY(c.gemm(E, H, H, wk.hra, c.G(NB200_DPP_G_EMB_W3), 0, wk.epre, 0, nullptr, nullptr));
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, EmbAddK{z, g.src, g.tgt, c.G(NB200_DPP_G_EMB_TI), c.G(NB200_DPP_G_EMB_TJ), wk.epre, wk.X}));
+    NB_TRY(pfor(eng, s, CAT_EMBED, Ex, H, EmbRbfK{wk.rbf, c.G(NB200_DPP_G_EMB_RBF_W), c.G(NB200_DPP_G_EMB_RBF_B), wk.hr, wk.hra}));
+    NB_TRY(c.gemm(Ex, H, H, wk.hra, c.G(NB200_DPP_G_EMB_W3), 0, wk.epre, 0, nullptr, nullptr));
+    NB_TRY(pfor(eng, s, CAT_EMBED, Ex, H, EmbAddK{z, g.src, g.tgt, c.G(NB200_DPP_G_EMB_TI), c.G(NB200_DPP_G_EMB_TJ), wk.epre, wk.X}));
     // blocks
     NB_TRY(output_fwd(c, wk, q, 0, wk.X));
     for (int b = 0; b < nb; b++) {
@@ -756,13 +814,13 @@ int energy_forces_pass(const Ctx& c, const Work& wk, const Geo& q, const int32_t
         float* t = gx; gx = gprev; gprev = t;
     }
     // embedding block reverse: gx = d/dx0
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, DActMulK{gx, wk.epre, wk.g1}));
-    NB_TRY(c.gemm(E, H, H, wk.g1, c.G(NB200_DPP_G_EMB_W3), 1, wk.g2, 0, nullptr, nullptr));
-    NB_TRY(pfor(eng, s, CAT_EMBED, EH, DActMulK{wk.g2, wk.hr, wk.g2}));
-    NB_TRY(pfor(eng, s, CAT_FILTER, E * NRAD, RbfBwdK{nullptr, wk.g2, nullptr, c.G(NB200_DPP_G_EMB_RBF_W), wk.grbf}));
+    NB_TRY(pfor(eng, s, CAT_EMBED, Ex, H, DActMulK{gx, wk.epre, wk.g1}));
+    NB_TRY(c.gemm(Ex, H, H, wk.g1, c.G(NB200_DPP_G_EMB_W3), 1, wk.g2, 0, nullptr, nullptr));
+    NB_TRY(pfor(eng, s, CAT_EMBED, Ex, H, DActMulK{wk.g2, wk.hr, wk.g2}));
+    NB_TRY(pfor(eng, s, CAT_FILTER, Ex, NRAD, RbfBwdK{nullptr, wk.g2, nullptr, c.G(NB200_DPP_G_EMB_RBF_W), wk.grbf}));
     if (!forces) return NB200_OK;
     // geometry reverse and forces
-    NB_TRY(pfor(eng, s, CAT_FORCE, E, GeomBwdK{g.ptr, g.src, g.tgt, g.rev, g.optr, g.oeid, g.tptr, wk.V, wk.d, wk.rbf, c.G(NB200_DPP_G_FREQ), inv_cut,
+    NB_TRY(pfor(eng, s, CAT_FORCE, Ex, 1, GeomBwdK{g.ptr, g.src, g.tgt, g.rev, g.optr, g.oeid, g.tptr, wk.V, wk.d, wk.rbf, c.G(NB200_DPP_G_FREQ), inv_cut,
                                                wk.grbf, wk.drbs, wk.grbs, wk.gct, wk.gV}));
     return pfor(eng, s, CAT_FORCE, 3 * n_atoms, ForceK{g.ptr, g.optr, g.oeid, wk.gV, forces});
 }
@@ -822,6 +880,62 @@ extern "C" int nb200_dimenet_energy_forces(nb200_engine* eng, const nb200_dimene
     return energy_forces_pass(c, wk, q, z, pos, mol_ptr, n_mol, T, energy, forces, graph_emb);
 }
 
+// Upper bounds of the counts from the molecule sizes alone (DESIGN.md 3.15.3).  Every edge lives inside one molecule.  For a molecule of m
+// atoms and kcap = max_neighbors + 1, NbrK keeps the first kcap in-cutoff candidates of a target in index order, the target itself included
+// (d = 0), then drops it.  A target at position t < kcap of its molecule has at most t atoms before it, so it is always among its own first
+// kcap candidates and keeps at most min(m - 1, kcap - 1) sources; a later one keeps at most kcap.  Edge j -> i has indeg(j) - [i -> j
+// exists] triplet slots (TcntK); indeg(j) <= min(m - 1, kcap), and indeg(j) = m - 1 means every other atom, i included, is a source of j, so
+// an edge has at most min(m - 2, kcap) slots.  A compact molecule (every pair inside the cutoff) attains the edge bound, and for
+// m <= kcap the slot bound too.
+extern "C" int nb200_dimenet_count_bounds(const nb200_dimenet_weights* w, const int32_t* mol_ptr_host, int32_t n_mol, int64_t* bounds) {
+    NB_TRY(config_rc(w));
+    if (!mol_ptr_host || !bounds || n_mol < 1 || mol_ptr_host[0] != 0) return NB200_EINVAL;
+    const int64_t kcap = w->max_neighbors + 1;
+    int64_t E = 0, T = 0;
+    for (int32_t i = 0; i < n_mol; i++) {
+        const int64_t m = (int64_t)mol_ptr_host[i + 1] - mol_ptr_host[i];
+        if (m < 1) return NB200_EINVAL;
+        const int64_t lo = m < kcap ? m : kcap;  // targets among their own first kcap candidates
+        const int64_t e = lo * (m - 1 < kcap - 1 ? m - 1 : kcap - 1) + (m - lo) * kcap;
+        E += e;
+        T += m < 2 ? 0 : e * (m - 2 < kcap ? m - 2 : kcap);
+        if (E > 0x7fffffff || T > 0x7fffffff) return NB200_EINVAL;  // the row pointers (ptr, tptr) are int32 scans
+    }
+    if (!sizes_ok(n_mol, mol_ptr_host[n_mol], w->max_neighbors)) return NB200_EINVAL;
+    for (int k = 0; k < NB200_DPP_C_COUNT; k++) bounds[k] = 0;
+    bounds[NB200_DPP_C_EDGES] = E;
+    bounds[NB200_DPP_C_TRIPLETS] = T;
+    return NB200_OK;
+}
+
+// Graph phase and energy-and-forces pass in one enqueue: no host read, no synchronisation.  Edge extents are the bounds; the counts stay on
+// the device and are checked against the bounds before the pass writes any edge or triplet row.
+extern "C" int nb200_dimenet_energy_forces_async(nb200_engine* eng, const nb200_dimenet_weights* w, const int32_t* z, const float* pos,
+                                                 const int32_t* mol_ptr, int32_t n_mol, int32_t n_atoms, void* graph_buf, int64_t graph_bytes,
+                                                 const int64_t* bounds, void* workspace, int64_t workspace_bytes, float* energy, float* forces,
+                                                 int32_t* status, void* stream) {
+    NB_TRY(config_rc(w));
+    if (!eng || !z || !pos || !mol_ptr || !graph_buf || !bounds || !workspace || !energy || !forces || !status ||
+        !sizes_ok(n_mol, n_atoms, w->max_neighbors))
+        return NB200_EINVAL;
+    const int64_t kcap = w->max_neighbors + 1, Eb = bounds[NB200_DPP_C_EDGES], Tb = bounds[NB200_DPP_C_TRIPLETS];
+    if (Eb < 0 || Tb < 0 || Eb > (int64_t)n_atoms * kcap || Tb > 0x7fffffff || graph_bytes < carve_graph(nullptr, n_atoms, kcap).bytes ||
+        workspace_bytes < carve_work(nullptr, w->num_blocks, n_mol, n_atoms, Eb, Tb, w->node_latent_dim).bytes)
+        return NB200_EINVAL;  // before any pointer is formed
+    const GraphBuf g = carve_graph(graph_buf, n_atoms, kcap);
+    const Work wk = carve_work(workspace, w->num_blocks, n_mol, n_atoms, Eb, Tb, w->node_latent_dim);
+    cudaStream_t s = (cudaStream_t)stream;
+    NB_TRY(graph_phase(eng, s, w, z, pos, mol_ptr, n_mol, n_atoms, g));
+    NB_TRY(goc_memset(status, 0, 8 * sizeof(int32_t), s));
+    NB_TRY(pfor(eng, s, CAT_NBR, n_atoms, StatusAtomK{g.bad, g.deg, status}));
+    NB_TRY(pfor(eng, s, CAT_NBR, 1, StatusCountsK{g.ptr + n_atoms, g.tptr + g.emax, (int32_t)Eb, (int32_t)Tb, status}));
+    NB_TRY(pfor(eng, s, CAT_NBR, 2 * ((int64_t)n_atoms + 1), ClearOnErrorK{status, g.ptr, g.optr, (int64_t)n_atoms + 1}));
+    const Ctx c{eng, s, w};
+    const Geo q{&g, n_atoms, Eb, g.ptr + n_atoms};
+    NB_TRY(energy_forces_pass(c, wk, q, z, pos, mol_ptr, n_mol, Tb, energy, forces, nullptr));
+    return pfor(eng, s, CAT_READOUT, (int64_t)n_mol + 3 * (int64_t)n_atoms, NanOnErrorK{status, energy, n_mol, forces});
+}
+
 extern "C" int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, const float* dist, int32_t n, float* rbs, float* drbs, void* stream) {
     NB_TRY(config_rc(w));
     if (!dist || !rbs || !drbs || n < 0) return NB200_EINVAL;
@@ -833,6 +947,15 @@ extern "C" int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, co
     const Ctx c{e, (cudaStream_t)stream, w};
     return pfor(e, c.s, CAT_FILTER, (int64_t)n * NSR, RbsK{dist, c.G(NB200_DPP_G_ZEROS), c.G(NB200_DPP_G_NORMS), 1.0f / w->cutoff, rbs, drbs});
 }
+
+#ifdef NB_EMU
+// the test entry of gemm_tc.cu in the emulation build, on the emulated GEMM (no act output: the engine applies the activation separately)
+extern "C" int nb200_gemm_tf32x3_rows(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb, int32_t trans_b,
+                                      float* C, int32_t ldc, int32_t accumulate, const float* bias, float* act, const int32_t* m_dev, void* stream) {
+    if (!A || !B || !C || act || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
+    return emu_gemm_rows(nullptr, (cudaStream_t)stream, M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, m_dev);
+}
+#endif
 
 #include "dimenet_train.inc"
 #include "dimenet_hvp.inc"

@@ -53,6 +53,7 @@ struct GemmParams {
     float* C; int ldc, accumulate;
     const float* bias;
     float* act; int act_kind;
+    const int32_t* m_dev;         // optional row count in device memory (M is then the bound the grid is sized by)
 };
 
 // L (tc_pipe.cuh): OneGroup for K <= 128 and the lm path, TwoGroups for K > 128 (see gemm_ps_impl)
@@ -68,6 +69,11 @@ __global__ void __launch_bounds__(NTHREADS, CTAS_PER_SM) k_gemm_ps(const GemmPar
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int t_begin = blockIdx.y * P.tiles_per_cta, t_end = min(t_begin + P.tiles_per_cta, P.n_nt);
     if (t_begin >= t_end) return;
+    if (P.m_dev) {  // a slab wholly beyond the device row count: the whole CTA leaves before any mbarrier exists or bulk copy is issued
+        const int rows = min(P.M, *P.m_dev);
+        if ((int)blockIdx.x * L::NT >= rows) return;
+        P.M = rows;
+    }
     const int n_it = t_end - t_begin, KC = P.KC, n_units = n_it * KC;
     Ctx<L> c = setup<L>(smem, tid);
     // unit u = (N tile t_begin + u / KC, K chunk u % KC).  K <= 128: the activation slab is written once and stays; else once per unit.
@@ -165,7 +171,8 @@ bool nb_gemm_ps_wanted(int M, int N, int K) { return M >= 2048 && N >= 64 && K >
 
 // `ws` (>= nb_gemm_ps_ws_bytes(N, K)) may be NULL: a per-stream grow-only scratch owned by this translation unit is used then.
 static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-                        const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, int epi, float epi_alpha) {
+                        const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, int epi, float epi_alpha,
+                        const int32_t* m_dev = nullptr) {
     if (!A || !B || !C || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
     if (K % 4 || lda % 4 || ldc < N) return NB200_EUNSUPPORTED;
     if (M == 0) return NB200_OK;
@@ -183,6 +190,7 @@ static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const floa
     P.C = C; P.ldc = ldc; P.accumulate = accumulate; P.bias = bias; P.act = act; P.act_kind = act_kind;
     P.spt = KC == 1 ? (K + KSTAGE - 1) / KSTAGE : STAGES_PER_TILE;
     P.epi = epi; P.epi_alpha = epi_alpha;
+    P.m_dev = m_dev;
     static_assert(OneGroup::NT == TwoGroups::NT, "one row tiling for both layouts");
     const int m_tiles = (M + OneGroup::NT - 1) / OneGroup::NT;
     int ny = 1;
@@ -195,8 +203,8 @@ static int gemm_ps_impl(int M, int N, int K, const float* A, int lda, const floa
 }
 
 int nb_gemm_ps(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-               const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s) {
-    return gemm_ps_impl(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, ws, ws_bytes, s, NB_EPI_PLAIN, 1.0f);
+               const float* bias, float* act, int act_kind, void* ws, size_t ws_bytes, cudaStream_t s, const int32_t* m_dev) {
+    return gemm_ps_impl(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, ws, ws_bytes, s, NB_EPI_PLAIN, 1.0f, m_dev);
 }
 
 // Dense layer with a fused tail (GemNet-OC: Dense + ScaledSiLU in place; the (x + act(.)) / sqrt 2 tail of a ResidualLayer into x)

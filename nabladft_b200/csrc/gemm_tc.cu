@@ -17,6 +17,8 @@
 //   optional second output  act[M,N] = silu(C)   (C then holds the pre-activation)
 // k_gemm_tf32x3: tile 128 x 64 x 32, 512 threads = four warpgroups (each a 64 x 32 quarter of the tile), double-buffered stages with
 // register prefetch.  Tall problems go to the pre-split-weight kernel of gemm_ps.cu.
+// Optional device row count m_dev: M is an upper bound that sizes the grid; a CTA whose first row is at or beyond min(M, *m_dev) returns at
+// entry (no kernel here runs in clusters and this one has no mbarrier), the others stage zeros for and store nothing to the rows beyond it.
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -35,12 +37,18 @@ struct Stage {
 __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_tf32x3(int M, int N, int K, const float* __restrict__ A, int lda,
                                                              const float* __restrict__ B, int ldb, int trans_b, float* C, int ldc,
                                                              int accumulate, const float* __restrict__ bias, float* __restrict__ act, int act_kind,
-                                                             int batch_kind, long long a_boff, long long b_boff, long long c_boff) {
+                                                             int batch_kind, long long a_boff, long long b_boff, long long c_boff,
+                                                             const int32_t* __restrict__ m_dev) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     Stage* stages = reinterpret_cast<Stage*>(smem_raw);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.x * G_BM, n0 = blockIdx.y * G_BN;
+    if (m_dev) {  // uniform over the CTA, before its first barrier
+        const int rows = min(M, *m_dev);
+        if (m0 >= rows) return;
+        M = rows;
+    }
     if (batch_kind != 0) {
         // batch over blockIdx.z: A and C advance by a fixed offset; B is selected per batch entry.
         // kind 1 = "lm blocks" of an equivariant feature [rows][(l,m)][channels]: z = (l,m) index,
@@ -169,7 +177,7 @@ __global__ void __launch_bounds__(G_THREADS, 1) k_gemm_tf32x3(int M, int N, int 
 
 int launch(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
            const float* bias, float* act, int act_kind, int batch_kind, int n_batch, long long a_boff, long long b_boff, long long c_boff,
-           cudaStream_t s) {
+           cudaStream_t s, const int32_t* m_dev = nullptr) {
     const int smem = 2 * (int)sizeof(Stage);
     static bool attr_set = false;
     if (!attr_set) {
@@ -178,7 +186,7 @@ int launch(int M, int N, int K, const float* A, int lda, const float* B, int ldb
     }
     dim3 grid((M + G_BM - 1) / G_BM, (N + G_BN - 1) / G_BN, batch_kind ? n_batch : 1);
     k_gemm_tf32x3<<<grid, G_THREADS, smem, s>>>(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, batch_kind, a_boff,
-                                                b_boff, c_boff);
+                                                b_boff, c_boff, m_dev);
     return nb_check_launch();
 }
 
@@ -186,14 +194,14 @@ int launch(int M, int N, int K, const float* A, int lda, const float* B, int ldb
 
 // Constraints: K % 32 == 0, N % 4 == 0, lda/ldb/ldc % 4 == 0, 16-byte aligned pointers; `act` (optional) shares ldc with C.
 int nb_gemm_tf32x3_ex(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,
-                      const float* bias, float* act, int act_kind, cudaStream_t s) {
+                      const float* bias, float* act, int act_kind, cudaStream_t s, const int32_t* m_dev) {
     if (!A || !B || !C || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
     if (K % G_BK || N % 4 || lda % 4 || ldb % 4 || ldc % 4) return NB200_EUNSUPPORTED;
     if (M == 0) return NB200_OK;
     // tall problems: weights pre-split once into shared-memory tile images and streamed (gemm_ps.cu)
     if (nb_gemm_ps_wanted(M, N, K))
-        return nb_gemm_ps(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, nullptr, 0, s);
-    return launch(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, 0, 1, 0, 0, 0, s);
+        return nb_gemm_ps(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, nullptr, 0, s, m_dev);
+    return launch(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, act_kind, 0, 1, 0, 0, 0, s, m_dev);
 }
 
 // batched over the 25 (l,m) rows of an equivariant feature: see batch_kind 1 in the kernel
@@ -211,4 +219,10 @@ extern "C" int nb200_gemm_tf32x3(int32_t M, int32_t N, int32_t K, const float* A
                                  int32_t trans_b, float* C, int32_t ldc, int32_t accumulate, const float* bias, float* act,
                                  void* stream) {
     return nb_gemm_tf32x3_ex(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, NB_ACT_SILU, (cudaStream_t)stream);
+}
+
+// test entry: nb200_gemm_tf32x3 with an optional row count in device memory (M is then the bound the launch is sized by)
+extern "C" int nb200_gemm_tf32x3_rows(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb, int32_t trans_b,
+                                      float* C, int32_t ldc, int32_t accumulate, const float* bias, float* act, const int32_t* m_dev, void* stream) {
+    return nb_gemm_tf32x3_ex(M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, act, NB_ACT_SILU, (cudaStream_t)stream, m_dev);
 }

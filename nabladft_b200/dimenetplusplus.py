@@ -12,12 +12,14 @@ per-element tables).
 Training: in training mode with autograd the forward goes through `DimeNetEnergyFn`, whose backward is `nb200_dimenet_train_grads` (the
 parameter gradients of energy and force losses, the force term by forward-over-reverse, DESIGN.md 3.15.1); the export is then differentiable,
 so autograd carries the flat-buffer gradient back to every reference-named parameter.  Hessians: `DimeNetRunner.run_hvp` (nb200_dimenet_hvp,
-DESIGN.md 3.15.2) gives exact Hessian-vector products of the unscaled prediction; `vibrations.hessians` / `normal_modes` take this model.  Supported: the shipped sizes, with
+DESIGN.md 3.15.2) gives exact Hessian-vector products of the unscaled prediction; `vibrations.hessians` / `normal_modes` take this model.
+Relaxation and molecular dynamics: `engine()` is the interface of `optimization.ASEBatchwiseLBFGS` and `md.BatchwiseMD`; its forward is the
+asynchronous call, sized by per-batch upper bounds of the edge and triplet counts (DESIGN.md 3.15.3).  Supported: the shipped sizes, with
 1 <= dimenet_num_blocks <= 16, 2 <= node_latent_dim <= 64 and dimenet_max_num_neighbors <= 64; anything else raises at construction.  No CPU
 fallback: CPU tensors raise NablaB200Error in eval mode and NotImplementedError in training mode.
 """
 import ctypes
-from ctypes import POINTER, byref, c_int64
+from ctypes import POINTER, byref, c_int32, c_int64
 from typing import Dict, List, Optional, Tuple
 
 import numpy as np
@@ -153,6 +155,7 @@ class DimeNetPlusPlusPotential(nn.Module):
         self.regr_or_cls_nn = nn.Sequential(nn.Linear(L, L), _Swish(), nn.Linear(L, L // 2), _Swish(), nn.Linear(L // 2, L // 2), _Swish(),
                                             nn.Linear(L // 2, 1))
         self._runner: Optional[DimeNetRunner] = None
+        self._engine: Optional[DimeNetEngine] = None
         self._export_key = None
 
     # ---- export: reference-named tensors -> flat buffer (include/nabla_b200.h NB200_DPP_*) ---------------------------------------------------
@@ -224,6 +227,12 @@ class DimeNetPlusPlusPotential(nn.Module):
         self._sync_weights(runner, pos.device)
         return runner.run(*self.batch_args(z, pos, batch))
 
+    def engine(self) -> "DimeNetEngine":
+        """The engine interface of the batch-wise optimiser and MD loops (`optimization.ASEBatchwiseLBFGS`, `md.BatchwiseMD`)."""
+        if self._engine is None:
+            self._engine = DimeNetEngine(self, self._get_runner())
+        return self._engine
+
     def _get_runner(self) -> "DimeNetRunner":
         if self._runner is None:
             self._runner = DimeNetRunner()
@@ -253,7 +262,9 @@ class DimeNetRunner(EngineDriver):
         super().__init__(lib)
         self._w = None
         self._keep = None
+        self._status = None
         self.last_counts: Dict[str, int] = {}
+        self.last_workspace_bytes = 0
 
     def set_weights(self, model: DimeNetPlusPlusPotential, device):
         self.bind(model, *model.export(device))
@@ -293,6 +304,35 @@ class DimeNetRunner(EngineDriver):
         self.last_counts = {"edges": int(counts[0]), "triplets": int(counts[1])}
         return gbuf, counts
 
+    def count_bounds(self, sizes):
+        """Upper bounds of {edges, triplet slots} for molecules of `sizes` atoms (host, nb200_dimenet_count_bounds): they hold for every
+        geometry, see DESIGN.md 3.15.3."""
+        if self._w is None:
+            raise NablaB200Error("DimeNetRunner.count_bounds before set_weights / bind")
+        mol_ptr = (c_int32 * (len(sizes) + 1))(0, *[int(v) for v in torch.as_tensor(sizes).cumsum(0)])
+        bounds = (c_int64 * N_COUNTS)()
+        check(self.lib.nb200_dimenet_count_bounds(byref(self._w), mol_ptr, len(sizes), bounds), "nb200_dimenet_count_bounds")
+        return bounds
+
+    def launch(self, z, pos, mol_ptr, n_mol: int, bounds):
+        """Asynchronous forward (nb200_dimenet_energy_forces_async): one enqueue on the current stream, no host read.  -> (energy, forces,
+        status); `status` is a device int32[8] that the next launch rewrites (include/nabla_b200.h).  Graph buffer and workspace are sized by
+        n_atoms and `bounds` (count_bounds), hence once per batch: later launches of the same batch reuse them."""
+        if self._w is None:
+            raise NablaB200Error("DimeNetRunner.launch before set_weights / bind")
+        lib, n, dev = self.lib, int(z.shape[0]), pos.device
+        gbytes = self._bytes("nb200_dimenet_graph_bytes", byref(self._w), n)
+        self.last_workspace_bytes = self._bytes("nb200_dimenet_workspace_bytes", byref(self._w), n_mol, n, bounds)
+        gbuf, ws = self._buffer("_graph_buf", gbytes, dev), self._buffer("_ws", self.last_workspace_bytes, dev)
+        if self._status is None or self._status.device != dev:
+            self._status = torch.zeros(8, dtype=torch.int32, device=dev)
+        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+        forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        check(lib.nb200_dimenet_energy_forces_async(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n,
+                                                    gbuf.data_ptr(), gbuf.numel(), bounds, ws.data_ptr(), ws.numel(), energy.data_ptr(),
+                                                    forces.data_ptr(), self._status.data_ptr(), self._stream()), "nb200_dimenet_energy_forces_async")
+        return energy, forces, self._status
+
     def train_grads(self, z, pos, mol_ptr, n_mol: int, seed_energy: Optional[torch.Tensor], seed_forces: Optional[torch.Tensor]) -> torch.Tensor:
         """d(sum_m seed_energy[m] E_m + sum_i seed_forces[i] . F_i)/d(flat weight buffer), in the buffer's layout (nb200_dimenet_train_grads).
         Either seed may be None.  Builds the graph again (one synchronisation for the counts), so it does not depend on an earlier call."""
@@ -331,6 +371,57 @@ class DimeNetRunner(EngineDriver):
                                     counts, ws.data_ptr(), ws.numel(), n_dir, v.data_ptr(), energy.data_ptr(),
                                     None if forces is None else forces.data_ptr(), hv.data_ptr(), self._stream()), "nb200_dimenet_hvp")
         return energy, forces, hv
+
+
+class DimeNetEngine:
+    """What `optimization.ASEBatchwiseLBFGS` and `md.BatchwiseMD` need from a model, with `PainnEngine`'s method names: `run` (synchronous,
+    validates), `launch` (asynchronous), `e_cap`, `raise_on_status`.  There is no edge capacity to grow (`grows_capacity` is False): `run`
+    derives upper bounds of the edge and triplet counts from the molecule sizes of the batch, and `launch` sizes everything by them (`e_cap`
+    is accepted and ignored).  A count above its bound is therefore a bug, not a reason to retry."""
+
+    grows_capacity = False
+
+    def __init__(self, model: DimeNetPlusPlusPotential, runner: DimeNetRunner):
+        self.model, self.runner, self.e_cap = model, runner, 0
+        self._batch = None
+        self.last_status = None
+
+    def run(self, z, pos, mol_ptr, n_mol: int):
+        """First evaluation of a batch: checks `mol_ptr` on the host (once, not per step), fixes the batch's bounds, launches and validates.
+        -> (energy, forces, status words on the host)."""
+        ptr_host = mol_ptr.cpu()
+        sizes = ptr_host[1:] - ptr_host[:-1]
+        if len(sizes) != n_mol or n_mol < 1 or int(ptr_host[0]) != 0 or int(sizes.min()) < 1 or int(ptr_host[-1]) != z.shape[0]:
+            raise NablaB200Error("DimeNet++: `mol_ptr` must hold n_mol + 1 increasing atom offsets starting at 0 (atoms of a molecule contiguous)")
+        self.model._sync_weights(self.runner, pos.device)
+        self._batch = ((mol_ptr.data_ptr(), n_mol, int(z.shape[0])), self.runner.count_bounds(sizes))
+        energy, forces, status = self.launch(z, pos, mol_ptr, n_mol)
+        host = status.cpu()
+        self.raise_on_status(host)
+        self.last_status = host
+        return energy, forces, host
+
+    def launch(self, z, pos, mol_ptr, n_mol: int, e_cap=None):
+        if self._batch is None or self._batch[0] != (mol_ptr.data_ptr(), n_mol, int(z.shape[0])):
+            raise NablaB200Error("DimeNetEngine.launch: call run() on this batch first (it derives the bounds the launch is sized by)")
+        return self.runner.launch(z, pos, mol_ptr, n_mol, self._batch[1])
+
+    @property
+    def bounds(self) -> Dict[str, int]:
+        return {"edges": int(self._batch[1][0]), "triplets": int(self._batch[1][1])} if self._batch else {}
+
+    @staticmethod
+    def raise_on_status(status_host) -> None:
+        """`status_host`: the status words of a launch on the host (the first four suffice).  Atoms without neighbours are not an error."""
+        n_edges, err, max_deg, n_iso = (int(v) for v in status_host[:4])
+        if err == -4:
+            raise NablaB200Error(f"NB200_ECAPACITY: a count exceeds its bound ({n_edges} edges); `mol_ptr` changed under the engine?")
+        if err == -1:
+            raise NablaB200Error("DimeNet++: atomic number outside [0, 94] or non-finite atom coordinates")
+        if err != 0:
+            from ._lib import ERRORS
+
+            raise NablaB200Error(f"DimeNet++ graph construction failed: {ERRORS.get(err, err)} (max in-degree {max_deg}, {n_iso} atoms without neighbours)")
 
 
 class DimeNetEnergyFn(torch.autograd.Function):

@@ -12,8 +12,9 @@ device only once per chunk of `check_every` steps.  Semantics are ASE 3.22's (re
     md.atoms, md.momenta, md.nsteps, md.log, md.frames
 
 Random numbers come from a counter-based Philox stream keyed by `seed`, so a run is reproducible bit for bit, whatever `check_every`, and
-however `run_md` splits the steps.  An edge-capacity overflow of the engine in a chunk is recovered by replaying the chunk from its
-start with a larger capacity; the replay draws the same noise.
+however `run_md` splits the steps.  An edge-capacity overflow of a PaiNN / SchNet engine in a chunk is recovered by replaying the chunk from
+its start with a larger capacity; the replay draws the same noise.  Engines sized by per-batch bounds (DimeNet++: `grows_capacity = False`)
+have no capacity to grow, so there the same status is an error and is raised at once.
 """
 import os
 from typing import List, Optional, Sequence
@@ -48,7 +49,9 @@ def mdlogger_line(time_ps: float, epot: float, ekin: float, temp: float, n_atoms
 
 
 class BatchwiseMD:
-    """Molecular dynamics of a batch of molecules with `SpkBatchwiseCalculator` (spk PaiNN, SchNet) or `PyGBatchwiseCalculator` (PaiNN-OC).
+    """Molecular dynamics of a batch of molecules with `SpkBatchwiseCalculator` (spk PaiNN, SchNet) or `PyGBatchwiseCalculator` (PaiNN-OC,
+    DimeNet++).  DimeNet++ with `do_postprocessing` and a scale other than 1 scales the energy but not the forces (the reference's semantics),
+    so the logged total energy is conserved only without postprocessing or with scale 1.
 
     `masses` [n_atoms] in u overrides the standard atomic weights; `seed` keys the random stream; `check_every` is the number of steps
     between host looks at the device (status word, logs).  `fixed_atoms` is not supported."""
@@ -199,7 +202,8 @@ class BatchwiseMD:
 
     def _chunk(self, k: int) -> None:
         """k steps: START, then per step one engine launch and one FINISH|START launch (FINISH alone at the end); one host look at the end.
-        On NB200_ECAPACITY the chunk is replayed from copies taken at its start with a larger edge capacity."""
+        On NB200_ECAPACITY the chunk is replayed from copies taken at its start with a larger edge capacity, unless the engine cannot grow
+        one (`grows_capacity` False): then it is raised like any other engine error."""
         eng = self._eng
         saved = [t.clone() for t in (self._pos, self._mom, self._pos32, self._forces, self._energy)]
         logged = [self.nsteps + j + 1 for j in range(k) if (self.nsteps + j + 1) % self.interval == 0]
@@ -217,7 +221,7 @@ class BatchwiseMD:
                 slot += int(log)
             host = worst.cpu()  # the one synchronisation of the chunk
             self.host_syncs += 1
-            if int(host[3]):
+            if int(host[3]) and getattr(eng, "grows_capacity", True):
                 # overflow: restore the chunk's starting state and replay it; the counter-based noise makes the replay draw the same numbers
                 eng.e_cap = int(1.25 * int(host[0])) + 1024
                 self._pos.copy_(saved[0]); self._mom.copy_(saved[1]); self._pos32.copy_(saved[2])
@@ -225,7 +229,7 @@ class BatchwiseMD:
                 self.replays += 1
                 continue
             if int(host[1]):
-                # any other engine error: leave the state as it was at the chunk start (nsteps and the noise step have not advanced), then raise
+                # any other engine error (or an overflow of an engine sized by bounds): leave the state as it was at the chunk start (nsteps and the noise step have not advanced), then raise
                 self._pos.copy_(saved[0]); self._mom.copy_(saved[1]); self._pos32.copy_(saved[2])
                 self._forces, self._energy = saved[3], saved[4]
                 eng.raise_on_status(host)

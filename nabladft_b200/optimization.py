@@ -132,7 +132,8 @@ class BatchwiseCalculator:
 
 
 class PyGBatchwiseCalculator(BatchwiseCalculator):
-    """calculator.py:98-129 for `nabladft_b200.painn_oc.PaiNN` and `nabladft_b200.gemnet_oc.GemNetOC` (net(data) -> (energy, forces))."""
+    """calculator.py:98-129 for `nabladft_b200.painn_oc.PaiNN`, `nabladft_b200.gemnet_oc.GemNetOC` and
+    `nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential` (net(data) -> (energy, forces))."""
 
     def engine(self):
         return self.model.engine()
