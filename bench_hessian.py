@@ -1,7 +1,7 @@
-"""Throughput of exact Hessians (nb200_painn_hvp, nb200_schnet_hvp, nb200_dimenet_hvp) on the config-2 batch: 256 synthetic conformations
+"""Throughput of exact Hessians (nb200_painn_hvp, nb200_schnet_hvp, nb200_dimenet_hvp, nb200_gemnet_oc_jvp) on the config-2 batch: 256 synthetic conformations
 (synth.py), one JSON line.
 
-    python bench_hessian.py [--model painn|painn-oc|schnet|dimenetplusplus] [--max-dir D] [--repeats R] [--batch B]
+    python bench_hessian.py [--model painn|painn-oc|schnet|dimenetplusplus|gemnet-oc] [--max-dir D] [--repeats R] [--batch B]
 
 Reports Hessians / s and HVP directions / s for the whole batch (3 n_max shared directions, chunks of --max-dir), peak device memory, ms per
 direction split into the tangent forward and the backward (CUDA events around the engine's launch categories), and the same Hessians by
@@ -14,6 +14,11 @@ limit come from the same run.  Writes nothing into the tree.
 pass over the 3 n_max shared directions (its cost per direction is about that of a training gradient call, so it is not repeated), the
 per-direction and once-per-call costs from one- and --probe-direction calls, and the same Hessians by central differences with two
 nb200_dimenet_energy_forces calls per direction.
+
+--model gemnet-oc (config/model/gemnet-oc.yaml sizes, the tests' weights, synth_batch(0, B), B = 32 unless --batch is given): the same, with
+force-Jacobian products (the direct forces' Jacobian, symmetrised as ASE does) against two two-phase nb200_gemnet_oc_energy_forces calls per
+direction, plus the workspace of the call at B and the largest synth_batch(0, B') whose workspace fits the card's free memory (bisection on
+the size query, graph phase only).
 """
 import argparse
 import ctypes
@@ -38,15 +43,21 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="painn", choices=["painn", "painn-oc", "schnet", "dimenetplusplus"])
+    ap.add_argument("--model", default="painn", choices=["painn", "painn-oc", "schnet", "dimenetplusplus", "gemnet-oc"])
     ap.add_argument("--max-dir", type=int, default=None)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--fd-step", type=float, default=1e-3)
-    ap.add_argument("--batch", type=int, default=256, help="molecules (dimenetplusplus only; the other models use the config-2 batch)")
-    ap.add_argument("--probe-directions", type=int, default=8, help="directions of the call the per-direction cost is taken from (dimenetplusplus)")
+    ap.add_argument("--batch", type=int, default=None,
+                    help="molecules (dimenetplusplus: 256, gemnet-oc: 32 by default; the other models use the config-2 batch)")
+    ap.add_argument("--probe-directions", type=int, default=8,
+                    help="directions of the call the per-direction cost is taken from (dimenetplusplus, gemnet-oc)")
     args = ap.parse_args()
     if args.model == "dimenetplusplus":
+        args.batch = args.batch or 256
         return dimenet_main(args)
+    if args.model == "gemnet-oc":
+        args.batch = args.batch or 32
+        return gemnet_main(args)
 
     import torch
 
@@ -249,6 +260,118 @@ def dimenet_main(args):
         "fd_max_rel_dev": max(devs), "fd_median_rel_dev": float(np.median(devs)),
         "fd_max_rel_dev_untruncated": max(smooth) if smooth else None, "untruncated_molecules": len(smooth), "analytic_speedup_vs_fd": t_fd / t_an, "max_asymmetry": hs.max_asymmetry,
         "card": name, "power_limit": limit,
+    }))
+
+
+def gemnet_main(args):
+    import os
+    import sys
+
+    import torch
+
+    root = os.path.dirname(os.path.abspath(__file__))
+    sys.path.insert(0, os.path.join(root, "tests"))
+    sys.path.insert(0, os.path.join(root, "tests", "golden"))
+    from test_gemnet_emu import _models
+
+    from nabladft_b200 import vibrations as vib
+    from nabladft_b200.synth import synth_batch
+
+    dev = torch.device("cuda:0")
+    model = _models(True)[0].to(dev).eval()
+
+    class D:
+        pass
+
+    def make_batch(n_mol):
+        b = synth_batch(0, n_mol)
+        d = D()
+        d.z = torch.from_numpy(b["z"]).long().to(dev)
+        d.pos = torch.from_numpy(b["pos"]).to(dev)
+        d.batch = torch.from_numpy(b["batch"]).to(dev)
+        return d
+
+    batch = make_batch(args.batch)
+    runner, zi, posf, mol_ptr, n_mol = vib._engine_inputs(model, batch)
+    ptr = mol_ptr.cpu().tolist()
+    n_max = max(q - p for p, q in zip(ptr[:-1], ptr[1:]))
+    n_dir = 3 * n_max
+    v = vib.shared_directions(ptr, 0, n_dir, dev)
+    k = max(2, min(args.probe_directions, n_dir))
+
+    def timed(vv):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        runner.run_hvp(zi, posf, mol_ptr, n_mol, vv, with_forces=False)
+        torch.cuda.synchronize()
+        return time.perf_counter() - t0
+
+    timed(v[:1])  # workspace allocation
+    torch.cuda.reset_peak_memory_stats(dev)
+    t1 = timed(v[:1])
+    tk = timed(v[:k])
+    per_dir = (tk - t1) / (k - 1)
+    ws = runner.last_workspace_bytes
+    counts = dict(runner.last_counts)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    hs = vib.hessians(model, batch, args.max_dir)
+    torch.cuda.synchronize()
+    t_an = time.perf_counter() - t0
+    peak = torch.cuda.max_memory_allocated(dev)
+
+    # central differences of the direct forces: two two-phase inference calls per shared direction
+    h = args.fd_step
+    max_atoms = n_max
+    runner.run(zi, posf, mol_ptr, n_mol, max_atoms)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    cols = []
+    for d in range(n_dir):
+        dv = v[d] * h
+        fp = runner.run(zi, (posf + dv).contiguous(), mol_ptr, n_mol, max_atoms)[1]
+        fm = runner.run(zi, (posf - dv).contiguous(), mol_ptr, n_mol, max_atoms)[1]
+        cols.append(-(fp - fm) / (2 * h))
+    torch.cuda.synchronize()
+    t_fd = time.perf_counter() - t0
+    hv_fd = torch.stack(cols)
+    fd = vib.hessians_from_hvp(lambda vv: hv_fd[:vv.shape[0]], ptr)
+    devs = [float((a - c).abs().max() / a.abs().max()) for a, c in zip(hs, fd)]
+
+    # the largest synth_batch(0, B) whose jvp workspace fits what the card has free now (graph phase and size query only, no model pass)
+    # drop the runner's buffers first: a small one carved from the cached jvp segment would pin that whole segment through empty_cache()
+    runner.release_hvp_workspace()
+    runner._ws = runner._graph_buf = None
+    del hv_fd, cols
+    torch.cuda.empty_cache()
+    free = torch.cuda.mem_get_info(dev)[0] - (1 << 30)  # 1 GiB for v, jv, the graph buffer and the allocator
+
+    def ws_bytes(n_mol_):
+        d = make_batch(n_mol_)
+        _, z_, p_, mp_, nm_ = vib._engine_inputs(model, d)
+        pt = mp_.cpu()
+        _, cnt = runner._graph(p_, mp_, nm_, int((pt[1:] - pt[:-1]).max()))
+        return runner._bytes("nb200_gemnet_oc_jvp_workspace_bytes", ctypes.byref(runner._w), nm_, int(z_.numel()), cnt)
+
+    lo, hi = args.batch, 2 * args.batch
+    if ws_bytes(lo) > free:
+        lo, hi = 0, lo
+    else:
+        while ws_bytes(hi) <= free:
+            lo, hi = hi, 2 * hi
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if ws_bytes(mid) <= free else (lo, mid)
+
+    name, limit = card()
+    print(json.dumps({
+        "metric": "gemnet_oc_hessians", "model": args.model, "batch": n_mol, "atoms": int(zi.numel()), "counts": counts, "n_max": n_max,
+        "directions": n_dir, "hessians_per_s": n_mol / t_an, "ms_per_batch": 1e3 * t_an, "ms_per_direction": 1e3 * t_an / n_dir,
+        "ms_once_per_call": 1e3 * (t1 - per_dir), "ms_per_direction_marginal": 1e3 * per_dir, "probe_directions": k,
+        "peak_mem_gb": peak / 1e9, "jvp_workspace_gb": ws / 1e9, "largest_batch_fitting": lo, "free_gb_for_workspace": free / 1e9,
+        "fd_ms_per_batch": 1e3 * t_fd, "fd_ms_per_direction": 1e3 * t_fd / n_dir, "fd_step_A": h,
+        "fd_max_rel_dev": max(devs), "fd_median_rel_dev": float(np.median(devs)), "analytic_speedup_vs_fd": t_fd / t_an,
+        "max_asymmetry": hs.max_asymmetry, "card": name, "power_limit": limit,
     }))
 
 

@@ -547,6 +547,20 @@ int nb200_gemnet_oc_energy_forces_grads(nb200_engine* eng, const nb200_gemnet_oc
  * and keep_token_host != NULL -- the engine keeps the tape and returns a token; then nb200_gemnet_oc_backward(eng, token, seeds) fills that
  * `grads` buffer.  NB200_EINVAL if the engine no longer holds that forward (another training forward ran on it): re-run the one-call form. */
 int nb200_gemnet_oc_backward(nb200_engine* eng, int64_t token, const float* energy_seed, const float* force_seed, void* stream);
+/* Force-Jacobian products (csrc/gemnet_oc_jvp.inc, DESIGN.md 3.9.1): for each of n_dir position-space directions v[d] ([n_atoms,3], Angstrom)
+ *   jv[d] = -(dF/dR) v[d]   in Ha/A, F the direct forces,
+ * exact (one forward-mode pass through the training forward, no finite step), fp32.  The forces are not a gradient, so this Jacobian is not
+ * symmetric; ASE's `Vibrations` reports the symmetric part of the same matrix.  Same two-phase protocol: nb200_gemnet_oc_graph_count, then
+ * nb200_gemnet_oc_jvp_workspace_bytes for the exact counts.  energy[n_mol] and forces[n_atoms,3] (NULL => not written) are bitwise those of
+ * nb200_gemnet_oc_energy_forces_grads with both seeds NULL.  The primal pass runs once per call, the directions one after another, so the
+ * workspace does not depend on n_dir.  No atomics: bitwise repeatable and independent of how the directions are split into calls.  The graph
+ * is that of `pos`: membership is piecewise constant and not differentiated.  NB200_EINVAL (nothing launched) for a NULL required pointer,
+ * n_dir < 1, counts above the graph capacity, or a short graph buffer or workspace; NB200_ENOEDGES for a batch without main-graph edges. */
+int64_t nb200_gemnet_oc_jvp_workspace_bytes(const nb200_gemnet_oc_weights* w, int32_t n_mol, int32_t n_atoms, const int64_t* counts_host);
+int nb200_gemnet_oc_jvp(nb200_engine* eng, const nb200_gemnet_oc_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
+                        int32_t n_mol, int32_t n_atoms, int32_t max_atoms_per_mol, void* graph_buf, int64_t graph_bytes,
+                        const int64_t* counts_host, void* workspace, int64_t workspace_bytes, int32_t n_dir, const float* v,
+                        float* energy, float* forces, float* jv, void* stream);
 /* Debug / parity hooks: copies of the per-atom embedding h [N,256] after the last interaction block (NULL = skip). */
 int nb200_gemnet_oc_debug_h(const void* workspace, const nb200_gemnet_oc_weights* w, int32_t n_mol, int32_t n_atoms,
                             const int64_t* counts_host, float* h_out, void* stream);

@@ -180,6 +180,9 @@ SIGNATURES = {
                                                       c_void_p, c_int64, POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                       POINTER(c_int64), c_void_p]),
     "nb200_gemnet_oc_backward": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "nb200_gemnet_oc_jvp_workspace_bytes": (c_int64, [POINTER(GemNetOCWeights), c_int32, c_int32, POINTER(c_int64)]),
+    "nb200_gemnet_oc_jvp": (c_int32, [c_void_p, POINTER(GemNetOCWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,
+                                      POINTER(c_int64), c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_dimenet_graph_bytes": (c_int64, [POINTER(DimeNetWeights), c_int32]),
     "nb200_dimenet_graph_count": (c_int32, [POINTER(DimeNetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64,
                                             POINTER(c_int64), c_void_p]),

@@ -12,6 +12,8 @@
 // molecule) -- a row permutation of every per-edge tensor that cancels in the per-atom sums (energy, forces, h).
 // Dense layers run on the wgmma 3xTF32 GEMM (gemm_tc.cu) when the shape tiles, else on the functor fallback below.
 // Every kernel is a functor launched through pfor() (gemnet_pf.cuh) so that the same source compiles for host emulation in tests/emu.
+// Training (parameter gradients) is gemnet_oc_train.inc; force-Jacobian products, a tangent pass through that training forward for normal
+// modes, are gemnet_oc_jvp.inc (DESIGN.md 3.9.1).
 #include "gemnet_oc_kernels.cuh"
 
 namespace {
@@ -606,3 +608,4 @@ extern "C" int nb200_gemnet_oc_debug_h(const void* workspace, const nb200_gemnet
 }
 
 #include "gemnet_oc_train.inc"
+#include "gemnet_oc_jvp.inc"

@@ -14,6 +14,9 @@ and dLoss/dF through every kernel (csrc/gemnet_oc_train.inc) and autograd un-fol
 Relaxation: `GemNetOC.engine()` hands `optimization.ASEBatchwiseLBFGS` a forward that never waits for the host
 (`nb200_gemnet_oc_energy_forces_async`, sized by per-batch upper bounds of the edge counts: DESIGN.md 3.9).
 
+Normal modes: `GemNetOCRunner.run_hvp` gives exact products with the direct forces' Jacobian, jv = -(dF/dR) v
+(`nb200_gemnet_oc_jvp`, one tangent pass through the training forward: DESIGN.md 3.9.1); `vibrations.hessians` / `normal_modes` use it.
+
 STATUS (round 1): every kernel has been checked against the oracle through the host-emulation build of the same source
 (tests/emu, tests/test_gemnet_emu.py); the GPU run of `tests/test_zz_gpu_first_runs.py` is the first execution on a device.
 """
@@ -477,6 +480,44 @@ class GemNetOCRunner(EngineDriver):
         if keep and not seeded:
             return energy, forces, (int(token.value), grads)
         return energy, forces, grads
+
+    def run_hvp(self, z, pos, mol_ptr, n_mol: int, v, with_forces: bool = True):
+        """Exact force-Jacobian products (nb200_gemnet_oc_jvp): v [n_dir, N, 3] (or [N, 3]) fp32 in Angstrom.  Returns (energy [B], forces
+        [N, 3] or None, jv [n_dir, N, 3]) with jv = -(dF/dR) v in Ha/A, F the direct forces, and energy / forces bitwise those of `run_train`
+        without seeds.  The direct forces are not a gradient, so this Jacobian is not symmetric (`vibrations.hessians` reports its symmetric
+        part, as ASE `Vibrations` does with finite differences); the name is the one `vibrations` calls for every model.  Builds the graph
+        (one synchronisation for the counts), then one call.  The workspace holds every activation of the training forward twice (44 GB for
+        32 molecules of 10-30 heavy atoms).  It is a buffer of its own, kept for the next call until `release_hvp_workspace()`
+        (`vibrations.hessians` releases it when it is done); a batch whose workspace does not fit raises NablaB200Error: split it by
+        molecules."""
+        if self._w is None:
+            raise NablaB200Error("GemNetOCRunner.run_hvp before set_weights")
+        lib, n, dev = self.lib, int(z.shape[0]), pos.device
+        if v.dim() == 2:
+            v = v.unsqueeze(0)
+        if not (v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n, 3) and v.shape[0] >= 1 and v.device == dev):
+            raise NablaB200Error(f"run_hvp(): v must be a contiguous fp32 tensor [n_dir, {n}, 3] with n_dir >= 1 on {dev}")
+        n_dir = int(v.shape[0])
+        ptr_host = mol_ptr.cpu()
+        max_atoms = int((ptr_host[1:] - ptr_host[:-1]).max())
+        gbuf, counts = self._graph(pos, mol_ptr, n_mol, max_atoms)
+        self.last_workspace_bytes = self._bytes("nb200_gemnet_oc_jvp_workspace_bytes", byref(self._w), n_mol, n, counts)
+        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+        forces = torch.empty(n, 3, dtype=torch.float32, device=dev) if with_forces else None
+        jv = torch.empty(n_dir, n, 3, dtype=torch.float32, device=dev)
+        try:
+            ws = self._buffer("_jvp_ws", self.last_workspace_bytes, dev)
+        except torch.cuda.OutOfMemoryError as exc:
+            raise NablaB200Error(f"GemNetOC run_hvp: the workspace for these {n_mol} molecules ({n} atoms) needs {self.last_workspace_bytes / 1e9:.1f} GB, "
+                                 "more than the device has free; split the batch by molecules") from exc
+        check(lib.nb200_gemnet_oc_jvp(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms, gbuf.data_ptr(),
+                                      gbuf.numel(), counts, ws.data_ptr(), ws.numel(), n_dir, v.data_ptr(), energy.data_ptr(),
+                                      None if forces is None else forces.data_ptr(), jv.data_ptr(), self._stream()), "nb200_gemnet_oc_jvp")
+        return energy, forces, jv
+
+    def release_hvp_workspace(self):
+        """Hand the workspace of `run_hvp` (tens of GB for a few dozen molecules) back to the allocator."""
+        self._jvp_ws = None
 
     def backward(self, token: int, seed_energy, seed_forces) -> bool:
         """Replay the tape of the forward kept under `token` into the gradient buffer handed out by that forward.  False: the engine no

@@ -1,9 +1,9 @@
-"""Analytic Hessians and normal modes of the PaiNN, SchNet and DimeNet++ models on the GPU.
+"""Analytic Hessians and normal modes of the PaiNN, SchNet, DimeNet++ and GemNet-OC models on the GPU.
 
 The reference's `PYGAseInterface.compute_normal_modes` (nablaDFT/optimization/pyg_ase_interface.py) runs ASE `Vibrations`: central finite
 differences of the forces, one molecule at a time, 6N + 1 force calls per molecule with a 0.01 A step.  Here the engine computes exact
-Hessian-vector products H v = -(dF/dR) v (`PainnEngine.run_hvp`, `DimeNetRunner.run_hvp`; DESIGN.md section 3.13 for PaiNN, 3.13.1 for
-SchNet, 3.15.2 for DimeNet++), and since
+Hessian-vector products H v = -(dF/dR) v (`PainnEngine.run_hvp`, `DimeNetRunner.run_hvp`, `GemNetOCRunner.run_hvp`; DESIGN.md section
+3.13 for PaiNN, 3.13.1 for SchNet, 3.15.2 for DimeNet++, 3.9.1 for GemNet-OC), and since
 molecules do not interact, ONE direction displaces atom k of every molecule of the batch at once: the Hessians of a whole batch take
 3 * n_max directions, n_max = the atom count of the largest molecule.
 
@@ -12,8 +12,10 @@ molecules do not interact, ONE direction displaces atom k of every molecule of t
     normal_modes(model, batch, masses=None) -> per-molecule eigenvalues, modes, wavenumbers (cm^-1) and ASE-style energies (meV)
 
 `model` is `spk.NeuralNetworkPotential` (PaiNN or SchNet representation; `batch` = its inputs dict), `painn_oc.PaiNN` (`batch` has
-.z, .pos, .batch and optionally .ptr) or `dimenetplusplus.DimeNetPlusPlusPotential` (`batch` has .z, .pos and a sorted .batch).  H is the
-Hessian of the energy the forces are the gradient of: for DimeNet++ that is the unscaled prediction (the scaler touches the energy only).  Everything runs in fp32 on the device except the diagonalisation (float64, `torch.linalg.eigh`).
+.z, .pos, .batch and optionally .ptr), `dimenetplusplus.DimeNetPlusPlusPotential` or `gemnet_oc.GemNetOC` (`batch` has .z, .pos and a sorted
+.batch).  H is the Hessian of the energy the forces are the gradient of: for DimeNet++ that is the unscaled prediction (the scaler touches
+the energy only).  GemNet-OC predicts its forces directly, so there H is the force Jacobian -(dF/dR), which is not symmetric; `hessians`
+reports its symmetric part, which is what ASE `Vibrations` computes from central differences of the same forces.  Everything runs in fp32 on the device except the diagonalisation (float64, `torch.linalg.eigh`).
 """
 import math
 from dataclasses import dataclass
@@ -44,7 +46,7 @@ MEV_PER_CM1 = 1e3 * PLANCK_JS * C_CM_PER_S / EV_J  # h c in meV cm
 # ---------------------------------------------------------------------------------------------------------------- model plumbing
 def _engine_inputs(model, batch):
     """(engine, z int32, pos fp32, mol_ptr int32, n_mol) for each mirror, with the errors the mirrors raise."""
-    from . import dimenetplusplus, painn_oc, spk
+    from . import dimenetplusplus, gemnet_oc, painn_oc, spk
 
     if isinstance(model, spk.NeuralNetworkPotential):
         eng, z, pos, mol_ptr, n_mol = model._prepare(batch)  # raises on CPU inputs and periodic systems
@@ -72,12 +74,23 @@ def _engine_inputs(model, batch):
         model._sync_weights(runner, batch.pos.device)
         z, pos, mol_ptr, n_mol = model.batch_args(batch.z, batch.pos, batch.batch)
         return runner, z, pos, mol_ptr, n_mol
-    raise NotImplementedError("Hessians need nabladft_b200.spk.NeuralNetworkPotential, nabladft_b200.painn_oc.PaiNN or "
-                              f"nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential, not {type(model).__name__}")
+    if isinstance(model, gemnet_oc.GemNetOC):
+        if not batch.pos.is_cuda:
+            raise NablaB200Error("GemNetOC runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
+        if model.training and torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters()):
+            raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
+        runner = model._get_runner()
+        model._sync_weights(runner, batch.pos.device)
+        z, pos, mol_ptr, n_mol, _ = model._batch_args(batch)  # raises for a molecule beyond max_neighbors_aint + 1 atoms
+        return runner, z, pos, mol_ptr, n_mol
+    raise NotImplementedError("Hessians need nabladft_b200.spk.NeuralNetworkPotential, nabladft_b200.painn_oc.PaiNN, "
+                              "nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential or nabladft_b200.gemnet_oc.GemNetOC, "
+                              f"not {type(model).__name__}")
 
 
 def hessian_vector_product(model, batch, v: torch.Tensor):
-    """(energy [B], forces [N, 3], hv) with hv = H v in Ha/A for v [N, 3] or [n_dir, N, 3] in A (hv has v's shape)."""
+    """(energy [B], forces [N, 3], hv) with hv = H v in Ha/A for v [N, 3] or [n_dir, N, 3] in A (hv has v's shape).  For GemNet-OC, whose
+    forces are a direct output, hv = -(dF/dR) v is the product with the force Jacobian, which is not symmetric."""
     eng, z, pos, mol_ptr, n_mol = _engine_inputs(model, batch)
     vv = v.detach().to(device=pos.device, dtype=torch.float32)
     one = vv.dim() == 2
@@ -89,7 +102,9 @@ def hessian_vector_product(model, batch, v: torch.Tensor):
 # ---------------------------------------------------------------------------------------------------------------- Hessians
 class Hessians(list):
     """Per-molecule symmetrised Hessians (H + H^T) / 2, [3n_m, 3n_m] in Ha/A^2, rows and columns ordered (atom, xyz).
-    `max_asymmetry`: the largest |H_ij - H_ji| of the raw products (Ha/A^2), a check of the fp32 arithmetic; `energy`: [B] in Ha."""
+    `max_asymmetry`: the largest |H_ij - H_ji| of the raw products (Ha/A^2), a check of the fp32 arithmetic; `energy`: [B] in Ha.
+    For GemNet-OC the raw products are those of the direct forces' Jacobian, which no energy has as its Hessian: there `max_asymmetry`
+    measures the model's non-conservative part, not fp32 error.  That part is what ASE `Vibrations` discards when it symmetrises."""
 
     max_asymmetry: float = 0.0
     energy: Optional[torch.Tensor] = None
@@ -154,7 +169,12 @@ def hessians(model, batch, max_dir: Optional[int] = None) -> Hessians:
         energy.append(e)
         return hv
 
-    out = hessians_from_hvp(hvp, ptr_host, max_dir, pos.device)
+    try:
+        out = hessians_from_hvp(hvp, ptr_host, max_dir, pos.device)
+    finally:
+        release = getattr(eng, "release_hvp_workspace", None)  # GemNet-OC: the workspace holds the training arena twice
+        if release is not None:
+            release()
     out.energy = energy[0]
     return out
 
