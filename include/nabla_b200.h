@@ -195,6 +195,12 @@ int nb200_gemm_tf32x3(int32_t M, int32_t N, int32_t K, const float* A, int32_t l
  * exactly nb200_gemm_tf32x3. */
 int nb200_gemm_tf32x3_rows(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb, int32_t trans_b,
                            float* C, int32_t ldc, int32_t accumulate, const float* bias, float* act, const int32_t* m_dev, void* stream);
+/* Test entry point: the tall-layer GEMM with a fused tail, as GemNet-OC's Dense layers run it (gemm_ps.cu).  With o = A . op(B) (+ bias):
+ *   epi = 1 (activation): C = act(o);   epi = 2 (residual): C = (C + act(o)) * alpha, C holding the layer input.
+ * act_kind: 3 = ScaledSiLU, silu(x) / 0.6.  Columns at and past N of each C row are not touched.  NB200_EINVAL (nothing launched) for
+ * another epi or A == C; NB200_EUNSUPPORTED for K % 4 != 0, lda % 4 != 0 or ldc < N.  Device library only. */
+int nb200_gemm_tf32x3_epi(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb, int32_t trans_b,
+                          float* C, int32_t ldc, const float* bias, int32_t epi, int32_t act_kind, float alpha, void* stream);
 /* Weight / bias gradient of a Linear layer (torch autograd: grad_weight = grad_out^T @ input, grad_bias = grad_out.sum(0); every
  * nn.Linear of nablaDFT/painn_pyg/painn.py), ACCUMULATED into dW / dbias:
  *   dW[out,in] += alpha * ( (c o G0)^T X0 + G1^T X1 ),   dbias[out] += bias_alpha * colsum(c o G0)
@@ -564,6 +570,32 @@ int nb200_gemnet_oc_jvp(nb200_engine* eng, const nb200_gemnet_oc_weights* w, con
 /* Debug / parity hooks: copies of the per-atom embedding h [N,256] after the last interaction block (NULL = skip). */
 int nb200_gemnet_oc_debug_h(const void* workspace, const nb200_gemnet_oc_weights* w, int32_t n_mol, int32_t n_atoms,
                             const int64_t* counts_host, float* h_out, void* stream);
+/* Test entry point, not a supported API: one edge aggregation of the GemNet-OC interaction block on caller-built graphs (CSR rows by target,
+ * sources ascending, unit vectors V source -> target).
+ *   quad = 0, triplet:    O[e, 64 i + ch] = sum_s R[e, 7 i + s] sum over k in in-row(tgt e), in.src[k] != src e of Y_s(V_e . V_k) x[k, ch]
+ *                         (o, in) = (main, main) or (main, a2ee2a); o needs src, tgt, V; in needs ptr, src, V; ldr >= 112.
+ *   quad = 1, quadruplet: o = the main graph (ptr, src, tgt, V), in = the qint graph (ptr, src, V), q_tin[qint edges] the input-triplet slot
+ *                         bases, x = x_t [slots, 32]; O[e, 32 i + ch] as the QuadrupletInteraction sums it; ldr >= 1568.
+ * O is [E_bound, 1024].  form = 0: the host dispatch the model calls (the warp-per-edge device kernels); form = 1: the one-thread-per-output
+ * functor the training forward runs.  tangent = 1: the forward-mode tangent Ot of O for the tangents Vot, Vit of the two graphs' V, xt of x
+ * and Rt of R (O is not written).  E_dev (primal only, may be NULL): the row count in device memory, E_bound then an upper bound; rows at or
+ * past min(*E_dev, E_bound) are not written.  NB200_EINVAL (nothing launched) for a NULL required pointer, E_bound < 0, a short ldr, or
+ * E_dev with tangent = 1.  The emulation build runs the functor for both forms. */
+typedef struct nb200_gemnet_oc_agg_args {
+    int32_t quad, form, tangent, ldr;
+    int64_t E_bound;
+    const int32_t* E_dev;
+    const int32_t *o_ptr, *o_src, *o_tgt;
+    const float* o_V;
+    const int32_t *in_ptr, *in_src;
+    const float* in_V;
+    const int32_t* q_tin;
+    const float *x, *R;
+    float* O;
+    const float *Vot, *Vit, *xt, *Rt;
+    float* Ot;
+} nb200_gemnet_oc_agg_args;
+int nb200_gemnet_oc_test_aggregate(const nb200_gemnet_oc_agg_args* args, void* stream);
 
 /* ----------------------------------------------------------------------------------------
  * DimeNet++ energy + conservative forces, config/model/dimenetplusplus.yaml: DimeNetPlusPlusPotential

@@ -71,6 +71,15 @@ class GemNetOCWeights(ctypes.Structure):
                 ("max_neighbors_aeaint", c_int32), ("w", c_void_p), ("off_host", POINTER(c_int64)), ("scale_host", POINTER(c_float))]
 
 
+class GemNetOCAggArgs(ctypes.Structure):
+    """Mirror of `struct nb200_gemnet_oc_agg_args` (include/nabla_b200.h)."""
+
+    _fields_ = [("quad", c_int32), ("form", c_int32), ("tangent", c_int32), ("ldr", c_int32), ("E_bound", c_int64), ("E_dev", c_void_p),
+                ("o_ptr", c_void_p), ("o_src", c_void_p), ("o_tgt", c_void_p), ("o_V", c_void_p), ("in_ptr", c_void_p), ("in_src", c_void_p),
+                ("in_V", c_void_p), ("q_tin", c_void_p), ("x", c_void_p), ("R", c_void_p), ("O", c_void_p), ("Vot", c_void_p), ("Vit", c_void_p),
+                ("xt", c_void_p), ("Rt", c_void_p), ("Ot", c_void_p)]
+
+
 class DimeNetWeights(ctypes.Structure):
     """Mirror of `struct nb200_dimenet_weights` (include/nabla_b200.h)."""
 
@@ -115,6 +124,8 @@ SIGNATURES = {
                                     c_int32, c_void_p, c_void_p, c_void_p]),
     "nb200_gemm_tf32x3_rows": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_int32,
                                          c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_gemm_tf32x3_epi": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_int32,
+                                        c_void_p, c_int32, c_int32, c_float, c_void_p]),
     "nb200_linear_wgrad": (c_int32, [c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32, c_float,
                                      c_void_p, c_float, c_void_p, c_int32, c_void_p]),
     "nb200_qh_expand_rows": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
@@ -168,6 +179,7 @@ SIGNATURES = {
     "nb200_gemnet_oc_energy_forces_async": (c_int32, [c_void_p, POINTER(GemNetOCWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
                                                       c_void_p, c_int64, POINTER(c_int64), c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_gemnet_oc_debug_h": (c_int32, [c_void_p, POINTER(GemNetOCWeights), c_int32, c_int32, POINTER(c_int64), c_void_p, c_void_p]),
+    "nb200_gemnet_oc_test_aggregate": (c_int32, [POINTER(GemNetOCAggArgs), c_void_p]),
     "nb200_schnet_train_count": (c_int32, [POINTER(SchnetWeights), c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "nb200_schnet_train_workspace_bytes": (c_int64, [POINTER(SchnetWeights), c_int32, c_int32, c_int64, c_int32]),
     "nb200_schnet_energy_grads": (c_int32, [c_void_p, POINTER(SchnetWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_void_p,

@@ -215,6 +215,11 @@ int nb_gemm_ps_epi(int M, int N, int K, const float* A, int lda, const float* B,
     return gemm_ps_impl(M, N, K, A, lda, B, ldb, trans_b, C, ldc, 0, bias, nullptr, act_kind, nullptr, 0, s, epi, alpha);
 }
 
+extern "C" int nb200_gemm_tf32x3_epi(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb, int32_t trans_b,
+                                     float* C, int32_t ldc, const float* bias, int32_t epi, int32_t act_kind, float alpha, void* stream) {
+    return nb_gemm_ps_epi(M, N, K, A, lda, B, ldb, trans_b, C, ldc, bias, epi, act_kind, alpha, (cudaStream_t)stream);
+}
+
 // o3.Linear batched over the n_lm = 25 (l,m) rows of an equivariant feature (the call of nb_gemm_tf32x3_lm for tall inputs): slice z reads
 // A + z K (row stride lda), writes C + z N (row stride ldc), uses W_l[l(z)] ([K][N], stride w_l_stride), bias on z = 0 only.
 bool nb_gemm_ps_lm_wanted(int M, int N, int K) { return M >= 2048 && N >= 32 && K >= 32 && K % 4 == 0; }

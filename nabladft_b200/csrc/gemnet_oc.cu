@@ -174,8 +174,9 @@ int output_block(const Ctx& c, const Work& w, int blk, int64_t n, Ext E) {
 
 
 #ifndef NB_EMU
-// Device form of QuadK (gemnet_oc_kernels.cuh; same sums in the same order, so the host-emulation tests of the functor pin this kernel's
-// arithmetic too).  The functor launches one logical thread per (edge, channel): the 32 channel-threads of an edge all recompute the
+// Device form of QuadK (gemnet_oc_kernels.cuh; same sums in the same order, bitwise equal to the functor on the H100 --
+// tests/test_gpu_gemnet_kernels.py checks both against each other and against float64).  The functor launches one logical thread per
+// (edge, channel): the 32 channel-threads of an edge all recompute the
 // geometry of every quadruplet -- two cross products, a square root, a division and the Legendre recurrence, more instructions than the
 // 49 FMAs they feed.  Here a WARP owns the edge (lane =
 // channel): 32 quadruplets at a time, lane j evaluates the dihedral basis of quadruplet j ONCE and stages it in shared memory; the warp
@@ -267,7 +268,8 @@ __global__ void __launch_bounds__(32 * QW_WARPS) k_quad_edges(Graph mn, Graph q,
 }
 #endif
 #ifndef NB_EMU
-// Device form of TripEdgeK (same sums in the same order): a warp owns an output edge, lane = channels (lane, lane + 32); 32 input edges at a time,
+// Device form of TripEdgeK (same sums in the same order, bitwise equal to the functor on the H100; tests/test_gpu_gemnet_kernels.py): a warp
+// owns an output edge, lane = channels (lane, lane + 32); 32 input edges at a time,
 // lane j evaluates the Legendre basis of the angle to input edge j ONCE (the functor's 64 channel-threads each did) and stages it in shared memory.
 constexpr int TW_WARPS = 8;
 __global__ void __launch_bounds__(32 * TW_WARPS) k_trip_edges(Graph o, Graph in, const float* __restrict__ x, const float* __restrict__ R, int32_t ldr,
@@ -609,3 +611,37 @@ extern "C" int nb200_gemnet_oc_debug_h(const void* workspace, const nb200_gemnet
 
 #include "gemnet_oc_train.inc"
 #include "gemnet_oc_jvp.inc"
+
+// One aggregation on caller-built graphs (include/nabla_b200.h), so that the warp-per-edge device kernels can be compared with the functors
+// and with a float64 reference on row shapes the fixture molecules never produce
+extern "C" int nb200_gemnet_oc_test_aggregate(const nb200_gemnet_oc_agg_args* a, void* stream) {
+    if (!a || a->E_bound < 0 || a->E_bound > 0x7fffffff || (a->form != 0 && a->form != 1) || (a->quad != 0 && a->quad != 1) ||
+        (a->tangent != 0 && a->tangent != 1))
+        return NB200_EINVAL;
+    const bool quad = a->quad, tangent = a->tangent;
+    if (a->ldr < (quad ? 32 * NS2 : 16 * NS)) return NB200_EINVAL;
+    if (!a->o_src || !a->o_tgt || !a->o_V || !a->in_ptr || !a->in_src || !a->in_V || !a->x || !a->R || (quad && (!a->o_ptr || !a->q_tin)))
+        return NB200_EINVAL;
+    if (tangent ? (a->E_dev || !a->Vot || !a->Vit || !a->xt || !a->Rt || !a->Ot) : !a->O) return NB200_EINVAL;
+    const Graph o{a->o_ptr, const_cast<int32_t*>(a->o_src), const_cast<int32_t*>(a->o_tgt), nullptr, const_cast<float*>(a->o_V)};
+    const Graph in{a->in_ptr, const_cast<int32_t*>(a->in_src), nullptr, nullptr, const_cast<float*>(a->in_V)};
+    cudaStream_t s = (cudaStream_t)stream;
+    nb200_engine* e = nullptr;
+#ifndef NB_EMU
+    nb200_engine tmp_engine{};  // launch counting only
+    e = &tmp_engine;
+#endif
+    const Ext E(a->E_bound, a->E_dev);
+    if (!tangent) {
+        if (a->form == 0)
+            return quad ? quad_aggregate(e, s, o, in, a->q_tin, a->x, a->R, a->ldr, a->O, E) : trip_edge_aggregate(e, s, o, in, a->x, a->R, a->ldr, a->O, E);
+        return quad ? pfor(e, s, CAT_MSG_FWD, E, QI, QuadK{o, in, a->q_tin, a->x, a->R, a->ldr, a->O})
+                    : pfor(e, s, CAT_MSG_FWD, E, TI, TripEdgeK{o, in, a->x, a->R, a->ldr, a->O});
+    }
+    if (quad) {
+        const QuadTK f{o, in, a->Vot, a->Vit, a->q_tin, a->x, a->xt, a->R, a->Rt, a->ldr, a->Ot};
+        return a->form == 0 ? quad_aggregate_t(e, s, f, a->E_bound) : pfor(e, s, CAT_MSG_FWD, a->E_bound * QI, f);
+    }
+    const TripEdgeTK f{o, in, a->Vot, a->Vit, a->x, a->xt, a->R, a->Rt, a->ldr, a->Ot};
+    return a->form == 0 ? trip_edge_aggregate_t(e, s, f, a->E_bound) : pfor(e, s, CAT_MSG_FWD, a->E_bound * TI, f);
+}
