@@ -271,6 +271,61 @@ int64_t nb200_painn_hvp_workspace_bytes(const nb200_painn_weights* w, int32_t b_
 int nb200_painn_hvp(nb200_engine* eng, const nb200_painn_weights* w, const int32_t* z, const float* pos, const int32_t* mol_ptr,
                     int32_t n_mol, int32_t n_atoms, int32_t e_cap, void* workspace, int64_t workspace_bytes,
                     int32_t n_dir, const float* v, float* energy, float* forces, float* hv, int32_t* status, void* stream);
+/* Test entry point, not a supported API: ONE kernel of the PaiNN tangent / Hessian-vector-product path on caller-built inputs, through the
+ * same host wrapper (hence launch configuration) the engine uses.  F = 128; per-atom arrays [n_atoms, k F] as in the engine; graph as in
+ * the batch layout above.  `op` (NB200_PT_*) selects the kernel and the fields it reads and writes:
+ *   GEOM_TAN          geom row_ptr col v -> t_geom
+ *   MUL_DACT          pre x n -> out                                  (n % 4 == 0)
+ *   ACT_BWD_TAN       t_g (in / out) g_pre pre t_pre n                 (n % 4 == 0)
+ *   READOUT_BWD_TAN   pre t_pre R2 width -> t_g_pre t_act              ([n_atoms, width])
+ *   MSG_FWD_TAN       xh t_xh xh_bias mu t_mu W dW geom t_geom row_ptr col [rev] -> t_q (accumulated) t_mu_out
+ *   UPD_NORM_TAN      VW t_VW nrm -> t_nrm
+ *   UPD_COMBINE_TAN   VW t_VW y t_y -> t_q t_mu (both accumulated)
+ *   UPD_COMBINE_BWD_TAN  g_q t_g_q g_mu t_g_mu y t_y VW t_VW -> t_gy t_gVW
+ *   UPD_NORM_BWD_TAN  gn t_gn VW t_VW nrm t_nrm -> t_gVW (accumulated)
+ *   MSG_BWD_TAN       as MSG_FWD_TAN without t_q, plus g_q t_g_q g_mu t_g_mu -> t_g_xh t_g_mu_in t_gW gWd
+ *   MSG_BWD_HVP       as MSG_BWD_TAN plus d2W, rev required -> t_g_xh t_g_mu_in t_egrad (accumulated)
+ *   EDGE_FORCES_HVP   egrad t_egrad geom t_geom row_ptr rev -> hv
+ *   FILTER_D2         geom status rev sort_scratch + radial fields, e_cap = row stride -> W dW d2W (one row per undirected pair)
+ *   FILTER_WGRAD      geom status sort_scratch + radial fields, e_cap >= status[0]; gW (tan = 0) or t_gW gWd (tan = 1) -> g_w g_b
+ *                     (accumulated; the entry sorts every directed edge by distance bin into sort_scratch first)
+ * `rev` NULL for MSG_FWD_TAN / MSG_BWD_TAN: every edge reads its own filter row; otherwise row min(e, rev[e]).  bf16 = 1 (MSG_FWD_TAN,
+ * MSG_BWD_TAN, FILTER_WGRAD only): W, dW, t_gW, gWd, gW hold bf16.  status = {n_edges, 0} in device memory; sort_scratch int32
+ * [768 + n_edges].  NB200_EINVAL (nothing launched) for an unknown op, a NULL field the op reads or writes, n_atoms < 0, n < 0, n % 4 != 0
+ * for the element-wise ops, width < 1, e_cap < 0, bf16 or tan where the op has no such instance; NB200_EUNSUPPORTED for radial
+ * parameters the filter kernels do not support. */
+enum {
+    NB200_PT_GEOM_TAN = 0, NB200_PT_MUL_DACT, NB200_PT_ACT_BWD_TAN, NB200_PT_READOUT_BWD_TAN, NB200_PT_MSG_FWD_TAN, NB200_PT_UPD_NORM_TAN,
+    NB200_PT_UPD_COMBINE_TAN, NB200_PT_UPD_COMBINE_BWD_TAN, NB200_PT_UPD_NORM_BWD_TAN, NB200_PT_MSG_BWD_TAN, NB200_PT_MSG_BWD_HVP,
+    NB200_PT_EDGE_FORCES_HVP, NB200_PT_FILTER_D2, NB200_PT_FILTER_WGRAD, NB200_PT_N_OPS
+};
+typedef struct nb200_painn_tan_args {
+    int32_t op, bf16, tan, n_atoms;
+    int64_t n;
+    int32_t width, e_cap;
+    const int32_t *row_ptr, *col, *rev, *status;
+    int32_t* sort_scratch;
+    const float *geom, *v;
+    float* t_geom;
+    const float *xh, *t_xh, *xh_bias, *mu;
+    float *t_mu, *t_q, *t_mu_out;
+    void *W, *dW;
+    float* d2W;
+    const float *g_q, *t_g_q, *g_mu, *t_g_mu;
+    float *t_g_xh, *t_g_mu_in;
+    void *gW, *t_gW, *gWd;
+    const float *VW, *t_VW, *nrm, *y, *t_y, *gn, *t_gn;
+    float *t_nrm, *t_gy, *t_gVW;
+    const float *pre, *t_pre, *x, *g_pre, *R2;
+    float *out, *t_g, *t_g_pre, *t_act;
+    const float* egrad;
+    float *t_egrad, *hv;
+    int32_t radial_mode, n_rbf, n_layers;
+    float cutoff, rbf_coeff, rbf_xscale, sign;
+    const float *rbf_offsets, *w_rbf, *b_rbf;
+    float *g_w, *g_b;
+} nb200_painn_tan_args;
+int nb200_painn_test_tangent(const nb200_painn_tan_args* args, void* stream);
 
 /* ----------------------------------------------------------------------------------------
  * SchNet energy + forces (config/model/schnet.yaml: schnetpack.representation.SchNet inside

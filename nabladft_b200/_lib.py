@@ -80,6 +80,23 @@ class GemNetOCAggArgs(ctypes.Structure):
                 ("xt", c_void_p), ("Rt", c_void_p), ("Ot", c_void_p)]
 
 
+class PainnTanArgs(ctypes.Structure):
+    """Mirror of `struct nb200_painn_tan_args` (include/nabla_b200.h)."""
+
+    _fields_ = [("op", c_int32), ("bf16", c_int32), ("tan", c_int32), ("n_atoms", c_int32), ("n", c_int64), ("width", c_int32), ("e_cap", c_int32)] + [
+        (name, c_void_p) for name in (
+            "row_ptr", "col", "rev", "status", "sort_scratch", "geom", "v", "t_geom", "xh", "t_xh", "xh_bias", "mu", "t_mu", "t_q", "t_mu_out",
+            "W", "dW", "d2W", "g_q", "t_g_q", "g_mu", "t_g_mu", "t_g_xh", "t_g_mu_in", "gW", "t_gW", "gWd", "VW", "t_VW", "nrm", "y", "t_y",
+            "gn", "t_gn", "t_nrm", "t_gy", "t_gVW", "pre", "t_pre", "x", "g_pre", "R2", "out", "t_g", "t_g_pre", "t_act", "egrad", "t_egrad", "hv")
+    ] + [("radial_mode", c_int32), ("n_rbf", c_int32), ("n_layers", c_int32), ("cutoff", c_float), ("rbf_coeff", c_float), ("rbf_xscale", c_float),
+         ("sign", c_float), ("rbf_offsets", c_void_p), ("w_rbf", c_void_p), ("b_rbf", c_void_p), ("g_w", c_void_p), ("g_b", c_void_p)]
+
+
+# nb200_painn_test_tangent ops (enum NB200_PT_*)
+PT_OPS = ("GEOM_TAN", "MUL_DACT", "ACT_BWD_TAN", "READOUT_BWD_TAN", "MSG_FWD_TAN", "UPD_NORM_TAN", "UPD_COMBINE_TAN", "UPD_COMBINE_BWD_TAN",
+          "UPD_NORM_BWD_TAN", "MSG_BWD_TAN", "MSG_BWD_HVP", "EDGE_FORCES_HVP", "FILTER_D2", "FILTER_WGRAD")
+
+
 class DimeNetWeights(ctypes.Structure):
     """Mirror of `struct nb200_dimenet_weights` (include/nabla_b200.h)."""
 
@@ -168,6 +185,7 @@ SIGNATURES = {
     "nb200_painn_hvp_workspace_bytes": (c_int64, [POINTER(PainnWeights), c_int32, c_int32, c_int32, c_int32]),
     "nb200_painn_hvp": (c_int32, [c_void_p, POINTER(PainnWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,
                                   c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_painn_test_tangent": (c_int32, [POINTER(PainnTanArgs), c_void_p]),
 
     "nb200_gemnet_oc_graph_bytes": (c_int64, [c_int32, c_int32]),
     "nb200_gemnet_oc_graph_count": (c_int32, [POINTER(GemNetOCWeights), c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,
