@@ -79,7 +79,7 @@ def main():
 
         batch = D()
         batch.z, batch.pos, batch.batch = z.long(), pos, bt
-    eng, zi, posf, mol_ptr, n_mol = vib._engine_inputs(model, batch)
+    eng, zi, posf, mol_ptr, n_mol = model.engine_inputs(batch)
     ptr = mol_ptr.cpu().tolist()
     n_max = max(b - a for a, b in zip(ptr[:-1], ptr[1:]))
     n_dir = 3 * n_max
@@ -198,7 +198,7 @@ def dimenet_main(args):
     batch.z = torch.from_numpy(b["z"]).long().to(dev)
     batch.pos = torch.from_numpy(b["pos"]).to(dev)
     batch.batch = torch.from_numpy(b["batch"]).to(dev)
-    runner, zi, posf, mol_ptr, n_mol = vib._engine_inputs(model, batch)
+    runner, zi, posf, mol_ptr, n_mol = model.engine_inputs(batch)
     ptr = mol_ptr.cpu().tolist()
     n_max = max(q - p for p, q in zip(ptr[:-1], ptr[1:]))
     n_dir = 3 * n_max
@@ -292,7 +292,7 @@ def gemnet_main(args):
         return d
 
     batch = make_batch(args.batch)
-    runner, zi, posf, mol_ptr, n_mol = vib._engine_inputs(model, batch)
+    runner, zi, posf, mol_ptr, n_mol = model.engine_inputs(batch)
     ptr = mol_ptr.cpu().tolist()
     n_max = max(q - p for p, q in zip(ptr[:-1], ptr[1:]))
     n_dir = 3 * n_max
@@ -348,7 +348,7 @@ def gemnet_main(args):
 
     def ws_bytes(n_mol_):
         d = make_batch(n_mol_)
-        _, z_, p_, mp_, nm_ = vib._engine_inputs(model, d)
+        _, z_, p_, mp_, nm_ = model.engine_inputs(d)
         pt = mp_.cpu()
         _, cnt = runner._graph(p_, mp_, nm_, int((pt[1:] - pt[:-1]).max()))
         return runner._bytes("nb200_gemnet_oc_jvp_workspace_bytes", ctypes.byref(runner._w), nm_, int(z_.numel()), cnt)

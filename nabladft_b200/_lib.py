@@ -333,3 +333,44 @@ class EngineDriver:
         for t, n in ((seed, n_mol), (force_seed, 3 * n_atoms)):
             if t is not None and not (t.device == device and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == n):
                 raise NablaB200Error("seeds must be contiguous fp32 tensors [n_mol] / [n_atoms, 3] on the batch's device")
+
+    def _directions(self, v, n_atoms: int, device):
+        """The directions of a Hessian-vector-product call, v [n_atoms, 3] or [n_dir, n_atoms, 3], as [n_dir, n_atoms, 3]."""
+        if v.dim() == 2:
+            v = v.unsqueeze(0)
+        if not (self._on_device(v) and v.device == device and v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3
+                and v.shape[1:] == (n_atoms, 3) and v.shape[0] >= 1):
+            raise NablaB200Error(f"run_hvp(): v must be a contiguous fp32 CUDA tensor [n_dir, {n_atoms}, 3] with n_dir >= 1 on {device}")
+        return v
+
+    # ---- forwards sized by per-batch upper bounds (DimeNet++, GemNet-OC): the C calls `<prefix>_count_bounds`, `<prefix>_graph_bytes`,
+    # `<prefix>_workspace_bytes` and `<prefix>_energy_forces_async` on the weights the driver binds as `_w`
+    def _count_bounds(self, prefix: str, sizes, n_counts: int):
+        """Upper bounds of the `n_counts` counts for molecules of `sizes` atoms (host, `<prefix>_count_bounds`): they hold for every geometry."""
+        if self._w is None:
+            raise NablaB200Error(f"{type(self).__name__}.count_bounds before set_weights")
+        mol_ptr = (c_int32 * (len(sizes) + 1))(0, *[int(v) for v in torch.as_tensor(sizes).cumsum(0)])
+        bounds = (c_int64 * n_counts)()
+        check(getattr(self.lib, prefix + "_count_bounds")(byref(self._w), mol_ptr, len(sizes), bounds), prefix + "_count_bounds")
+        return bounds
+
+    def _launch_bounded(self, prefix: str, z, pos, mol_ptr, n_mol: int, bounds, *size_args):
+        """Asynchronous forward (`<prefix>_energy_forces_async`): one enqueue on the current stream, no host read.  -> (energy, forces,
+        status); `status` is a device int32[8] that the next launch rewrites (include/nabla_b200.h).  `size_args`: the per-batch sizes the
+        call takes after n_atoms (GemNet-OC: the largest molecule); the graph buffer holds `self._graph_bytes(n_atoms, *size_args)` bytes.
+        Graph buffer and workspace are sized by n_atoms and `bounds`, hence once per batch: later launches of the same batch reuse them."""
+        if self._w is None:
+            raise NablaB200Error(f"{type(self).__name__}.launch before set_weights")
+        n, dev = int(z.shape[0]), pos.device
+        gbytes = self._graph_bytes(n, *size_args)
+        self.last_workspace_bytes = self._bytes(prefix + "_workspace_bytes", byref(self._w), n_mol, n, bounds)
+        gbuf, ws = self._buffer("_graph_buf", gbytes, dev), self._buffer("_ws", self.last_workspace_bytes, dev)
+        if self._status is None or self._status.device != dev:
+            self._status = torch.zeros(8, dtype=torch.int32, device=dev)
+        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
+        forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        check(getattr(self.lib, prefix + "_energy_forces_async")(
+            self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, *size_args, gbuf.data_ptr(), gbuf.numel(),
+            bounds, ws.data_ptr(), ws.numel(), energy.data_ptr(), forces.data_ptr(), self._status.data_ptr(), self._stream()),
+            prefix + "_energy_forces_async")
+        return energy, forces, self._status

@@ -19,7 +19,7 @@ asynchronous call, sized by per-batch upper bounds of the edge and triplet count
 fallback: CPU tensors raise NablaB200Error in eval mode and NotImplementedError in training mode.
 """
 import ctypes
-from ctypes import POINTER, byref, c_int32, c_int64
+from ctypes import POINTER, byref, c_int64
 from typing import Dict, List, Optional, Tuple
 
 import numpy as np
@@ -28,6 +28,7 @@ from torch import nn
 
 from . import _lib
 from ._lib import DimeNetWeights, EngineDriver, NablaB200Error, check
+from .engine import BoundedEngine, refuse_training
 
 # ---- canonical layout: keep in step with the enums of include/nabla_b200.h -----------------------------------------------------------------
 G_NAMES = ["FREQ", "ZEROS", "NORMS", "EMB_TI", "EMB_TJ", "EMB_RBF_W", "EMB_RBF_B", "EMB_W3", "HEAD_W0", "HEAD_B0", "HEAD_W1", "HEAD_B1",
@@ -221,9 +222,7 @@ class DimeNetPlusPlusPotential(nn.Module):
 
     def run(self, z, pos, batch):
         """-> (energy [B], forces [N,3], graph embeddings [B, node_latent_dim])."""
-        if not pos.is_cuda:
-            raise NablaB200Error("DimeNetPlusPlusPotential runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
-        runner = self._get_runner()
+        runner = self._cuda_runner(pos)
         self._sync_weights(runner, pos.device)
         return runner.run(*self.batch_args(z, pos, batch))
 
@@ -232,6 +231,19 @@ class DimeNetPlusPlusPotential(nn.Module):
         if self._engine is None:
             self._engine = DimeNetEngine(self, self._get_runner())
         return self._engine
+
+    def engine_inputs(self, data):
+        """(runner, z int32, pos fp32, mol_ptr int32, n_mol) of `data` for the inference engine, with the weights synced: the inputs of
+        `DimeNetRunner.run_hvp` (`vibrations`)."""
+        runner = self._cuda_runner(data.pos)
+        refuse_training(self)
+        self._sync_weights(runner, data.pos.device)
+        return (runner, *self.batch_args(data.z, data.pos, data.batch))
+
+    def _cuda_runner(self, pos) -> "DimeNetRunner":
+        if not pos.is_cuda:
+            raise NablaB200Error("DimeNetPlusPlusPotential runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
+        return self._get_runner()
 
     def _get_runner(self) -> "DimeNetRunner":
         if self._runner is None:
@@ -297,41 +309,25 @@ class DimeNetRunner(EngineDriver):
         lib, n = self.lib, int(z.shape[0])
         if n == 0 or n_mol == 0:
             raise NablaB200Error("DimeNetPlusPlusPotential: empty batch")
-        gbuf = self._buffer("_graph_buf", self._bytes("nb200_dimenet_graph_bytes", byref(self._w), n), pos.device)
+        gbuf = self._buffer("_graph_buf", self._graph_bytes(n), pos.device)
         counts = (c_int64 * N_COUNTS)()
         check(lib.nb200_dimenet_graph_count(byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, gbuf.data_ptr(), gbuf.numel(),
                                             counts, self._stream()), "nb200_dimenet_graph_count")
         self.last_counts = {"edges": int(counts[0]), "triplets": int(counts[1])}
         return gbuf, counts
 
+    def _graph_bytes(self, n: int) -> int:
+        return self._bytes("nb200_dimenet_graph_bytes", byref(self._w), n)
+
     def count_bounds(self, sizes):
         """Upper bounds of {edges, triplet slots} for molecules of `sizes` atoms (host, nb200_dimenet_count_bounds): they hold for every
         geometry, see DESIGN.md 3.15.3."""
-        if self._w is None:
-            raise NablaB200Error("DimeNetRunner.count_bounds before set_weights / bind")
-        mol_ptr = (c_int32 * (len(sizes) + 1))(0, *[int(v) for v in torch.as_tensor(sizes).cumsum(0)])
-        bounds = (c_int64 * N_COUNTS)()
-        check(self.lib.nb200_dimenet_count_bounds(byref(self._w), mol_ptr, len(sizes), bounds), "nb200_dimenet_count_bounds")
-        return bounds
+        return self._count_bounds("nb200_dimenet", sizes, N_COUNTS)
 
     def launch(self, z, pos, mol_ptr, n_mol: int, bounds):
-        """Asynchronous forward (nb200_dimenet_energy_forces_async): one enqueue on the current stream, no host read.  -> (energy, forces,
-        status); `status` is a device int32[8] that the next launch rewrites (include/nabla_b200.h).  Graph buffer and workspace are sized by
-        n_atoms and `bounds` (count_bounds), hence once per batch: later launches of the same batch reuse them."""
-        if self._w is None:
-            raise NablaB200Error("DimeNetRunner.launch before set_weights / bind")
-        lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        gbytes = self._bytes("nb200_dimenet_graph_bytes", byref(self._w), n)
-        self.last_workspace_bytes = self._bytes("nb200_dimenet_workspace_bytes", byref(self._w), n_mol, n, bounds)
-        gbuf, ws = self._buffer("_graph_buf", gbytes, dev), self._buffer("_ws", self.last_workspace_bytes, dev)
-        if self._status is None or self._status.device != dev:
-            self._status = torch.zeros(8, dtype=torch.int32, device=dev)
-        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
-        forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        check(lib.nb200_dimenet_energy_forces_async(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n,
-                                                    gbuf.data_ptr(), gbuf.numel(), bounds, ws.data_ptr(), ws.numel(), energy.data_ptr(),
-                                                    forces.data_ptr(), self._status.data_ptr(), self._stream()), "nb200_dimenet_energy_forces_async")
-        return energy, forces, self._status
+        """Asynchronous forward (nb200_dimenet_energy_forces_async) sized by n_atoms and `bounds` (count_bounds): see
+        `EngineDriver._launch_bounded`."""
+        return self._launch_bounded("nb200_dimenet", z, pos, mol_ptr, n_mol, bounds)
 
     def train_grads(self, z, pos, mol_ptr, n_mol: int, seed_energy: Optional[torch.Tensor], seed_forces: Optional[torch.Tensor]) -> torch.Tensor:
         """d(sum_m seed_energy[m] E_m + sum_i seed_forces[i] . F_i)/d(flat weight buffer), in the buffer's layout (nb200_dimenet_train_grads).
@@ -357,10 +353,7 @@ class DimeNetRunner(EngineDriver):
         if self._w is None:
             raise NablaB200Error("DimeNetRunner.run_hvp before set_weights / bind")
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        if v.dim() == 2:
-            v = v.unsqueeze(0)
-        if not (v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n, 3) and v.shape[0] >= 1 and v.device == dev):
-            raise NablaB200Error(f"run_hvp(): v must be a contiguous fp32 tensor [n_dir, {n}, 3] with n_dir >= 1 on {dev}")
+        v = self._directions(v, n, dev)
         n_dir = int(v.shape[0])
         gbuf, counts = self._graph(z, pos, mol_ptr, n_mol)
         ws = self._buffer("_ws", self._bytes("nb200_dimenet_hvp_workspace_bytes", byref(self._w), n_mol, n, counts), dev)
@@ -373,55 +366,12 @@ class DimeNetRunner(EngineDriver):
         return energy, forces, hv
 
 
-class DimeNetEngine:
-    """What `optimization.ASEBatchwiseLBFGS` and `md.BatchwiseMD` need from a model, with `PainnEngine`'s method names: `run` (synchronous,
-    validates), `launch` (asynchronous), `e_cap`, `raise_on_status`.  There is no edge capacity to grow (`grows_capacity` is False): `run`
-    derives upper bounds of the edge and triplet counts from the molecule sizes of the batch, and `launch` sizes everything by them (`e_cap`
-    is accepted and ignored).  A count above its bound is therefore a bug, not a reason to retry."""
+class DimeNetEngine(BoundedEngine):
+    """`BoundedEngine` of DimeNet++: edge and triplet-slot bounds."""
 
-    grows_capacity = False
-
-    def __init__(self, model: DimeNetPlusPlusPotential, runner: DimeNetRunner):
-        self.model, self.runner, self.e_cap = model, runner, 0
-        self._batch = None
-        self.last_status = None
-
-    def run(self, z, pos, mol_ptr, n_mol: int):
-        """First evaluation of a batch: checks `mol_ptr` on the host (once, not per step), fixes the batch's bounds, launches and validates.
-        -> (energy, forces, status words on the host)."""
-        ptr_host = mol_ptr.cpu()
-        sizes = ptr_host[1:] - ptr_host[:-1]
-        if len(sizes) != n_mol or n_mol < 1 or int(ptr_host[0]) != 0 or int(sizes.min()) < 1 or int(ptr_host[-1]) != z.shape[0]:
-            raise NablaB200Error("DimeNet++: `mol_ptr` must hold n_mol + 1 increasing atom offsets starting at 0 (atoms of a molecule contiguous)")
-        self.model._sync_weights(self.runner, pos.device)
-        self._batch = ((mol_ptr.data_ptr(), n_mol, int(z.shape[0])), self.runner.count_bounds(sizes))
-        energy, forces, status = self.launch(z, pos, mol_ptr, n_mol)
-        host = status.cpu()
-        self.raise_on_status(host)
-        self.last_status = host
-        return energy, forces, host
-
-    def launch(self, z, pos, mol_ptr, n_mol: int, e_cap=None):
-        if self._batch is None or self._batch[0] != (mol_ptr.data_ptr(), n_mol, int(z.shape[0])):
-            raise NablaB200Error("DimeNetEngine.launch: call run() on this batch first (it derives the bounds the launch is sized by)")
-        return self.runner.launch(z, pos, mol_ptr, n_mol, self._batch[1])
-
-    @property
-    def bounds(self) -> Dict[str, int]:
-        return {"edges": int(self._batch[1][0]), "triplets": int(self._batch[1][1])} if self._batch else {}
-
-    @staticmethod
-    def raise_on_status(status_host) -> None:
-        """`status_host`: the status words of a launch on the host (the first four suffice).  Atoms without neighbours are not an error."""
-        n_edges, err, max_deg, n_iso = (int(v) for v in status_host[:4])
-        if err == -4:
-            raise NablaB200Error(f"NB200_ECAPACITY: a count exceeds its bound ({n_edges} edges); `mol_ptr` changed under the engine?")
-        if err == -1:
-            raise NablaB200Error("DimeNet++: atomic number outside [0, 94] or non-finite atom coordinates")
-        if err != 0:
-            from ._lib import ERRORS
-
-            raise NablaB200Error(f"DimeNet++ graph construction failed: {ERRORS.get(err, err)} (max in-degree {max_deg}, {n_iso} atoms without neighbours)")
+    label = "DimeNet++"
+    einval_text = "atomic number outside [0, 94] or non-finite atom coordinates"
+    count_names = ("edges", "triplets")
 
 
 class DimeNetEnergyFn(torch.autograd.Function):

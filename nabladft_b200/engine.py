@@ -1,4 +1,5 @@
-"""Host-side driver of the PaiNN energy+forces engine (`nb200_painn_energy_forces`).
+"""Host-side driver of the PaiNN energy+forces engine (`nb200_painn_energy_forces`), and `BoundedEngine`, the same interface for the
+forwards sized by per-batch upper bounds (DimeNet++, GemNet-OC).
 
 Owns: the C engine object, the device workspace, the canonical weight export.
 The model classes (`painn_oc.PaiNN`, `spk.NeuralNetworkPotential`) only describe how their
@@ -251,11 +252,7 @@ class PainnEngine(EngineDriver):
         n_atoms, dev = z.shape[0], z.device
         if not (self._on_device(z) and z.dtype == torch.int32 and pos.dtype == torch.float32 and mol_ptr.dtype == torch.int32):
             raise NablaB200Error("run_hvp(): need CUDA int32 z / mol_ptr and fp32 pos")
-        if v.dim() == 2:
-            v = v.unsqueeze(0)
-        if not (self._on_device(v) and v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n_atoms, 3)
-                and v.shape[0] >= 1):
-            raise NablaB200Error("run_hvp(): v must be a contiguous fp32 CUDA tensor [n_dir, n_atoms, 3] with n_dir >= 1")
+        v = self._directions(v, n_atoms, dev)
         n_dir = v.shape[0]
         self._kept_token = 0  # this call overwrites the workspace a kept training forward lives in
         if self.kind == "schnet":
@@ -334,6 +331,75 @@ class PainnEngine(EngineDriver):
         if the guess was too small (the only host<->device sync of the whole path)."""
         (energy, forces, _), st = self._regrow(lambda: self.launch(z, pos, mol_ptr, n_mol, with_forces))
         return energy, forces, st
+
+
+class BoundedEngine:
+    """What `optimization.ASEBatchwiseLBFGS` and `md.BatchwiseMD` need from a model whose forward is sized by per-batch upper bounds, with
+    `PainnEngine`'s method names.  `run` derives the bounds from the molecule sizes and `launch` sizes everything by them (`e_cap` is ignored):
+    there is no capacity to grow, and a count above its bound is a bug.  A model's subclass (`DimeNetEngine`, `GemNetOCEngine`) declares
+    `label` and `einval_text` for messages, the `count_names` behind `bounds`, and may refine `check_sizes` and `size_args`."""
+
+    grows_capacity = False
+
+    def __init__(self, model, runner):
+        self.model, self.runner, self.e_cap = model, runner, 0
+        self._batch = None
+        self.last_status = None
+
+    @staticmethod
+    def check_sizes(model, max_atoms: int) -> None:
+        """Host check of the largest molecule of a batch (the bounds refuse counts past int32)."""
+
+    @staticmethod
+    def size_args(max_atoms: int) -> tuple:
+        """What the runner's `launch` takes between n_mol and the bounds."""
+        return ()
+
+    def run(self, z, pos, mol_ptr, n_mol: int):
+        """First evaluation of a batch: checks the batch on the host (once, not per step), fixes its bounds, launches and validates.
+        -> (energy, forces, status words on the host)."""
+        ptr_host = mol_ptr.cpu()
+        sizes = ptr_host[1:] - ptr_host[:-1]
+        if len(sizes) != n_mol or n_mol < 1 or int(ptr_host[0]) != 0 or int(sizes.min()) < 1 or int(ptr_host[-1]) != z.shape[0]:
+            raise NablaB200Error(f"{self.label}: `mol_ptr` must hold n_mol + 1 increasing atom offsets starting at 0 (atoms of a molecule "
+                                 "contiguous)")
+        max_atoms = int(sizes.max())
+        self.check_sizes(self.model, max_atoms)
+        self.model._sync_weights(self.runner, pos.device)
+        self._batch = ((mol_ptr.data_ptr(), n_mol, int(z.shape[0])), *self.size_args(max_atoms), self.runner.count_bounds(sizes))
+        energy, forces, status = self.launch(z, pos, mol_ptr, n_mol)
+        host = status.cpu()
+        self.raise_on_status(host)
+        self.last_status = host
+        return energy, forces, host
+
+    def launch(self, z, pos, mol_ptr, n_mol: int, e_cap=None):
+        if self._batch is None or self._batch[0] != (mol_ptr.data_ptr(), n_mol, int(z.shape[0])):
+            raise NablaB200Error(f"{type(self).__name__}.launch: call run() on this batch first (it derives the bounds the launch is sized by)")
+        return self.runner.launch(z, pos, mol_ptr, n_mol, *self._batch[1:])
+
+    @property
+    def bounds(self) -> Dict[str, int]:
+        return {k: int(self._batch[-1][i]) for i, k in enumerate(self.count_names)} if self._batch else {}
+
+    @classmethod
+    def raise_on_status(cls, status_host) -> None:
+        """`status_host`: the status words of a launch on the host; the first four read like `PainnEngine`'s.  Atoms without neighbours are
+        not an error."""
+        n_edges, err, max_deg, n_iso = (int(v) for v in status_host[:4])
+        if err == -4:
+            raise NablaB200Error(f"NB200_ECAPACITY: a count exceeds its bound ({n_edges} edges); `mol_ptr` changed under the engine?")
+        if err == -1:
+            raise NablaB200Error(f"{cls.label}: {cls.einval_text}")
+        if err != 0:
+            raise NablaB200Error(f"{cls.label} graph construction failed: {_lib.ERRORS.get(err, err)} (max degree {max_deg}, {n_iso} atoms "
+                                 "without neighbours)")
+
+
+def refuse_training(model) -> None:
+    """Hessian-vector products run through the inference engine: refuse a model in training mode with autograd on."""
+    if model.training and torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters()):
+        raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
 
 
 def mol_ptr_from_batch(batch: torch.Tensor, n_mol: Optional[int] = None) -> Tuple[torch.Tensor, int]:

@@ -23,7 +23,7 @@ STATUS (round 1): every kernel has been checked against the oracle through the h
 import ctypes
 import math
 import re
-from ctypes import POINTER, byref, c_float, c_int32, c_int64
+from ctypes import POINTER, byref, c_float, c_int64
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -31,6 +31,7 @@ from torch import nn
 
 from . import _lib
 from ._lib import EngineDriver, GemNetOCWeights, NablaB200Error, check
+from .engine import BoundedEngine, refuse_training
 
 # ---- canonical layout: keep in step with the enums of include/nabla_b200.h (tests/test_host.py compares the names) -------------------
 G_NAMES = ["RBF_OFFSET", "EMB", "CAT_MAIN", "CAT_AE", "CAT_Q", "CAT_A2A", "EDGE_EMB", "OUT_E0", "OUT_E_RES", "OUT_ENERGY", "OUT_F0", "OUT_F_RES",
@@ -240,6 +241,8 @@ class GemNetOC(nn.Module):
         if bad:
             raise NablaB200Error("GemNetOC: configuration outside the compiled path (config/model/gemnet-oc.yaml): " + "; ".join(bad))
         self.num_blocks, self.cutoff, self.num_elements = num_blocks, float(cutoff), num_elements
+        # the forces are a direct output of the model, not the gradient of its energy (`md.BatchwiseMD` refuses such a model)
+        self.regress_forces, self.direct_forces = regress_forces, direct_forces
         self.max_neighbors = max_neighbors
         self.max_neighbors_qint = max_neighbors_qint or max_neighbors
         self.max_neighbors_aeaint = max_neighbors_aeaint or max_neighbors
@@ -370,13 +373,24 @@ class GemNetOC(nn.Module):
     # ---- forward ------------------------------------------------------------------------------------------------------------------------
     def forward(self, data):
         """data.z [N], data.pos [N,3], data.batch [N] (sorted) -> (E_t [B], F_t [N,3])   (gemnet_oc.py:1121-1251)."""
-        pos = data.pos
-        if not pos.is_cuda:
-            raise NablaB200Error("GemNetOC runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
-        runner = self._get_runner()
+        runner = self._cuda_runner(data.pos)
         if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             return self._train_with(runner, data)
         return self._forward_with(runner, data)
+
+    def engine_inputs(self, data):
+        """(runner, z int32, pos fp32, mol_ptr int32, n_mol) of `data` for the inference engine, with the weights synced: the inputs of
+        `GemNetOCRunner.run_hvp` (`vibrations`)."""
+        runner = self._cuda_runner(data.pos)
+        refuse_training(self)
+        self._sync_weights(runner, data.pos.device)
+        z, pos, mol_ptr, n_mol, _ = self._batch_args(data)
+        return runner, z, pos, mol_ptr, n_mol
+
+    def _cuda_runner(self, pos) -> "GemNetOCRunner":
+        if not pos.is_cuda:
+            raise NablaB200Error("GemNetOC runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
+        return self._get_runner()
 
     def _get_runner(self) -> "GemNetOCRunner":
         if self._runner is None:
@@ -403,9 +417,7 @@ class GemNetOC(nn.Module):
         if bool((batch[1:] < batch[:-1]).any()):
             raise NablaB200Error("GemNetOC: `batch` must be sorted (atoms of a molecule contiguous), as PyG collation produces it")
         max_atoms = int(counts.max().item())
-        if max_atoms - 1 > self.max_neighbors_aint:
-            raise NablaB200Error(f"GemNetOC: a molecule has {max_atoms} atoms, more than max_neighbors_aint + 1 = {self.max_neighbors_aint + 1}; "
-                                 "the atom-atom graph of the compiled path keeps every in-cutoff pair")
+        GemNetOCEngine.check_sizes(self, max_atoms)
         mol_ptr = torch.zeros(n_mol + 1, dtype=torch.int32, device=pos.device)
         mol_ptr[1:] = torch.cumsum(counts, 0)
         return z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr, n_mol, max_atoms
@@ -447,12 +459,15 @@ class GemNetOCRunner(EngineDriver):
     def _graph(self, pos, mol_ptr, n_mol: int, max_atoms_per_mol: int, attr: str = "_graph_buf"):
         """Phase one of a two-phase call: the four graphs in the buffer `self.<attr>` and their counts (one synchronisation)."""
         n = int(pos.shape[0])
-        gbuf = self._buffer(attr, self._bytes("nb200_gemnet_oc_graph_bytes", n, max_atoms_per_mol), pos.device)
+        gbuf = self._buffer(attr, self._graph_bytes(n, max_atoms_per_mol), pos.device)
         counts = (c_int64 * N_COUNTS)()
         check(self.lib.nb200_gemnet_oc_graph_count(byref(self._w), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol, gbuf.data_ptr(),
                                                    gbuf.numel(), counts, self._stream()), "nb200_gemnet_oc_graph_count")
         self.last_counts = {k: int(counts[i]) for i, k in enumerate(C_NAMES)}
         return gbuf, counts
+
+    def _graph_bytes(self, n: int, max_atoms_per_mol: int) -> int:
+        return self._bytes("nb200_gemnet_oc_graph_bytes", n, max_atoms_per_mol)
 
     def run_train(self, z, pos, mol_ptr, n_mol: int, max_atoms_per_mol: int, seed_energy=None, seed_forces=None, keep: bool = False):
         """nb200_gemnet_oc_energy_forces_grads with the weights bound by set_weights_from.
@@ -493,10 +508,7 @@ class GemNetOCRunner(EngineDriver):
         if self._w is None:
             raise NablaB200Error("GemNetOCRunner.run_hvp before set_weights")
         lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        if v.dim() == 2:
-            v = v.unsqueeze(0)
-        if not (v.dtype == torch.float32 and v.is_contiguous() and v.dim() == 3 and v.shape[1:] == (n, 3) and v.shape[0] >= 1 and v.device == dev):
-            raise NablaB200Error(f"run_hvp(): v must be a contiguous fp32 tensor [n_dir, {n}, 3] with n_dir >= 1 on {dev}")
+        v = self._directions(v, n, dev)
         n_dir = int(v.shape[0])
         ptr_host = mol_ptr.cpu()
         max_atoms = int((ptr_host[1:] - ptr_host[:-1]).max())
@@ -547,86 +559,33 @@ class GemNetOCRunner(EngineDriver):
             return energy, forces, h
         return energy, forces
 
-
     def count_bounds(self, sizes):
         """Upper bounds of the five counts for molecules of `sizes` atoms (host): they hold for every geometry, see DESIGN.md 3.9."""
-        if self._w is None:
-            raise NablaB200Error("GemNetOCRunner.count_bounds before set_weights")
-        mol_ptr = (c_int32 * (len(sizes) + 1))(0, *[int(v) for v in torch.as_tensor(sizes).cumsum(0)])
-        bounds = (c_int64 * N_COUNTS)()
-        check(self.lib.nb200_gemnet_oc_count_bounds(byref(self._w), mol_ptr, len(sizes), bounds), "nb200_gemnet_oc_count_bounds")
-        return bounds
+        return self._count_bounds("nb200_gemnet_oc", sizes, N_COUNTS)
 
     def launch(self, z, pos, mol_ptr, n_mol: int, max_atoms_per_mol: int, bounds):
-        """Asynchronous forward: one enqueue on the current stream, no host read.  -> (energy, forces, status); `status` is a device int32[8]
-        that the next launch rewrites (include/nabla_b200.h).  Graph buffer and workspace are sized by `bounds` (count_bounds), hence once per
-        batch: later launches of the same batch reuse them."""
-        if self._w is None:
-            raise NablaB200Error("GemNetOCRunner.launch before set_weights")
-        lib, n, dev = self.lib, int(z.shape[0]), pos.device
-        gbytes = self._bytes("nb200_gemnet_oc_graph_bytes", n, max_atoms_per_mol)
-        self.last_workspace_bytes = self._bytes("nb200_gemnet_oc_workspace_bytes", byref(self._w), n_mol, n, bounds)
-        gbuf, ws = self._buffer("_graph_buf", gbytes, dev), self._buffer("_ws", self.last_workspace_bytes, dev)
-        if self._status is None or self._status.device != dev:
-            self._status = torch.zeros(N_COUNTS, dtype=torch.int32, device=dev)
-        energy = torch.empty(n_mol, dtype=torch.float32, device=dev)
-        forces = torch.empty(n, 3, dtype=torch.float32, device=dev)
-        check(lib.nb200_gemnet_oc_energy_forces_async(self._h, byref(self._w), z.data_ptr(), pos.data_ptr(), mol_ptr.data_ptr(), n_mol, n, max_atoms_per_mol,
-                                                      gbuf.data_ptr(), gbuf.numel(), bounds, ws.data_ptr(), ws.numel(), energy.data_ptr(), forces.data_ptr(),
-                                                      self._status.data_ptr(), self._stream()), "nb200_gemnet_oc_energy_forces_async")
-        return energy, forces, self._status
+        """Asynchronous forward (nb200_gemnet_oc_energy_forces_async) sized by n_atoms, the largest molecule and `bounds` (count_bounds):
+        see `EngineDriver._launch_bounded`."""
+        return self._launch_bounded("nb200_gemnet_oc", z, pos, mol_ptr, n_mol, bounds, max_atoms_per_mol)
 
 
-class GemNetOCEngine:
-    """What `optimization.ASEBatchwiseLBFGS` needs from a model, with `PainnEngine`'s method names: `run` (synchronous, validates),
-    `launch` (asynchronous), `e_cap`, `raise_on_status`.  There is no edge capacity to grow here: `run` derives upper bounds of the edge counts
-    from the molecule sizes of the batch, and `launch` sizes everything by them (`e_cap` is accepted and ignored)."""
+class GemNetOCEngine(BoundedEngine):
+    """`BoundedEngine` of GemNet-OC: bounds of the five counts; the launch also takes the largest molecule."""
 
-    def __init__(self, model: GemNetOC, runner: GemNetOCRunner):
-        self.model, self.runner, self.e_cap = model, runner, 0
-        self._batch = None
-        self.last_status = None
-
-    def run(self, z, pos, mol_ptr, n_mol: int):
-        """First evaluation of a batch: checks the batch on the host (once, not per step), fixes its bounds, launches and validates.
-        -> (energy, forces, status words on the host)."""
-        ptr_host = mol_ptr.cpu()
-        sizes = ptr_host[1:] - ptr_host[:-1]
-        if len(sizes) != n_mol or n_mol < 1 or int(ptr_host[0]) != 0 or int(sizes.min()) < 1 or int(ptr_host[-1]) != z.shape[0]:
-            raise NablaB200Error("GemNetOC: `mol_ptr` must hold n_mol + 1 increasing atom offsets starting at 0 (atoms of a molecule contiguous)")
-        max_atoms = int(sizes.max())
-        if max_atoms - 1 > self.model.max_neighbors_aint:
-            raise NablaB200Error(f"GemNetOC: a molecule has {max_atoms} atoms, more than max_neighbors_aint + 1 = {self.model.max_neighbors_aint + 1}; "
-                                 "the atom-atom graph of the compiled path keeps every in-cutoff pair")
-        self.model._sync_weights(self.runner, pos.device)
-        self._batch = ((mol_ptr.data_ptr(), n_mol, int(z.shape[0])), max_atoms, self.runner.count_bounds(sizes))
-        energy, forces, status = self.launch(z, pos, mol_ptr, n_mol)
-        host = status.cpu()
-        self.raise_on_status(host)
-        self.last_status = host
-        return energy, forces, host
-
-    def launch(self, z, pos, mol_ptr, n_mol: int, e_cap=None):
-        if self._batch is None or self._batch[0] != (mol_ptr.data_ptr(), n_mol, int(z.shape[0])):
-            raise NablaB200Error("GemNetOCEngine.launch: call run() on this batch first (it derives the bounds the launch is sized by)")
-        return self.runner.launch(z, pos, mol_ptr, n_mol, self._batch[1], self._batch[2])
-
-    @property
-    def bounds(self) -> Dict[str, int]:
-        return {k: int(self._batch[2][i]) for i, k in enumerate(C_NAMES)} if self._batch else {}
+    label = "GemNetOC"
+    einval_text = "non-finite atom coordinates"
+    count_names = C_NAMES
 
     @staticmethod
-    def raise_on_status(status_host) -> None:
-        """`status_host`: the status words of a launch on the host (the first four suffice)."""
-        n_edges, err, max_deg, n_iso = (int(v) for v in status_host[:4])
-        if err == -4:
-            raise NablaB200Error(f"NB200_ECAPACITY: an edge count exceeds its bound ({n_edges} main-graph edges); `mol_ptr` changed under the engine?")
-        if err == -1:
-            raise NablaB200Error("GemNetOC: non-finite atom coordinates")
-        if err != 0:
-            from ._lib import ERRORS
+    def check_sizes(model: GemNetOC, max_atoms: int) -> None:
+        """Refuse a molecule of more than `max_neighbors_aint` + 1 atoms."""
+        if max_atoms - 1 > model.max_neighbors_aint:
+            raise NablaB200Error(f"GemNetOC: a molecule has {max_atoms} atoms, more than max_neighbors_aint + 1 = {model.max_neighbors_aint + 1}; "
+                                 "the atom-atom graph of the compiled path keeps every in-cutoff pair")
 
-            raise NablaB200Error(f"GemNetOC graph construction failed: {ERRORS.get(err, err)} (max degree {max_deg}, {n_iso} atoms without neighbours)")
+    @staticmethod
+    def size_args(max_atoms: int) -> tuple:
+        return (max_atoms,)
 
 
 class GemNetOCFn(torch.autograd.Function):

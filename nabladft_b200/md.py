@@ -63,7 +63,8 @@ class BatchwiseMD:
         dev = calculator.device
         if dev.type != "cuda":
             raise NablaB200Error("BatchwiseMD runs on CUDA only (no CPU fallback)")
-        if type(getattr(calculator, "model", None)).__name__ == "GemNetOC":
+        model = getattr(calculator, "model", None)
+        if getattr(model, "regress_forces", False) and getattr(model, "direct_forces", False):
             raise NotImplementedError("BatchwiseMD does not run GemNet-OC: its direct forces are not the gradient of its energy, so the dynamics "
                                       "would not conserve energy; use it for relaxation (ASEBatchwiseLBFGS)")
         if int(check_every) < 1:

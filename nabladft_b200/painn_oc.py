@@ -17,7 +17,7 @@ import torch
 from torch import nn
 
 from ._lib import RADIAL_OC, NablaB200Error
-from .engine import PainnEngine, mol_ptr_from_batch
+from .engine import PainnEngine, mol_ptr_from_batch, refuse_training
 
 
 class _GaussianSmearing(nn.Module):
@@ -153,9 +153,8 @@ class PaiNN(nn.Module):
         return self._engine
 
     # -------------------------------------------------------------- forward
-    def forward(self, data):
-        """`data` exposes .z [N], .pos [N,3], .batch [N] (sorted) and optionally .ptr / .num_graphs,
-        as a PyG Batch does (painn.py:90-104). Returns (energy [B], forces [N,3]) or energy."""
+    def _batch_args(self, data):
+        """`data` -> (z int32, pos fp32, mol_ptr int32, n_mol) of the engine calls; the molecule pointer is `data.ptr` if present."""
         pos, z = data.pos, data.z
         if not pos.is_cuda:
             raise NablaB200Error("nabladft_b200.PaiNN runs on CUDA only (no CPU fallback)")
@@ -164,6 +163,19 @@ class PaiNN(nn.Module):
             mol_ptr, n_mol = ptr_attr.to(torch.int32), ptr_attr.numel() - 1
         else:
             mol_ptr, n_mol = mol_ptr_from_batch(data.batch, getattr(data, "num_graphs", None))
+        return z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr.contiguous(), n_mol
+
+    def engine_inputs(self, data):
+        """(engine, z int32, pos fp32, mol_ptr int32, n_mol) of `data` for the inference engine: the inputs of `PainnEngine.run_hvp`
+        (`vibrations`)."""
+        z, pos, mol_ptr, n_mol = self._batch_args(data)
+        refuse_training(self)
+        return self.engine(), z, pos, mol_ptr, n_mol
+
+    def forward(self, data):
+        """`data` exposes .z [N], .pos [N,3], .batch [N] (sorted) and optionally .ptr / .num_graphs,
+        as a PyG Batch does (painn.py:90-104). Returns (energy [B], forces [N,3]) or energy."""
+        z, pos, mol_ptr, n_mol = self._batch_args(data)
         if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             # energy and force losses train through the engine (training.py: analytic gradients, tangent pass for the force term)
             from .training import energy_forces_training
@@ -175,12 +187,9 @@ class PaiNN(nn.Module):
             if self._train_engine.edge_storage != self.train_edge_storage:
                 self._train_engine.set_edge_storage(self.train_edge_storage)
             tensors, scalars = self._export_impl(detach=False)
-            return energy_forces_training(self._train_engine, tensors, scalars, z.to(torch.int32).contiguous(),
-                                          pos.detach().to(torch.float32).contiguous(), mol_ptr.contiguous(), n_mol)
+            return energy_forces_training(self._train_engine, tensors, scalars, z, pos, mol_ptr, n_mol)
         # inference: enqueue and return (no host synchronisation; the status check is deferred to the next call / `check()`)
-        energy, forces = self.engine().run_async(
-            z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr.contiguous(), n_mol,
-            with_forces=self.regress_forces)
+        energy, forces = self.engine().run_async(z, pos, mol_ptr, n_mol, with_forces=self.regress_forces)
         return (energy, forces) if self.regress_forces else energy
 
     def check(self) -> None:

@@ -26,7 +26,7 @@ import torch
 from torch import nn
 
 from ._lib import RADIAL_SPK, NablaB200Error
-from .engine import PainnEngine, mol_ptr_from_batch
+from .engine import PainnEngine, mol_ptr_from_batch, refuse_training
 
 INT32_MAX = 2**31 - 1
 
@@ -306,6 +306,13 @@ class NeuralNetworkPotential(nn.Module):
         # nablaDFT's test/predict steps call self(batch) => post-processing on (ase_model/task.py:43,63)
         post = self.do_postprocessing and not self.training
         return self.engine(post), z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr, n_mol
+
+    def engine_inputs(self, inputs: Dict[str, torch.Tensor]):
+        """(engine, z int32, pos fp32, mol_ptr int32, n_mol) of `inputs` for the inference engine: the inputs of `PainnEngine.run_hvp`
+        (`vibrations`)."""
+        eng, z, pos, mol_ptr, n_mol = self._prepare(inputs)  # raises on CPU inputs and periodic systems
+        refuse_training(self)
+        return eng, z, pos, mol_ptr, n_mol
 
     def _pack(self, energy, forces):
         out = {self._atomwise.output_key: energy}

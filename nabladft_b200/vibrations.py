@@ -23,8 +23,6 @@ from typing import Callable, Dict, List, Optional, Sequence
 
 import torch
 
-from ._lib import NablaB200Error
-from .engine import mol_ptr_from_batch
 
 # Standard atomic weights in u: IUPAC conventional values as used by ASE 3.22 (`ase.data.atomic_masses`), for the elements of nablaDFT.
 ATOMIC_MASSES: Dict[int, float] = {1: 1.008, 6: 12.011, 7: 14.007, 8: 15.999, 9: 18.998403163, 16: 32.06, 17: 35.45, 35: 79.904}
@@ -45,47 +43,12 @@ MEV_PER_CM1 = 1e3 * PLANCK_JS * C_CM_PER_S / EV_J  # h c in meV cm
 
 # ---------------------------------------------------------------------------------------------------------------- model plumbing
 def _engine_inputs(model, batch):
-    """(engine, z int32, pos fp32, mol_ptr int32, n_mol) for each mirror, with the errors the mirrors raise."""
-    from . import dimenetplusplus, gemnet_oc, painn_oc, spk
-
-    if isinstance(model, spk.NeuralNetworkPotential):
-        eng, z, pos, mol_ptr, n_mol = model._prepare(batch)  # raises on CPU inputs and periodic systems
-        if model._training_mode():
-            raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
-        return eng, z, pos, mol_ptr.contiguous(), n_mol
-    if isinstance(model, painn_oc.PaiNN):
-        pos, z = batch.pos, batch.z
-        if not pos.is_cuda:
-            raise NablaB200Error("nabladft_b200.PaiNN runs on CUDA only (no CPU fallback)")
-        if model.training and torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters()):
-            raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
-        ptr_attr = getattr(batch, "ptr", None)
-        if ptr_attr is not None:
-            mol_ptr, n_mol = ptr_attr.to(torch.int32), ptr_attr.numel() - 1
-        else:
-            mol_ptr, n_mol = mol_ptr_from_batch(batch.batch, getattr(batch, "num_graphs", None))
-        return model.engine(), z.to(torch.int32).contiguous(), pos.detach().to(torch.float32).contiguous(), mol_ptr.contiguous(), n_mol
-    if isinstance(model, dimenetplusplus.DimeNetPlusPlusPotential):
-        if not batch.pos.is_cuda:
-            raise NablaB200Error("DimeNetPlusPlusPotential runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
-        if model.training and torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters()):
-            raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
-        runner = model._get_runner()
-        model._sync_weights(runner, batch.pos.device)
-        z, pos, mol_ptr, n_mol = model.batch_args(batch.z, batch.pos, batch.batch)
-        return runner, z, pos, mol_ptr, n_mol
-    if isinstance(model, gemnet_oc.GemNetOC):
-        if not batch.pos.is_cuda:
-            raise NablaB200Error("GemNetOC runs on CUDA tensors only (sm_90a engine; there is no CPU path)")
-        if model.training and torch.is_grad_enabled() and any(p.requires_grad for p in model.parameters()):
-            raise NotImplementedError("Hessians run through the inference engine; call .eval() or torch.no_grad()")
-        runner = model._get_runner()
-        model._sync_weights(runner, batch.pos.device)
-        z, pos, mol_ptr, n_mol, _ = model._batch_args(batch)  # raises for a molecule beyond max_neighbors_aint + 1 atoms
-        return runner, z, pos, mol_ptr, n_mol
-    raise NotImplementedError("Hessians need nabladft_b200.spk.NeuralNetworkPotential, nabladft_b200.painn_oc.PaiNN, "
-                              "nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential or nabladft_b200.gemnet_oc.GemNetOC, "
-                              f"not {type(model).__name__}")
+    """(engine, z int32, pos fp32, mol_ptr int32, n_mol) of `model.engine_inputs(batch)`, with the errors the model raises."""
+    if not hasattr(model, "engine_inputs"):
+        raise NotImplementedError("Hessians need nabladft_b200.spk.NeuralNetworkPotential, nabladft_b200.painn_oc.PaiNN, "
+                                  "nabladft_b200.dimenetplusplus.DimeNetPlusPlusPotential or nabladft_b200.gemnet_oc.GemNetOC, "
+                                  f"not {type(model).__name__}")
+    return model.engine_inputs(batch)
 
 
 def hessian_vector_product(model, batch, v: torch.Tensor):

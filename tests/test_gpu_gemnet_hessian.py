@@ -53,7 +53,7 @@ def _raw_jacobians(net, data, max_dir=64):
     """Per-molecule J = -(dF/dR), [3n, 3n] float64 on the host, NOT symmetrised: column 3k + c from the shared direction 3k + c."""
     from nabladft_b200 import vibrations as vib
 
-    runner, z, pos, mol_ptr, n_mol = vib._engine_inputs(net, data)
+    runner, z, pos, mol_ptr, n_mol = net.engine_inputs(data)
     ptr = mol_ptr.cpu().tolist()
     sizes = [b - a for a, b in zip(ptr[:-1], ptr[1:])]
     n_dir = 3 * max(sizes)
@@ -124,7 +124,7 @@ def test_gpu_energy_and_forces_match_training_and_inference_forwards(net):
 
     data = _data(*_fixture([26, 3, 99]))
     e, f, _ = vib.hessian_vector_product(net, data, _dirs(1, data.z.numel(), 5)[0].float().cuda())
-    runner, z, pos, mol_ptr, n_mol = vib._engine_inputs(net, data)
+    runner, z, pos, mol_ptr, n_mol = net.engine_inputs(data)
     e_tr, f_tr, _ = runner.run_train(z, pos, mol_ptr, n_mol, int((mol_ptr[1:] - mol_ptr[:-1]).max()))
     assert torch.equal(e, e_tr) and torch.equal(f, f_tr)
     with torch.no_grad():

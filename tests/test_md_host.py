@@ -141,3 +141,22 @@ def test_units_and_mdlogger_format():
     assert md.mdlogger_header() == "Time[ps]      Etot[eV]     Epot[eV]     Ekin[eV]    T[K]"
     assert md.mdlogger_line(0.0005, -1.5, 0.25, 300.04, 29) == "0.0005          -1.2500      -1.5000       0.2500   300.0"
     assert md.mdlogger_line(1.0, -1234.5, 2.0, 15.0, 150) == "1.0000        -1232.500    -1234.500        2.000    15.0"
+
+
+def test_md_refuses_gemnet_oc_whose_forces_are_not_the_gradient_of_its_energy():
+    """The refusal comes before the library is loaded, so a stand-in calculator on a CUDA device runs it without a GPU."""
+    import torch
+    import yaml
+
+    from nabladft_b200.gemnet_oc import GemNetOC
+    from nabladft_b200.md import BatchwiseMD
+
+    cfg = yaml.safe_load(open(os.path.join(ROOT, "config", "model", "gemnet-oc-b200.yaml")))["net"]
+    cfg.pop("_target_")
+
+    class Calculator:
+        device = torch.device("cuda")
+        model = GemNetOC(**cfg)
+
+    with pytest.raises(NotImplementedError, match="GemNet-OC"):
+        BatchwiseMD(Calculator(), [])
