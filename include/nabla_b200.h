@@ -326,6 +326,47 @@ typedef struct nb200_painn_tan_args {
     float *g_w, *g_b;
 } nb200_painn_tan_args;
 int nb200_painn_test_tangent(const nb200_painn_tan_args* args, void* stream);
+/* Test entry point, not a supported API: ONE program of the fused PaiNN node kernels (painn_fused.cu), their weight preparation, or one
+ * primal per-atom kernel of painn_node.cu, on caller-built inputs, through the host wrapper the engine calls (hence its launch
+ * configuration).  F = 128; per-atom arrays [n_atoms, k F] as in the engine; weights, eps and biases from `w` (n_feat = F).  `op`:
+ *   PREP              w -> wtiles [nb_fused_wtile_bytes(n_layers) bytes: (22 n_layers + 2) tiles of 128 KB]
+ *   NODE_FWD          prep into wtiles, then the forward program (layer_upd, layer_mlp, readout):
+ *                       (-1, l, 0)   q_mlp_in -> h1pre xh                        (message MLP of layer l on the embedding)
+ *                       (l, l+1, 0)  q_mid mu_mid -> VW nrm dot g1pre y q_next mu_next h1pre xh
+ *                       (l, -1, 1)   q_mid mu_mid -> VW nrm dot g1pre y q_next mu_next ro_pre (without e1)
+ *   NODE_BWD          prep into wtiles, then the backward program:
+ *                       readout = 1, layer_mlp = -1, layer_upd = l:  ro_pre (with e1) y VW nrm dot g1pre, cur (in / out) -> gq_b gdot gn gq_a
+ *                       readout = 0, layer_mlp = l+1, layer_upd = l: g_xh h1pre y VW nrm dot g1pre, gq_a cur (in / out) -> gq_b gdot gn
+ *                     tile: 0 (the engine's rule), 64 or 80 atoms per CTA in; the width that ran out.
+ *   EMBED             z -> q mu, status[1] = NB200_EINVAL for an element outside [z_offset, z_offset + n_elem)
+ *   ACT_BWD           g (in / out) pre n kind (NB_ACT_SILU 0 or NB_ACT_SSP 1)      (n % 4 == 0)
+ *   UPD_COMBINE_BWD   gq gmu y VW -> gy gVW
+ *   UPD_NORM_BWD      gn VW nrm -> gVW (accumulated)
+ *   READOUT           pre [n_atoms, F/2] (in / out: += e1) -> eps_atom
+ *   MOL_SUM           eps_atom mol_ptr n_mol -> energy
+ *   READOUT_BWD       pre -> g_pre [n_atoms, F/2]
+ *   POISON            status energy n_mol, forces (may be NULL) n -> NaN where status[1] != 0
+ * NB200_EINVAL (nothing launched) for an unknown op or program, a layer index outside [0, n_layers), tile not in {0, 64, 80}, n_atoms < 0,
+ * n < 0, n_mol < 0, a NULL field the op uses, or a pointer the float4 paths read or write that is not 16-byte aligned. */
+enum {
+    NB200_PN_PREP = 0, NB200_PN_NODE_FWD, NB200_PN_NODE_BWD, NB200_PN_EMBED, NB200_PN_ACT_BWD, NB200_PN_UPD_COMBINE_BWD, NB200_PN_UPD_NORM_BWD,
+    NB200_PN_READOUT, NB200_PN_MOL_SUM, NB200_PN_READOUT_BWD, NB200_PN_POISON, NB200_PN_N_OPS
+};
+typedef struct nb200_painn_node_args {
+    int32_t op, n_atoms, tile, layer_upd, layer_mlp, readout;
+    const nb200_painn_weights* w;
+    void* wtiles;
+    const float *q_mid, *mu_mid, *q_mlp_in, *g_xh;
+    float *VW, *nrm, *dot, *g1pre, *y, *q_next, *mu_next, *h1pre, *xh, *ro_pre;
+    float *gq_a, *gq_b, *cur, *gn, *gdot;
+    const int32_t *z, *mol_ptr;
+    int32_t* status;
+    int32_t n_mol, kind;
+    int64_t n;
+    const float *gq, *gmu;
+    float *q, *mu, *g, *pre, *gy, *gVW, *eps_atom, *energy, *forces, *g_pre;
+} nb200_painn_node_args;
+int nb200_painn_test_node(nb200_painn_node_args* args, void* stream);
 
 /* ----------------------------------------------------------------------------------------
  * SchNet energy + forces (config/model/schnet.yaml: schnetpack.representation.SchNet inside

@@ -97,6 +97,20 @@ PT_OPS = ("GEOM_TAN", "MUL_DACT", "ACT_BWD_TAN", "READOUT_BWD_TAN", "MSG_FWD_TAN
           "UPD_NORM_BWD_TAN", "MSG_BWD_TAN", "MSG_BWD_HVP", "EDGE_FORCES_HVP", "FILTER_D2", "FILTER_WGRAD")
 
 
+class PainnNodeArgs(ctypes.Structure):
+    """Mirror of `struct nb200_painn_node_args` (include/nabla_b200.h)."""
+
+    _fields_ = [(name, c_int32) for name in ("op", "n_atoms", "tile", "layer_upd", "layer_mlp", "readout")] + [
+        ("w", POINTER(PainnWeights))] + [(name, c_void_p) for name in (
+            "wtiles", "q_mid", "mu_mid", "q_mlp_in", "g_xh", "VW", "nrm", "dot", "g1pre", "y", "q_next", "mu_next", "h1pre", "xh", "ro_pre",
+            "gq_a", "gq_b", "cur", "gn", "gdot", "z", "mol_ptr", "status")] + [("n_mol", c_int32), ("kind", c_int32), ("n", c_int64)] + [
+        (name, c_void_p) for name in ("gq", "gmu", "q", "mu", "g", "pre", "gy", "gVW", "eps_atom", "energy", "forces", "g_pre")]
+
+
+# nb200_painn_test_node ops (enum NB200_PN_*)
+PN_OPS = ("PREP", "NODE_FWD", "NODE_BWD", "EMBED", "ACT_BWD", "UPD_COMBINE_BWD", "UPD_NORM_BWD", "READOUT", "MOL_SUM", "READOUT_BWD", "POISON")
+
+
 class DimeNetWeights(ctypes.Structure):
     """Mirror of `struct nb200_dimenet_weights` (include/nabla_b200.h)."""
 
@@ -186,6 +200,7 @@ SIGNATURES = {
     "nb200_painn_hvp": (c_int32, [c_void_p, POINTER(PainnWeights), c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,
                                   c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_painn_test_tangent": (c_int32, [POINTER(PainnTanArgs), c_void_p]),
+    "nb200_painn_test_node": (c_int32, [POINTER(PainnNodeArgs), c_void_p]),
 
     "nb200_gemnet_oc_graph_bytes": (c_int64, [c_int32, c_int32]),
     "nb200_gemnet_oc_graph_count": (c_int32, [POINTER(GemNetOCWeights), c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,

@@ -528,6 +528,13 @@ bool wide_tiles(int n_atoms) {
     return waves80 < waves64;
 }
 
+// the tile width of a launch: *tile = 64 or 80 forces it, 0 (or tile == nullptr) takes wide_tiles; *tile is set to the width that runs
+int pick_width(int n_atoms, int* tile) {
+    const int nt = tile && *tile ? *tile : wide_tiles(n_atoms) ? Node80::NT : Node64::NT;
+    if (tile) *tile = nt;
+    return nt;
+}
+
 // launch of a fused node kernel instantiated for layout L (its shared-memory limit is raised once per kernel and device)
 template <class L, class Params>
 int launch_tiles(void (*kernel)(Params), const Params& P, int n_atoms, cudaStream_t s) {
@@ -553,7 +560,7 @@ int nb_fused_prep(const nb200_painn_weights* w, void* wtiles, cudaStream_t s) {
     return nb_check_launch();
 }
 
-int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s) {
+int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s, int* tile) {
     FwdParams P{};
     // One worker group, whole-operand hand-over: the K-halves hand-over of tc_pipe.cuh's two-group layout gains nothing here, because most
     // operands of these kernels are written by the previous GEMM's epilogue, which cannot start earlier.
@@ -564,10 +571,11 @@ int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s) {
     P.q_next = a.q_next; P.mu_next = a.mu_next; P.eps = a.eps; P.q_mlp_in = a.q_mlp_in; P.c1 = a.c1; P.h1pre = a.h1pre; P.xh = a.xh;
     P.ro_pre = a.ro_pre;
     if (a.n_atoms <= 0) return NB200_OK;
-    return wide_tiles(a.n_atoms) ? launch_tiles<Node80>(k_node_fwd<Node80>, P, a.n_atoms, s) : launch_tiles<Node64>(k_node_fwd<Node64>, P, a.n_atoms, s);
+    return pick_width(a.n_atoms, tile) == Node80::NT ? launch_tiles<Node80>(k_node_fwd<Node80>, P, a.n_atoms, s)
+                                                     : launch_tiles<Node64>(k_node_fwd<Node64>, P, a.n_atoms, s);
 }
 
-int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s) {
+int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s, int* tile) {
     BwdParams P{};
     P.n_atoms = a.n_atoms; P.do_mlp = a.layer_mlp >= 0; P.do_ro = a.readout; P.do_upd = a.layer_upd >= 0;
     P.wt = static_cast<const unsigned char*>(a.wtiles);
@@ -575,5 +583,6 @@ int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s) {
     P.gq_a = a.gq_a; P.gq_b = a.gq_b; P.cur = a.cur; P.gn = a.gn; P.gdot = a.gdot; P.dot = a.dot; P.g_xh = a.g_xh; P.h1pre = a.h1pre; P.ro_pre = a.ro_pre; P.R2 = a.R2;
     P.y = a.y; P.VW = a.VW; P.nrm = a.nrm; P.g1pre = a.g1pre;
     if (a.n_atoms <= 0) return NB200_OK;
-    return wide_tiles(a.n_atoms) ? launch_tiles<Node80>(k_node_bwd<Node80>, P, a.n_atoms, s) : launch_tiles<Node64>(k_node_bwd<Node64>, P, a.n_atoms, s);
+    return pick_width(a.n_atoms, tile) == Node80::NT ? launch_tiles<Node80>(k_node_bwd<Node80>, P, a.n_atoms, s)
+                                                     : launch_tiles<Node64>(k_node_bwd<Node64>, P, a.n_atoms, s);
 }

@@ -82,5 +82,6 @@ struct NbFusedBwd {
 };
 int64_t nb_fused_wtile_bytes(int n_layers);
 int nb_fused_prep(const nb200_painn_weights* w, void* wtiles, cudaStream_t s);
-int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s);
-int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s);
+// tile (optional, in / out): 64 or 80 atoms per CTA forces that width, 0 takes the rule of wide_tiles (painn_fused.cu); set to the width used
+int nb_fused_node_fwd(const NbFusedFwd& a, cudaStream_t s, int* tile = nullptr);
+int nb_fused_node_bwd(const NbFusedBwd& a, cudaStream_t s, int* tile = nullptr);
