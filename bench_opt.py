@@ -10,7 +10,11 @@ process: the device loop (asynchronous forward sized by per-batch upper bounds, 
 the synchronous two-phase forward (`GemNetOCRunner.run`, which waits for the edge counts) at every step.  It also reports the host
 synchronisations of a run, real count / bound of the five edge counts, the workspace size, and the card's name and power limit.
 `--model dimenetplusplus` does the same for DimeNet++ (config/model/dimenetplusplus.yaml, seeded test weights), and also times one
-asynchronous against one two-phase forward at the start geometry with CUDA events."""
+asynchronous against one two-phase forward at the start geometry with CUDA events.
+
+`--optimizer quasinewton` relaxes with `BatchwiseQuasiNewton` instead (PaiNN at `--batch`, or `--model dimenetplusplus` at batch 32): optimiser
+steps/s, engine launches per optimiser step, `nb200_qn_step` against engine time per launch from CUDA events, host synchronisations, and a
+host-driven arm (the oracle's numpy state machine on the same engine, one synchronisation per evaluation)."""
 import argparse
 from ctypes import c_int64
 import json
@@ -242,6 +246,98 @@ def dimenet_main(args):
     print(json.dumps(out))
 
 
+def qn_main(args):
+    """`--optimizer quasinewton`: BatchwiseQuasiNewton (ASE's QuasiNewton per molecule) with PaiNN at batch `--batch` or DimeNet++ at batch 32."""
+    import numpy as np
+    import torch
+
+    from nabladft_b200.optimization import BatchwiseQuasiNewton, PyGBatchwiseCalculator, SimpleAtoms, SpkBatchwiseCalculator, convert_units
+    from nabladft_b200.synth import synth_batch
+    from oracle.quasinewton import BatchQuasiNewton
+
+    dev = torch.device("cuda:0")
+    if args.model == "dimenetplusplus":
+        batch, calc = 32, PyGBatchwiseCalculator(dimenet_model(dev), device=dev, energy_unit="Hartree", position_unit="Ang")
+    else:
+        from bench import build_model
+
+        batch, calc = args.batch, SpkBatchwiseCalculator(build_model("painn", dev), device=dev, energy_unit="Hartree", position_unit="Ang")
+    name, power = card_and_power()
+    b = synth_batch(1, batch)
+    ptr = b["mol_ptr"]
+    atoms = [SimpleAtoms(b["pos"][ptr[m]:ptr[m + 1]], b["z"][ptr[m]:ptr[m + 1]]) for m in range(batch)]
+    opt = BatchwiseQuasiNewton(calc, check_every=args.check_every)
+    opt.run(atoms, fmax=1e-9, steps=3)  # warm-up
+    torch.cuda.synchronize()
+    opt.initialize()
+    t0 = time.perf_counter()
+    opt.run(atoms, fmax=1e-9, steps=args.steps)  # fmax unreachable: every molecule takes `steps` BFGS steps
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    mol_steps = int(opt.nsteps.sum())
+    out = {"metric": f"QuasiNewton steps/sec ({args.model} E+F + batched BFGSLineSearch, B molecules)", "card": name, "power_limit": power,
+           "model": args.model, "batch": batch, "atoms": int(ptr[-1]), "steps": args.steps, "check_every": args.check_every,
+           "value": float(opt.nsteps.mean()) / dt, "molecule_steps_per_s": mol_steps / dt, "ms_per_launch": dt / opt.launches * 1e3,
+           "engine_launches": opt.launches, "engine_launches_used": opt.launches_used,
+           "launches_per_optimiser_step": opt.launches_used / float(opt.nsteps.max()),
+           "force_calls_per_step_mean": float(opt.force_calls.sum()) / mol_steps, "host_syncs": opt.host_syncs,
+           "hessian_bytes": int(((3 * np.diff(ptr)) ** 2).sum() * 8),
+           "timing": "host wall clock around BatchwiseQuasiNewton.run ending in a device synchronise (includes packing, H2D, final D2H)"}
+
+    # per-launch device time of nb200_qn_step against the engine launch: CUDA events around each call, in a separate run
+    eng = calc.engine()
+    lib, times = opt.lib, {"qn": [], "engine": []}
+
+    class Timed:
+        def __init__(self, fn, key):
+            self.fn, self.key = fn, key
+
+        def __call__(self, *a, **k):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            r = self.fn(*a, **k)
+            e1.record()
+            times[self.key].append((e0, e1))
+            return r
+
+    class TimedLib:
+        def __getattr__(self, n):
+            return Timed(getattr(lib, n), "qn") if n == "nb200_qn_step" else getattr(lib, n)
+
+    launch = eng.launch
+    eng.launch = Timed(launch, "engine")
+    opt.lib = TimedLib()
+    try:
+        opt.initialize()
+        opt.run(atoms, fmax=1e-9, steps=min(args.steps, 10))
+        torch.cuda.synchronize()
+    finally:
+        eng.launch, opt.lib = launch, lib
+    ms = {k: float(np.mean([a.elapsed_time(c) for a, c in v])) for k, v in times.items()}
+    out["qn_step_ms_per_launch"] = round(ms["qn"], 4)
+    out["engine_ms_per_launch"] = round(ms["engine"], 4)
+    out["qn_step_share_of_engine"] = round(ms["qn"] / ms["engine"], 4)
+
+    # host-driven arm: the oracle's numpy state machine stepping the same engine, one synchronisation per evaluation (the reference's cost
+    # model, batched)
+    z, pos, mol_ptr, sizes = calc.pack(atoms)
+    e_scale = calc.energy_conversion * convert_units("Hartree", "eV")
+    f_scale = np.float32(e_scale / calc.position_conversion)
+
+    def ff(p):
+        e, f, _ = eng.launch(z, torch.from_numpy(np.asarray(p, dtype=np.float32)).to(dev), mol_ptr, batch, e_cap=eng.e_cap)
+        return e.cpu().numpy().astype(np.float64) * e_scale, f.cpu().numpy() * f_scale
+
+    host = BatchQuasiNewton(ff, sizes)
+    t0 = time.perf_counter()
+    host.run(pos.cpu().numpy(), fmax=1e-9, steps=args.host_steps)
+    dth = time.perf_counter() - t0
+    out["host_driven"] = {"steps": args.host_steps, "value": float(host.nsteps.mean()) / dth, "molecule_steps_per_s": float(host.nsteps.sum()) / dth,
+                          "ms_per_launch": dth / host.n_calls * 1e3, "host_syncs": host.n_calls,
+                          "kind": "oracle/quasinewton.py numpy state machine + the same engine, a device synchronisation per evaluation"}
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", choices=["painn", "gemnet-oc", "dimenetplusplus"], default="painn")
@@ -254,7 +350,13 @@ def main():
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--cpu-mols", type=int, default=8)
     ap.add_argument("--cpu-steps", type=int, default=3)
+    ap.add_argument("--optimizer", choices=["lbfgs", "quasinewton"], default="lbfgs")
+    ap.add_argument("--host-steps", type=int, default=5, help="quasinewton: BFGS steps of the host-driven arm")
     args = ap.parse_args()
+    if args.optimizer == "quasinewton":
+        if args.model == "gemnet-oc":
+            raise SystemExit("--optimizer quasinewton: --model painn or dimenetplusplus")
+        return qn_main(args)
     if args.model == "gemnet-oc":
         return gemnet_main(args)
     if args.model == "dimenetplusplus":

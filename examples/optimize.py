@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Batched L-BFGS relaxation of every molecule of a packed dataset (reference: job_type optimize, config/schnet_optim.yaml and
 config/gemnet-oc_optim.yaml, config/dimenetplusplus_optim-b200.yaml): `--model painn` (default), `--model gemnet-oc` or
-`--model dimenetplusplus` (without --weights: the seeded test weights of tests/golden/make_golden_dimenet.py)."""
+`--model dimenetplusplus` (without --weights: the seeded test weights of tests/golden/make_golden_dimenet.py).
+`--optimizer quasinewton` relaxes with ASE's QuasiNewton per molecule instead (PYGAseInterface.optimize, BatchwiseQuasiNewton)."""
 import argparse
 import os
 import sys
@@ -13,7 +14,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 from nabladft_b200.data import PackedEnergyDataset  # noqa: E402
-from nabladft_b200.optimization import ASEBatchwiseLBFGS, PackedOptimizeTask, PyGBatchwiseCalculator, SpkBatchwiseCalculator  # noqa: E402
+from nabladft_b200.optimization import (ASEBatchwiseLBFGS, BatchwiseQuasiNewton, PackedOptimizeTask, PyGBatchwiseCalculator,  # noqa: E402
+                                        SpkBatchwiseCalculator)
 from train_painn import build_model  # noqa: E402
 
 
@@ -25,6 +27,7 @@ def main():
     ap.add_argument("--batch", type=int, default=32)   # config/schnet_optim.yaml: batch_size 32, fmax 1e-5, steps 500
     ap.add_argument("--fmax", type=float, default=1e-5)
     ap.add_argument("--steps", type=int, default=500)
+    ap.add_argument("--optimizer", choices=["lbfgs", "quasinewton"], default="lbfgs")
     a = ap.parse_args()
     if a.model == "gemnet-oc":
         import yaml
@@ -51,7 +54,10 @@ def main():
         model.load_state_dict(torch.load(a.weights, map_location="cpu"), strict=True)
     calculator = SpkBatchwiseCalculator if a.model == "painn" else PyGBatchwiseCalculator
     calc = calculator(model, device="cuda:0", energy_unit="Hartree", position_unit="Ang")
-    opt = ASEBatchwiseLBFGS(calc, logfile="-", check_every=10)
+    if a.optimizer == "quasinewton":
+        opt = BatchwiseQuasiNewton(calc, logfile="-", check_every=10)  # pyg_opt.py: optimize(fmax=1e-4, steps=100)
+    else:
+        opt = ASEBatchwiseLBFGS(calc, logfile="-", check_every=10)
     out = PackedOptimizeTask(PackedEnergyDataset.load(a.cache), opt, a.batch, a.fmax, a.steps).run()
     np.savez_compressed("relaxed.npz", **out)
     print("batches", len(out["nsteps"]), "steps per batch", out["nsteps"].tolist()[:8], "-> relaxed.npz")

@@ -500,6 +500,36 @@ int nb200_lbfgs_step(void* state, int64_t state_bytes, const int32_t* mol_ptr, i
                      float* pos32_out, int32_t* unconverged_out, int32_t* n_normalizations, void* stream);
 
 /* ----------------------------------------------------------------------------------------
+ * Batch-wise QuasiNewton geometry optimisation: ASE's BFGSLineSearch + LineSearch (the optimiser of
+ * PYGAseInterface.optimize, nablaDFT/optimization/pyg_ase_interface.py:296-315) for every molecule of a batch
+ * independently (csrc/quasinewton.cu, oracle/quasinewton.py).  Call once after each energy + forces evaluation:
+ * every molecule consumes E and F at its current trial point and either writes its next trial point to pos /
+ * pos32 or stops; a stopped molecule is never touched again.  One CTA per molecule.
+ *   state        device buffer of nb200_qn_state_bytes() bytes, zero-filled before the first call: line-search
+ *                scalars, the dense inverse Hessians (3n_i x 3n_i float64 at hess_off[i], hess_elems doubles in
+ *                all), the start point, direction and scaled gradient of the current step
+ *   hess_off     int64 [n_mol], element offset of molecule i's inverse Hessian
+ *   fmax         stop a molecule when max |F| < fmax (tested in float32); max_steps caps its BFGS steps
+ *   maxstep, c1, c2, alpha, stpmax   BFGSLineSearch arguments (ASE units: eV, A)
+ *   e_scale, f_scale   energy [n_mol] / forces [n_atoms,3] float32 of the model times these = eV, eV/A
+ *   fixed_mask   optional uint8 [n_atoms]: 1 = FixAtoms (force zeroed, position never changes)
+ *   pos          double [n_atoms,3], in/out;  pos32 = (float)pos, out (unchanged for stopped molecules)
+ *   max_atoms_per_mol   at least the largest mol_ptr[i+1] - mol_ptr[i]: it sizes the kernel's shared memory; a larger
+ *                molecule is refused (status 4) without being touched
+ *   mol_info     int32 [n_mol][4], zero-filled before the first call: status (0 running, 1 converged, 2 max_steps,
+ *                3 line search failed, 4 molecule larger than max_atoms_per_mol or hess_off outside hess_elems), nsteps,
+ *                force_calls, function_calls
+ *   running_out  int32: molecules still running after this call
+ * NB200_EINVAL (nothing launched) for a null required pointer, a negative size, alpha or maxstep <= 0, or a short
+ * state.  Asynchronous on `stream`; no host synchronisation. */
+int64_t nb200_qn_state_bytes(int32_t n_mol, int32_t n_atoms, int64_t hess_elems);
+int nb200_qn_step(void* state, int64_t state_bytes, const int32_t* mol_ptr, const int64_t* hess_off, int32_t n_mol,
+                  int32_t n_atoms, int32_t max_atoms_per_mol, int64_t hess_elems, double fmax, int32_t max_steps,
+                  double maxstep, double c1, double c2, double alpha, double stpmax, double e_scale, double f_scale,
+                  const uint8_t* fixed_mask, const float* energy, const float* forces, double* pos, float* pos32,
+                  int32_t* mol_info, int32_t* running_out, void* stream);
+
+/* ----------------------------------------------------------------------------------------
  * Batched molecular dynamics (PYGAseInterface.init_md / run_md of nablaDFT/optimization/pyg_ase_interface.py): ASE 3.22
  * VelocityVerlet and Langevin(fixcm=True) for a whole batch, one CTA per molecule, float64 positions and momenta (csrc/md.cu,
  * oracle/md.py).  ASE units: eV, A, u, ASE time.  Noise: counter-based Philox4x32-10, key = seed, counter = (global atom index,

@@ -178,6 +178,9 @@ SIGNATURES = {
     "nb200_lbfgs_state_bytes": (c_int64, [c_int32, c_int32, c_int32]),
     "nb200_lbfgs_step": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_double, c_double, c_double,
                                    c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_qn_state_bytes": (c_int64, [c_int32, c_int32, c_int64]),
+    "nb200_qn_step": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int64, c_double, c_int32] + [c_double] * 7
+                      + [c_void_p] * 8),
     "nb200_md_init_momenta": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_double, c_uint64, c_int64, c_void_p, c_void_p]),
     "nb200_md_step": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_double, c_double, c_double, c_uint64, c_int64, c_double, c_double]
                       + [c_void_p] * 11),

@@ -17,6 +17,8 @@ FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ] + os.environ.get("NB200_NVCC_EXTRA", "").split()
+# per-source flags: the quasi-Newton line search rounds every float64 operation as Python does, so no FMA contraction there
+SOURCE_FLAGS = {"quasinewton.cu": ["-fmad=false"]}
 
 
 def sources():
@@ -28,7 +30,7 @@ STAMP = os.path.join(HERE, "build", "stamp.txt")
 
 def stamp_text() -> str:
     """What the library was built with: compiler, flags (architecture and NB200_NVCC_EXTRA included)."""
-    return " ".join([NVCC, *FLAGS])
+    return " ".join([NVCC, *FLAGS, repr(sorted(SOURCE_FLAGS.items()))])
 
 
 def stale() -> bool:
@@ -52,7 +54,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     for src in sources():
         obj = os.path.join(HERE, "build", os.path.basename(src)[:-3] + ".o")
-        cmd = [NVCC, *FLAGS, "-c", src, "-o", obj] + (["-Xptxas", "-v"] if verbose else [])
+        cmd = [NVCC, *FLAGS, *SOURCE_FLAGS.get(os.path.basename(src), []), "-c", src, "-o", obj] + (["-Xptxas", "-v"] if verbose else [])
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
         objs.append(obj)
     for src, p in procs:

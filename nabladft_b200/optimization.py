@@ -152,6 +152,15 @@ class SpkBatchwiseCalculator(BatchwiseCalculator):
         return self.model.engine(self.model.do_postprocessing and not self.model.training)
 
 
+def _fold_status(worst: torch.Tensor, status: torch.Tensor) -> None:
+    """Fold an engine launch's status words into `worst` on the device: the engine rewrites them at every launch, so a loop that looks
+    at them once per chunk keeps the worst error code and the largest edge count / degree of the chunk, and an overflow in the middle
+    of a chunk cannot hide behind a later clean launch."""
+    torch.minimum(worst[1:2], status[1:2], out=worst[1:2])   # error codes are negative
+    torch.maximum(worst[0:1], status[0:1], out=worst[0:1])   # edges
+    torch.maximum(worst[2:3], status[2:3], out=worst[2:3])   # max degree
+
+
 class BatchwiseOptimizer:
     """optimizers.py:126-289 (the parts that do not depend on ASE's Dynamics base class)."""
 
@@ -194,6 +203,12 @@ class BatchwiseOptimizer:
 
             for idx, at in enumerate(self.atoms):
                 write(self.trajectory + f"_{idx}.xyz", at, format="extxyz", append=self.nsteps != 0)
+
+    def _sync_atoms(self, pos: torch.Tensor) -> None:
+        """`.atoms` = new Atoms objects at the device positions (float64 [n_atoms, 3]), split by `n_ats_per_config`."""
+        host = pos.cpu().numpy()
+        off = np.concatenate([[0], np.cumsum(self.n_ats_per_config)])
+        self.atoms = [_like(a, host[off[i]:off[i + 1]]) for i, a in enumerate(self.atoms)]
 
     def get_relaxation_results(self):
         self.calculator.get_forces(self.atoms)
@@ -260,8 +275,6 @@ class ASEBatchwiseLBFGS(BatchwiseOptimizer):
         if self.nsteps == 0:
             self._log_device(forces, fixed)
         self.positions_history = [pos.cpu().numpy().copy()]
-        # the engine rewrites its status word at every launch: keep the worst error code and the largest edge count of the chunk on the
-        # device, so that an overflow in the middle of a chunk cannot hide behind a later clean launch
         worst = torch.zeros(4, dtype=torch.int32, device=dev)
         done_at, it = None, 0
         while it < self.max_steps and done_at is None:
@@ -273,9 +286,7 @@ class ASEBatchwiseLBFGS(BatchwiseOptimizer):
                 check(rc, "nb200_lbfgs_step")
                 self.iteration += 1
                 energy, forces, status = eng.launch(z, pos32, mol_ptr, n_mol, e_cap=eng.e_cap)
-                torch.minimum(worst[1:2], status[1:2], out=worst[1:2])   # error codes are negative
-                torch.maximum(worst[0:1], status[0:1], out=worst[0:1])   # edges
-                torch.maximum(worst[2:3], status[2:3], out=worst[2:3])   # max degree
+                _fold_status(worst, status)
                 if f_unit != 1.0:
                     forces = forces * f_unit
             host = unconv[:n_chunk].cpu()  # the only host<->device synchronisation of the loop
@@ -306,16 +317,110 @@ class ASEBatchwiseLBFGS(BatchwiseOptimizer):
         self.log(calc.results[calc.force_key])
         return self.converged(calc.results[calc.force_key])
 
-    def _sync_atoms(self, pos: torch.Tensor) -> None:
-        host = pos.cpu().numpy()
-        off = np.concatenate([[0], np.cumsum(self.n_ats_per_config)])
-        self.atoms = [_like(a, host[off[i]:off[i + 1]]) for i, a in enumerate(self.atoms)]
-
     def _log_device(self, forces: torch.Tensor, fixed) -> None:
         if self.logfile is None and self.trajectory is None:
             return
         f = forces if fixed is None else forces.masked_fill(fixed.bool()[:, None], 0.0)
         self.log(f.cpu().numpy())
+
+
+class BatchwiseQuasiNewton(BatchwiseOptimizer):
+    """`PYGAseInterface.optimize()` (pyg_ase_interface.py:296-315: ASE's QuasiNewton = BFGSLineSearch) for a whole batch on the device.
+    Every molecule follows its own BFGS + More-Thuente line-search trajectory exactly as ASE runs it alone (oracle/quasinewton.py); the
+    batch shares the force calls.  The loop is the engine's E+F launch followed by ONE kernel (`nb200_qn_step`, csrc/quasinewton.cu) on
+    the same stream; the host looks at a device counter of running molecules every `check_every` launches.  Energies and forces enter
+    the optimiser in eV and eV/A, converted from the calculator's declared units as `PYGCalculator` does.
+
+    After `run`: `.atoms`, `calculator.results` (the calculator's units, fixed atoms' forces zeroed), and per molecule `nsteps`,
+    `force_calls`, `function_calls` and `status` (0 running, 1 converged, 2 reached `steps`, 3 line search failed) as numpy arrays;
+    `launches` = engine launches of the run, `launches_used` = those whose evaluation some molecule consumed (the rest are the no-op
+    tail of the last `check_every` chunk), `host_syncs` = times the loop waited for the device.  Every `run` starts these afresh."""
+
+    def __init__(self, calculator: BatchwiseCalculator, logfile: Optional[str] = None, maxstep: Optional[float] = None, c1: float = 0.23,
+                 c2: float = 0.46, alpha: float = 10.0, stpmax: float = 50.0, fixed_atoms_mask: Optional[List[int]] = None, check_every: int = 10):
+        super().__init__(calculator, None, logfile, None, None, False, False, fixed_atoms_mask)
+        self.maxstep = maxstep if maxstep is not None else self.defaults["maxstep"]
+        self.c1, self.c2, self.alpha, self.stpmax = float(c1), float(c2), float(alpha), float(stpmax)
+        self.check_every = max(1, int(check_every))
+        self.lib = _lib.load()
+
+    def initialize(self) -> None:
+        self.nsteps = self.force_calls = self.function_calls = self.status = None
+        self.launches = self.launches_used = self.host_syncs = 0
+
+    def run(self, atoms: Sequence, fmax: float = 0.05, steps: Optional[int] = None) -> bool:
+        if any(len(getattr(a, "constraints", ()) or ()) for a in atoms):
+            raise NotImplementedError("ase.Atoms constraints are not read by the device loop: pass the fixed atoms as fixed_atoms_mask "
+                                      "(global indices into the batch) instead of a FixAtoms constraint")
+        self.initialize()
+        calc, dev = self.calculator, self.calculator.device
+        self.atoms, self.fmax = list(atoms), fmax
+        max_steps = steps if steps else 100000000
+        z, pos, mol_ptr, sizes = calc.pack(self.atoms)
+        self.n_ats_per_config = sizes
+        n_mol, n_atoms, max_at = len(sizes), int(sizes.sum()), int(sizes.max()) if len(sizes) else 0
+        e_scale = calc.energy_conversion * convert_units("Hartree", "eV")
+        f_scale = e_scale / calc.position_conversion
+        h_off = np.concatenate([[0], np.cumsum((3 * sizes) ** 2)]).astype(np.int64)
+        hess_elems = int(h_off[-1])
+        h_off = torch.from_numpy(h_off[:-1].copy()).to(dev)
+        need = self.lib.nb200_qn_state_bytes(n_mol, n_atoms, hess_elems)
+        if need < 0:
+            check(int(need), "nb200_qn_state_bytes")
+        state = torch.zeros(int(need), dtype=torch.uint8, device=dev)
+        info = torch.zeros(n_mol, 4, dtype=torch.int32, device=dev)
+        pos32 = pos.float().contiguous()
+        fixed = None
+        if self.fixed_atoms_mask is not None:
+            fixed = torch.zeros(n_atoms, dtype=torch.uint8, device=dev)
+            fixed[torch.as_tensor(list(self.fixed_atoms_mask), dtype=torch.long, device=dev)] = 1
+        chunk = self.check_every
+        running = torch.full((chunk,), -1, dtype=torch.int32, device=dev)
+
+        eng = calc.engine()
+        energy, forces, st = eng.run(z, pos32, mol_ptr, n_mol)  # first evaluation: synchronous, sizes the edge capacity
+        eng.e_cap = max(eng.e_cap, int(1.5 * int(st[0])) + 1024)  # head-room: the geometry moves without the host looking
+        self.host_syncs += 1
+        self.launches = self.launches_used = 1
+        worst = torch.zeros(4, dtype=torch.int32, device=dev)
+        while True:
+            for k in range(chunk):
+                rc = self.lib.nb200_qn_step(ptr(state), state.numel(), ptr(mol_ptr), ptr(h_off), n_mol, n_atoms, max_at, hess_elems, float(fmax),
+                                            int(max_steps), float(self.maxstep), self.c1, self.c2, self.alpha, self.stpmax, float(e_scale),
+                                            float(f_scale), ptr(fixed), ptr(energy), ptr(forces), ptr(pos), ptr(pos32), ptr(info),
+                                            running[k:].data_ptr(), current_stream())
+                check(rc, "nb200_qn_step")
+                energy, forces, status = eng.launch(z, pos32, mol_ptr, n_mol, e_cap=eng.e_cap)
+                _fold_status(worst, status)
+                self.launches += 1
+            host, mol = running.cpu(), info.cpu().numpy()  # the only host<->device synchronisation of the loop
+            self.host_syncs += 1
+            self.launches_used += int((host > 0).sum())  # the launch after a step that left molecules running is consumed by the next step
+            eng.raise_on_status(worst.cpu())
+            self.status, self.nsteps, self.force_calls, self.function_calls = (mol[:, i].copy() for i in range(4))
+            if (self.status == 4).any():
+                raise NablaB200Error("nb200_qn_step: a molecule larger than max_atoms_per_mol or inverse-Hessian offsets outside the state buffer")
+            failed = np.flatnonzero(self.status == 3)
+            if len(failed):
+                self._sync_atoms(pos)
+                raise RuntimeError(f"LineSearch failed! (molecules {failed.tolist()})")
+            if int(host[-1]) == 0:
+                break
+        if fixed is not None:
+            forces = forces.masked_fill(fixed.bool()[:, None], 0.0)
+        self._sync_atoms(pos)
+        calc.results = {calc.energy_key: energy.cpu().numpy() * calc.property_units[calc.energy_key],
+                        calc.force_key: forces.cpu().numpy() * calc.property_units[calc.force_key]}
+        calc.atoms = [a.copy() for a in self.atoms]
+        self.host_syncs += 1
+        if self.logfile is not None:
+            f = calc.results[calc.force_key]
+            self.logfile.write("%s: %d molecules, %d converged, steps %d..%d, force calls %d..%d, %d engine launches, fmax %.4f\n"
+                               % (self.__class__.__name__, n_mol, int((self.status == 1).sum()), int(self.nsteps.min(initial=0)),
+                                  int(self.nsteps.max(initial=0)), int(self.force_calls.min(initial=0)), int(self.force_calls.max(initial=0)),
+                                  self.launches, sqrt(float((f ** 2).sum(axis=1).max(initial=0.0)))))
+            self.logfile.flush()
+        return bool((self.status == 1).all())
 
 
 class BatchwiseOptimizeTask:
@@ -373,5 +478,5 @@ class PackedOptimizeTask:
             pos_out[a:b] = np.concatenate([at.get_positions() for at in self.optimizer.atoms])
             forces_out[a:b] = res[self.optimizer.calculator.force_key]
             energy_out[ids[0]:ids[-1] + 1] = res[self.optimizer.calculator.energy_key]
-            nsteps.append(self.optimizer.nsteps)
+            nsteps.append(int(np.max(self.optimizer.nsteps)))  # BatchwiseQuasiNewton counts per molecule: the batch's longest
         return {"positions": pos_out, "model_forces": forces_out, "model_energy": energy_out, "nsteps": np.asarray(nsteps)}
