@@ -4,7 +4,7 @@ CUDA events, the engine's per-category split, and the CPU oracle on a bounded sa
 bench.py); prints one JSON line.  NOT YET RUN ON A DEVICE (DESIGN.md 3.9): written together with the first correct path so that the next
 round starts from a measurement.
 
-    python bench_gemnet.py --batch 512 --steps 3 --warmup 3 [--cpu] [--simt]
+    python bench_gemnet.py --batch 512 --steps 3 --warmup 3 [--cpu]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29511 bench_gemnet.py --batch 512
 (weak scaling: every rank runs its own 512-molecule batch, no data-path collective; time = max over ranks, value = all molecules / time)
 """
@@ -50,10 +50,7 @@ def main():
     ap.add_argument("--cpu", action="store_true", help="also time the CPU oracle on the first two molecules")
     ap.add_argument("--train", action="store_true", help="time training steps (L1 energy + L2 force loss as GemNetOCLightning, AdamW) instead of inference; "
                                                          "keeps every activation: use a training-sized batch, e.g. --batch 16")
-    ap.add_argument("--simt", action="store_true", help="NB200_GOC_GEMM=simt: functor GEMM fallback instead of the wgmma GEMMs (bring-up A/B)")
     args = ap.parse_args()
-    if args.simt:
-        os.environ["NB200_GOC_GEMM"] = "simt"
     import numpy as np
     import torch
     import yaml
@@ -127,7 +124,7 @@ def main():
         ms = float(t.item())
         dist.barrier()
     out = {"metric": "molecules/sec (GemNet-OC training step, L1(E) + 100 L2(F), AdamW)" if args.train else "molecules/sec (GemNet-OC E + direct F forward)", "value": world * args.batch / (ms / 1e3), "unit": "molecules/s", "ms_per_step": ms,
-           "n_gpus": world, "scaling": "weak", "batch": args.batch, "atoms": int(b["z"].shape[0]), "counts": net._runner.last_counts, "gemm": "simt" if args.simt else "wgmma-3xTF32",
+           "n_gpus": world, "scaling": "weak", "batch": args.batch, "atoms": int(b["z"].shape[0]), "counts": net._runner.last_counts,
            "peak_mem_gb": torch.cuda.max_memory_allocated() / 2**30, "dtype": "f32", "data": "synthetic", "finite": bool(torch.isfinite(E).all() and torch.isfinite(F).all())}
     if not args.train:
         # tensor roofline of the dense layers: algorithmic fp32 FLOPs / time against the measured bf16 peak / 6 (TF32 runs at half the bf16

@@ -26,7 +26,6 @@ using std::isfinite;
 
 constexpr int H = 256, IE = 64, BE = 8, NSPH = 7, NRAD = 6, NSR = 42, OE = 256, NRES = 3, NLIN = 3, MAXL = 64, NZ = 95;
 
-GD float silu(float x) { return x / (1.0f + expf(-x)); }
 GD float dsilu(float x) {
     const float s = 1.0f / (1.0f + expf(-x));
     return s * (1.0f + x * (1.0f - s));
@@ -243,21 +242,6 @@ struct RbsK {  // SphericalBasisLayer radial part: env(x) N_ln j_l(z_ln x); opti
 };
 
 // ------------------------------------------------------------------ dense helpers
-struct GemmK {  // C[r, n] = (acc ? C : 0) + bias[n] + sum_k A[r, k] op(B)[k, n];  op(B) = B[n, k] (trans 0) | B[k, n] (trans 1)
-    const float* A; int32_t lda; const float* B; int32_t ldb; int32_t trans; float* C; int32_t ldc; int32_t N, K; int32_t acc; const float* bias;
-    GD void operator()(int64_t i) const {
-        const int64_t r = i / N;
-        const int n = (int)(i % N);
-        float s = 0.0f;
-        for (int k = 0; k < K; k++) s += A[r * lda + k] * (trans ? B[(int64_t)k * ldb + n] : B[(int64_t)n * ldb + k]);
-        if (bias) s += bias[n];
-        C[r * ldc + n] = acc ? C[r * ldc + n] + s : s;
-    }
-};
-struct ActK {  // y = silu(x)
-    const float* x; float* y;
-    GD void operator()(int64_t i) const { y[i] = silu(x[i]); }
-};
 struct DActMulK {  // y = g * silu'(pre)
     const float* g; const float* pre; float* y;
     GD void operator()(int64_t i) const { y[i] = g[i] * dsilu(pre[i]); }
@@ -608,16 +592,6 @@ int config_rc(const nb200_dimenet_weights* w) {
     return NB200_OK;
 }
 
-#ifdef NB_EMU
-// host emulation of nb_gemm_tf32x3_ex with a device row count: the "device" count is readable here, so the emulated library GEMM
-// (goc_tc_gemm_ex) runs over min(M, *m_dev) rows and the rows beyond are not written
-inline int emu_gemm_rows(nb200_engine* e, cudaStream_t s, int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans, float* C,
-                         int ldc, int acc, const float* bias, const int32_t* m_dev) {
-    const int64_t rows = ext_rows(M, m_dev);
-    return rows > 0 ? goc_tc_gemm_ex(e, s, (int)rows, N, K, A, lda, B, ldb, trans, C, ldc, acc, bias) : NB200_OK;
-}
-#endif
-
 struct Ctx {
     nb200_engine* e; cudaStream_t s; const nb200_dimenet_weights* w;
     const float* G(int idx) const { return w->w + w->off_host[idx]; }
@@ -626,25 +600,12 @@ struct Ctx {
         return w->w + w->off_host[NB200_DPP_G_COUNT + w->num_blocks * NB200_DPP_I_COUNT + blk * NB200_DPP_O_COUNT + idx];
     }
     // C[M, N] (ldc = N) = (acc ? C : 0) + A[M, K] op(B) (+ bias); act != nullptr: act = silu(C) (C keeps the pre-activation).
+    // trans = 0: B[N, K], a layer (dense_fwd); trans = 1: B[K, N], the input gradient of a layer (dense_dgrad), without bias or act.
     // Mx.dev set: Mx.n is the bound (grid, kernel choice), rows at or beyond the device count are neither computed nor written.
     int gemm(Ext Mx, int N, int K, const float* A, const float* B, int trans, float* C, int acc, const float* bias, float* act) const {
-        const int64_t M = Mx.n;
-        if (M <= 0) return NB200_OK;
-        if (M > 0x7fffffff) return NB200_EUNSUPPORTED;
-        const int ldb = trans ? N : K;
-#ifndef NB_EMU
-        if (goc_tc_ok(N, K, K, ldb, N)) {
-            Scope sc(e, s, CAT_GEMM, 1);
-            return nb_gemm_tf32x3_ex((int)M, N, K, A, K, B, ldb, trans, C, N, acc, bias, act, NB_ACT_SILU, s, Mx.dev);
-        }
-#else
-        if (goc_tc_ok(N, K, K, ldb, N)) {
-            NB_TRY(emu_gemm_rows(e, s, (int)M, N, K, A, K, B, ldb, trans, C, N, acc, bias, Mx.dev));
-            return act ? pfor(e, s, CAT_NODE, Mx, N, ActK{C, act}) : NB200_OK;
-        }
-#endif
-        NB_TRY(pfor(e, s, CAT_GEMM, Mx, N, GemmK{A, K, B, ldb, trans, C, N, N, K, acc, bias}));
-        return act ? pfor(e, s, CAT_NODE, Mx, N, ActK{C, act}) : NB200_OK;
+        if (Mx.n > 0x7fffffff) return NB200_EUNSUPPORTED;
+        if (!trans) return dense_fwd(e, s, Mx, N, K, A, K, B, K, C, N, acc, bias, act);
+        return bias || act ? NB200_EINVAL : dense_dgrad(e, s, Mx, K, N, A, K, B, N, C, N, acc);
     }
     // ResidualLayer: out = in + silu(W2 silu(W1 in + b1) + b2); keeps q1, q2 (pre-activations); tmp holds silu(q1)
     int res_fwd(Ext E, const float* in, int r, int blk, float* q1, float* q2, float* tmp, float* out) const {
@@ -949,11 +910,11 @@ extern "C" int nb200_dimenet_debug_sbf_radial(const nb200_dimenet_weights* w, co
 }
 
 #ifdef NB_EMU
-// the test entry of gemm_tc.cu in the emulation build, on the emulated GEMM (no act output: the engine applies the activation separately)
+// the test entry of gemm_tc.cu in the emulation build, on the emulated GEMM (no act output: the emulation applies the activation separately)
 extern "C" int nb200_gemm_tf32x3_rows(int32_t M, int32_t N, int32_t K, const float* A, int32_t lda, const float* B, int32_t ldb, int32_t trans_b,
                                       float* C, int32_t ldc, int32_t accumulate, const float* bias, float* act, const int32_t* m_dev, void* stream) {
     if (!A || !B || !C || act || M < 0 || N <= 0 || K <= 0) return NB200_EINVAL;
-    return emu_gemm_rows(nullptr, (cudaStream_t)stream, M, N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, m_dev);
+    return tc_gemm(nullptr, (cudaStream_t)stream, Ext(M, m_dev), N, K, A, lda, B, ldb, trans_b, C, ldc, accumulate, bias, nullptr);
 }
 #endif
 

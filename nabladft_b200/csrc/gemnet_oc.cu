@@ -112,11 +112,8 @@ struct Ctx {
 
     // M.n rows are computed whether or not M.dev says fewer: rows are independent, and no kernel reads a row at or past the device count
     int gemm(Ext Mx, int N, int K, const float* A, int lda, const float* W, int ldw, float* C, int ldc) const {
-        const int64_t M = Mx.n;
-        if (M <= 0) return NB200_OK;
-        if (M > 0x7fffffff) return NB200_EUNSUPPORTED;
-        if (goc_tc_ok(N, K, lda, ldw, ldc)) return goc_tc_gemm(e, s, (int)M, N, K, A, lda, W, ldw, C, ldc);
-        return pfor(e, s, CAT_GEMM, M * N, LinK{A, lda, W, ldw, C, ldc, N, K});
+        if (Mx.n > 0x7fffffff) return NB200_EUNSUPPORTED;
+        return dense_fwd(e, s, Mx.n, N, K, A, lda, W, ldw, C, ldc);
     }
     int act(float* x, Ext M, int C) const { return pfor(e, s, CAT_NODE, M, C, SsiluK{x}); }
     // tall layers on the device: the activation / residual tail runs in the GEMM's epilogue (gemm_ps.cu NB_EPI_*) -- one pass over the

@@ -362,18 +362,6 @@ struct AggAtomRbfK {
         out[i] = acc * scale;
     }
 };
-struct LinK {  // functor GEMM fallback: C[r, n] = A[r, :] . W[n, :]
-    const float* A; int32_t lda; const float* W; int32_t ldw; float* C; int32_t ldc; int32_t N, K;
-    GD void operator()(int64_t i) const {
-        const int64_t r = i / N; const int n = (int)(i % N);
-        const float* a = A + r * lda; const float* w = W + (int64_t)n * ldw;
-        float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
-        int k = 0;
-        for (; k + 4 <= K; k += 4) { s0 += a[k] * w[k]; s1 += a[k + 1] * w[k + 1]; s2 += a[k + 2] * w[k + 2]; s3 += a[k + 3] * w[k + 3]; }
-        for (; k < K; k++) s0 += a[k] * w[k];
-        C[r * ldc + n] = (s0 + s1) + (s2 + s3);
-    }
-};
 struct DotRowK {
     const float* x; int32_t C; const float* w; float* out;
     GD void operator()(int64_t r) const {

@@ -1,4 +1,4 @@
-// gemnet_pf.cuh -- launch abstraction of the functor engines (gemnet_oc.cu + gemnet_oc_train.inc, schnet_train.cu).
+// gemnet_pf.cuh -- launch abstraction and dense layers of the functor engines (gemnet_oc.cu, schnet_train.cu, dimenet.cu).
 //
 // Every kernel of these engines is a functor with `operator()(int64_t i)`: one logical thread per output element, no shared memory, no warp
 // intrinsics; forward aggregations are gathers over CSR rows (deterministic), only some backward scatters use atomicAdd.  `pfor` launches a
@@ -149,31 +149,17 @@ inline int goc_d2h_sync(void* dst, const void* src, size_t bytes, cudaStream_t s
 inline int goc_d2d(void* dst, const void* src, size_t bytes, cudaStream_t s) {
     return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s) == cudaSuccess ? NB200_OK : NB200_ECUDA;
 }
-// tensor-core GEMM when the shape fits the wgmma kernels' tiling, else the functor fallback in gemnet_oc.cu
-// NB200_GOC_GEMM=simt forces the fallback everywhere (A/B runs, bring-up of new shapes)
+// the shape fits the tiling of the wgmma GEMM (nb_gemm_tf32x3_ex)
 inline bool goc_tc_ok(int N, int K, int lda, int ldw, int ldc) {
-    static const bool simt = [] { const char* e = getenv("NB200_GOC_GEMM"); return e && e[0] == 's'; }();
     // N % 32: the 128 x 64 tile kernel masks the columns beyond N, so the quadruplet bilinear layer (1024 -> 32 per edge, ~6 % of the model's
     // FLOPs) runs on the tensor cores with a half-empty tile instead of the functor fallback
-    return !simt && N % 32 == 0 && K % 32 == 0 && lda % 4 == 0 && ldw % 4 == 0 && ldc % 4 == 0;
-}
-inline int goc_tc_gemm(nb200_engine* e, cudaStream_t s, int M, int N, int K, const float* A, int lda, const float* W, int ldw, float* C, int ldc) {
-    Scope sc(e, s, CAT_GEMM, 1);
-    return nb_gemm_tf32x3_ex(M, N, K, A, lda, W, ldw, 0, C, ldc, 0, nullptr, nullptr, NB_ACT_SILU, s);
-}
-// general form: C (+)= A op(W) (+ bias);  trans_w = 0: W[N,K] (Linear forward), 1: W[K,N] (Linear backward w.r.t. the input)
-inline int goc_tc_gemm_ex(nb200_engine* e, cudaStream_t s, int M, int N, int K, const float* A, int lda, const float* W, int ldw, int trans_w, float* C,
-                          int ldc, int accumulate, const float* bias) {
-    Scope sc(e, s, CAT_GEMM, 1);
-    return nb_gemm_tf32x3_ex(M, N, K, A, lda, W, ldw, trans_w, C, ldc, accumulate, bias, nullptr, NB_ACT_SILU, s);
+    return N % 32 == 0 && K % 32 == 0 && lda % 4 == 0 && ldw % 4 == 0 && ldc % 4 == 0;
 }
 // dW[out, in] (lddw) += alpha * gY[M, out]^T (ldgy) . X[M, in] (ldx): weight gradient of a Linear layer as ONE cuBLAS SGEMM (fp32, no TF32).
-// false = not available (NB200_GOC_GEMM=simt, no handle): the caller falls back to its row-chunked functor reduction (which is also what host
-// emulation runs).
+// false = not available (no handle, M beyond int32): the caller falls back to the row-chunked functor reduction.
 inline bool goc_wgrad(nb200_engine* e, cudaStream_t s, int64_t M, int out, int in, const float* gY, int ldgy, const float* X, int ldx, float* dW, int lddw,
                       float alpha, int* rc) {
-    static const bool simt = [] { const char* v = getenv("NB200_GOC_GEMM"); return v && v[0] == 's'; }();
-    if (simt || !e || !e->blas || M > 0x7fffffff || M <= 0 || out <= 0 || in <= 0) return false;
+    if (!e || !e->blas || M > 0x7fffffff || M <= 0 || out <= 0 || in <= 0) return false;
     Scope sc(e, s, CAT_GEMM, 0);
     const float beta = 1.0f;
     *rc = (cublasSetStream(e->blas, s) == CUBLAS_STATUS_SUCCESS &&
@@ -183,3 +169,96 @@ inline bool goc_wgrad(nb200_engine* e, cudaStream_t s, int64_t M, int out, int i
     return true;
 }
 #endif
+
+// ---------------------------------------------------------------- dense layers of the functor engines
+// Each layer runs on the wgmma 3xTF32 GEMM when its shape tiles and M fits int32, else on a functor GEMM; weight gradients run as one cuBLAS
+// SGEMM, else as a row-chunked functor reduction.  Host emulation takes the functors, or with NB200_EMU_LIBGEMM=1 the library stand-ins of
+// emu_shim.h.
+namespace {
+constexpr int WGRAD_ROWS = 512;  // rows one thread of DenseWgradK sums before its atomicAdd
+
+GD float silu(float x) { return x / (1.0f + expf(-x)); }
+struct ActK {  // y = silu(x)
+    const float* x; float* y;
+    GD void operator()(int64_t i) const { y[i] = silu(x[i]); }
+};
+struct DenseK {  // C[r, n] (+)= A[r, :] . W[n, :] (+ bias[n])
+    const float* A; int32_t lda; const float* W; int32_t ldw; float* C; int32_t ldc; int32_t N, K; const float* bias; int32_t acc;
+    GD void operator()(int64_t i) const {
+        const int64_t r = i / N; const int n = (int)(i % N);
+        const float* a = A + r * lda; const float* w = W + (int64_t)n * ldw;
+        float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
+        int k = 0;
+        for (; k + 4 <= K; k += 4) { s0 += a[k] * w[k]; s1 += a[k + 1] * w[k + 1]; s2 += a[k + 2] * w[k + 2]; s3 += a[k + 3] * w[k + 3]; }
+        for (; k < K; k++) s0 += a[k] * w[k];
+        float v = (s0 + s1) + (s2 + s3);
+        if (bias) v += bias[n];
+        float& c = C[r * ldc + n];
+        c = acc ? c + v : v;
+    }
+};
+struct DenseDgradK {  // gA[r, k] (+)= sum_n gC[r, n] W[n, k]
+    const float* gC; int32_t ldc; const float* W; int32_t ldw; float* gA; int32_t lda; int32_t N, K; int32_t acc;
+    GD void operator()(int64_t i) const {
+        const int64_t r = i / K; const int k = (int)(i % K);
+        const float* g = gC + r * ldc;
+        float s0 = 0.0f, s1 = 0.0f;
+        int n = 0;
+        for (; n + 2 <= N; n += 2) { s0 += g[n] * W[(int64_t)n * ldw + k]; s1 += g[n + 1] * W[(int64_t)(n + 1) * ldw + k]; }
+        if (n < N) s0 += g[n] * W[(int64_t)n * ldw + k];
+        float& c = gA[r * lda + k];
+        c = acc ? c + (s0 + s1) : (s0 + s1);
+    }
+};
+struct DenseWgradK {  // gW[n, k] += alpha * sum over a chunk of rows of gC[r, n] A[r, k];  i = (chunk, n, k)
+    const float* gC; int32_t ldc; const float* A; int32_t lda; float* gW; int32_t ldw; int32_t N, K; int64_t M; float alpha;
+    GD void operator()(int64_t i) const {
+        const int64_t nk = (int64_t)N * K, chunk = i / nk;
+        const int n = (int)((i % nk) / K), k = (int)(i % K);
+        const int64_t r0 = chunk * WGRAD_ROWS, r1 = r0 + WGRAD_ROWS < M ? r0 + WGRAD_ROWS : M;
+        float s = 0.0f;
+        for (int64_t r = r0; r < r1; r++) s += gC[r * ldc + n] * A[r * lda + k];
+        atomicAdd(gW + (int64_t)n * ldw + k, alpha * s);
+    }
+};
+
+// The wgmma GEMM nb_gemm_tf32x3_ex: C[M, N] (ldc) (+)= A[M, K] (lda) . op(W) (+ bias[N]), op(W) = W[N, K]^T (trans 0) | W[K, N] (trans 1);
+// act != nullptr (ldc == N): act = silu(C).  Host emulation runs the stand-in goc_tc_gemm_ex of emu_shim.h over the rows below the "device"
+// count (readable there) and applies the activation separately.
+inline int tc_gemm(nb200_engine* e, cudaStream_t s, Ext M, int N, int K, const float* A, int lda, const float* W, int ldw, int trans, float* C, int ldc,
+                   bool acc, const float* bias, float* act) {
+#ifdef NB_EMU
+    const int64_t rows = ext_rows(M.n, M.dev);
+    if (rows > 0) NB_TRY(goc_tc_gemm_ex(e, s, (int)rows, N, K, A, lda, W, ldw, trans, C, ldc, acc, bias));
+    return act ? pfor(e, s, CAT_NODE, M, N, ActK{C, act}) : NB200_OK;
+#else
+    Scope sc(e, s, CAT_GEMM, 1);
+    return nb_gemm_tf32x3_ex((int)M.n, N, K, A, lda, W, ldw, trans, C, ldc, acc, bias, act, NB_ACT_SILU, s, M.dev);
+#endif
+}
+
+// C[M, N] (ldc) (+)= A[M, K] (lda) . W[N, K]^T (ldw) (+ bias[N]);  act != nullptr (ldc == N): act = silu(C), C keeps the pre-activation.
+// M.dev set: M.n is the bound, and rows at or past the device count are neither computed nor written.
+inline int dense_fwd(nb200_engine* e, cudaStream_t s, Ext M, int N, int K, const float* A, int lda, const float* W, int ldw, float* C, int ldc,
+                     bool acc = false, const float* bias = nullptr, float* act = nullptr) {
+    if (M.n <= 0) return NB200_OK;
+    if (M.n <= 0x7fffffff && goc_tc_ok(N, K, lda, ldw, ldc)) return tc_gemm(e, s, M, N, K, A, lda, W, ldw, 0, C, ldc, acc, bias, act);
+    NB_TRY(pfor(e, s, CAT_GEMM, M, N, DenseK{A, lda, W, ldw, C, ldc, N, K, bias, acc}));
+    return act ? pfor(e, s, CAT_NODE, M, N, ActK{C, act}) : NB200_OK;
+}
+// gA[M, K] (lda) (+)= gC[M, N] (ldc) . W[N, K] (ldw): the input gradient of dense_fwd.  M as in dense_fwd.
+inline int dense_dgrad(nb200_engine* e, cudaStream_t s, Ext M, int N, int K, const float* gC, int ldc, const float* W, int ldw, float* gA, int lda,
+                       bool acc) {
+    if (M.n <= 0) return NB200_OK;
+    if (M.n <= 0x7fffffff && goc_tc_ok(K, N, ldc, ldw, lda)) return tc_gemm(e, s, M, K, N, gC, ldc, W, ldw, 1, gA, lda, acc, nullptr, nullptr);
+    return pfor(e, s, CAT_GEMM, M, K, DenseDgradK{gC, ldc, W, ldw, gA, lda, N, K, acc});
+}
+// gW[N, K] (ldw) += alpha * gC[M, N]^T (ldc) . A[M, K] (lda): the weight gradient of dense_fwd
+inline int dense_wgrad(nb200_engine* e, cudaStream_t s, int64_t M, int N, int K, const float* gC, int ldc, const float* A, int lda, float* gW, int ldw,
+                       float alpha = 1.0f) {
+    if (M <= 0) return NB200_OK;
+    int rc = NB200_OK;
+    if (goc_wgrad(e, s, M, N, K, gC, ldc, A, lda, gW, ldw, alpha, &rc)) return rc;
+    return pfor(e, s, CAT_GEMM, (M + WGRAD_ROWS - 1) / WGRAD_ROWS * N * K, DenseWgradK{gC, ldc, A, lda, gW, ldw, N, K, M, alpha});
+}
+}  // namespace

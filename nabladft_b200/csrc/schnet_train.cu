@@ -1,14 +1,12 @@
 // schnet_train.cu -- SchNet parameter gradients of an energy loss (SURVEY.md section 8 a8 + a10/a11; BASELINE configs[0]: SchNet energy-only
-// training).  First correct path, NOT YET RUN ON A DEVICE: verified on the CPU through the host-emulation build (tests/emu,
-// tests/test_schnet_train_emu.py) against the autograd of the oracle (oracle/spk.py).
+// training).  Runs on the device, checked there and under host emulation (tests/emu) against the autograd of the oracle (oracle/spk.py).
 //
 // Reference: schnetpack 2.0.4 SchNet / Atomwise as wired by config/model/schnet.yaml (SURVEY.md A.1) trained by `loss.backward()` through the
 // eager graph (nablaDFT/ase_model/task.py).  Here ONE call does the forward with saved activations and the reverse sweep:
 //     grads = d( sum_m seed_m E_m ) / d(canonical weights),   seed = dLoss/dE from the autograd bridge (nabladft_b200/training.py).
 // The neighbour relation is symmetric and the filter of an edge depends on its length only, so both the cfconv forward and its backward
 // w.r.t. the source features are GATHERS over the CSR row of the receiving atom -- the same kernel (CfconvK) serves both; no atomics there.
-// Weight gradients G^T X are row-chunked functor reductions with atomicAdd into zeroed buffers (cuBLAS would do on the device; the functor
-// keeps the emulated and the device code identical).  A force loss (the reference's create_graph double backward) is handled as in the PaiNN
+// Weight gradients G^T X accumulate into zeroed buffers (dense_wgrad, gemnet_pf.cuh: cuBLAS on the device).  A force loss (the reference's create_graph double backward) is handled as in the PaiNN
 // engine (DESIGN.md 3.7): sum_i v_i . dF_i/dtheta = -(v . d/dR)[dE_tot/dtheta], i.e. a second reverse sweep with unit seeds that carries the
 // tangent of every forward and backward quantity along v in position space.
 #include "gemnet_pf.cuh"
@@ -95,45 +93,6 @@ struct SLinKmajorK {
         for (; k + 2 <= K; k += 2) { s0 += a[k] * Wt[(int64_t)k * N + n]; s1 += a[k + 1] * Wt[(int64_t)(k + 1) * N + n]; }
         if (k < K) s0 += a[k] * Wt[(int64_t)k * N + n];
         out[i] = s0 + s1 + (bias ? bias[n] : 0.0f);
-    }
-};
-// C[r, n] (+)= bias[n] + sum_k A[r, k] W[n, k]   (torch.nn.Linear forward)
-struct SLinK {
-    const float* A; int32_t K; const float* W; const float* bias; float* C; int32_t N; int32_t accumulate;
-    GD void operator()(int64_t i) const {
-        const int64_t r = i / N; const int n = (int)(i % N);
-        const float* a = A + r * K; const float* w = W + (int64_t)n * K;
-        float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
-        int k = 0;
-        for (; k + 4 <= K; k += 4) { s0 += a[k] * w[k]; s1 += a[k + 1] * w[k + 1]; s2 += a[k + 2] * w[k + 2]; s3 += a[k + 3] * w[k + 3]; }
-        for (; k < K; k++) s0 += a[k] * w[k];
-        const float v = (s0 + s1) + (s2 + s3) + (bias ? bias[n] : 0.0f);
-        C[i] = accumulate ? C[i] + v : v;
-    }
-};
-// C[r, k] (+)= sum_n G[r, n] W[n, k]   (Linear backward w.r.t. its input)
-struct SLinBwdK {
-    const float* G; int32_t N; const float* W; float* C; int32_t K; int32_t accumulate;
-    GD void operator()(int64_t i) const {
-        const int64_t r = i / K; const int k = (int)(i % K);
-        const float* g = G + r * N;
-        float s0 = 0.0f, s1 = 0.0f;
-        int n = 0;
-        for (; n + 2 <= N; n += 2) { s0 += g[n] * W[(int64_t)n * K + k]; s1 += g[n + 1] * W[(int64_t)(n + 1) * K + k]; }
-        if (n < N) s0 += g[n] * W[(int64_t)n * K + k];
-        C[i] = accumulate ? C[i] + (s0 + s1) : (s0 + s1);
-    }
-};
-// dW[n, k] += sum over a chunk of rows of G[r, n] X[r, k];  i = (chunk, n, k)
-struct SWgradK {
-    const float* G; int32_t N; const float* X; int32_t K; int64_t M; float* dW; float alpha;
-    GD void operator()(int64_t i) const {
-        const int64_t nk = (int64_t)N * K, chunk = i / nk;
-        const int n = (int)((i % nk) / K), k = (int)(i % K);
-        const int64_t r0 = chunk * WG_ROWS, r1 = r0 + WG_ROWS < M ? r0 + WG_ROWS : M;
-        float s = 0.0f;
-        for (int64_t r = r0; r < r1; r++) s += G[r * N + n] * X[r * K + k];
-        atomicAdd(dW + (int64_t)n * K + k, alpha * s);
     }
 };
 struct SColsumK {  // db[n] += alpha * sum over a chunk of rows of G[r, n];  i = (chunk, n)
@@ -368,27 +327,18 @@ inline int64_t chunks(int64_t M) { return (M + WG_ROWS - 1) / WG_ROWS; }
 
 struct Run {
     nb200_engine* e; cudaStream_t s;
-    // dense layers: the wgmma 3xTF32 GEMM of gemm_tc.cu on the device (shapes of the classes its unit tests cover: N, K in {64, 128},
-    // bias epilogue, trans_b, accumulate), the functor fallback under host emulation or NB200_GOC_GEMM=simt
+    // dense layers (gemnet_pf.cuh) on packed rows: C[M, N] (+)= A[M, K] W[N, K]^T (+ bias)
     int lin(int64_t M, int N, int K, const float* A, const float* W, const float* bias, float* C, bool acc = false) const {
-        if (M <= 0) return NB200_OK;
-        if (M <= 0x7fffffff && goc_tc_ok(N, K, K, K, N)) return goc_tc_gemm_ex(e, s, (int)M, N, K, A, K, W, K, 0, C, N, acc ? 1 : 0, bias);
-        return pfor(e, s, CAT_GEMM, M * N, SLinK{A, K, W, bias, C, N, acc ? 1 : 0});
+        return dense_fwd(e, s, M, N, K, A, K, W, K, C, N, acc, bias);
     }
     // C[M, K] (+)= G[M, N] W[N, K]
     int lin_bwd(int64_t M, int N, int K, const float* G, const float* W, float* C, bool acc = false) const {
-        if (M <= 0) return NB200_OK;
-        if (M <= 0x7fffffff && goc_tc_ok(K, N, N, K, K)) return goc_tc_gemm_ex(e, s, (int)M, K, N, G, N, W, K, 1, C, K, acc ? 1 : 0, nullptr);
-        return pfor(e, s, CAT_GEMM, M * K, SLinBwdK{G, N, W, C, K, acc ? 1 : 0});
+        return dense_dgrad(e, s, M, N, K, G, N, W, K, C, K, acc);
     }
     // dW[N, K] += G[M, N]^T X[M, K];  db[N] += colsum(G)
     int wgrad(int64_t M, int N, int K, const float* G, const float* X, float* dW, float* db, float alpha = 1.0f) const {
         if (M <= 0) return NB200_OK;
-        if (dW) {
-            int rc = NB200_OK;
-            if (goc_wgrad(e, s, M, N, K, G, N, X, K, dW, K, alpha, &rc)) NB_TRY(rc);  // cuBLAS on the device
-            else NB_TRY(pfor(e, s, CAT_GEMM, chunks(M) * N * K, SWgradK{G, N, X, K, M, dW, alpha}));
-        }
+        if (dW) NB_TRY(dense_wgrad(e, s, M, N, K, G, N, X, K, dW, K, alpha));
         if (db) NB_TRY(pfor(e, s, CAT_NODE, chunks(M) * N, SColsumK{G, N, M, db, alpha}));
         return NB200_OK;
     }

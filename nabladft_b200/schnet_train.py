@@ -10,8 +10,8 @@ activations and returns the gradient w.r.t. the canonical weight tensors; autogr
 Both terms are exact: the energy term is a reverse sweep seeded with dLoss/dE; the force term (the reference's create_graph double backward)
 is the tangent pass of DESIGN.md 3.7: sum_i v_i . dF_i/dtheta = -(v . d/dR)[dE_tot/dtheta] with v = dLoss/dF.  The force VALUES come from the
 inference engine (csrc/schnet.cu).
-STATUS (round 1): first correct path, verified against the oracle's autograd under host emulation (tests/test_schnet_train_emu.py); not yet run
-on a device.  No CPU fallback: the product entry (`spk.NeuralNetworkPotential.forward`) accepts CUDA tensors only.
+STATUS: runs on the device; its gradients match the oracle's autograd there and under host emulation (tests/test_schnet_train_emu.py).
+No CPU fallback: the product entry (`spk.NeuralNetworkPotential.forward`) accepts CUDA tensors only.
 """
 from ctypes import byref, c_int64
 from typing import Dict, List, Optional

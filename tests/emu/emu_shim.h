@@ -73,9 +73,6 @@ inline int emu_ref_gemm(int M, int N, int K, const float* A, int lda, const floa
     }
     return NB200_OK;
 }
-inline int goc_tc_gemm(nb200_engine*, cudaStream_t, int M, int N, int K, const float* A, int lda, const float* W, int ldw, float* C, int ldc) {
-    return emu_ref_gemm(M, N, K, A, lda, W, ldw, 0, C, ldc, 0, nullptr);
-}
 inline int goc_tc_gemm_ex(nb200_engine*, cudaStream_t, int M, int N, int K, const float* A, int lda, const float* W, int ldw, int trans_w, float* C, int ldc,
                           int accumulate, const float* bias) {
     return emu_ref_gemm(M, N, K, A, lda, W, ldw, trans_w, C, ldc, accumulate, bias);

@@ -9,7 +9,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "nabladft_b200")
 
 ALLOWED = {
-    "NB200_GOC_GEMM",        # =simt: GemNet-OC dense layers on the functor GEMM (tells kernel faults from GEMM-dispatch faults)
     "NB200_TRAIN_STORAGE",   # default per-edge storage of the training arrays (a precision choice, INTEGRATION.md)
     "NB200_QH_PAIR_CHUNK",   # QHNet memory bound: atom pairs whose path weights exist at a time
     "NVCC",                  # build: compiler
