@@ -151,7 +151,8 @@ typedef struct nb200_painn_weights {
     int32_t radial_mode, z_offset;           /* NB200_RADIAL_*, 0 (spk) or 1 (OC: emb[z-1]) */
     float cutoff, epsilon;                   /* 5.0, 1e-8                                   */
     float rbf_coeff, rbf_xscale;             /* phi_k = exp(coeff (d*xscale - offsets[k])^2) */
-    const float* rbf_offsets;                /* [K] Gaussian centres (module buffer)        */
+    const float* rbf_offsets;                /* [K] Gaussian centres (module buffer); must be k dx, dx = cutoff xscale / (K - 1):
+                                              * the filter evaluates only the 16 centres around bin floor(d xscale / dx) */
     float energy_shift_per_atom;             /* spk AddOffsets mean (eval); 0 otherwise     */
     int32_t max_neighbors;                   /* OC: 100; spk: INT32_MAX                     */
     const float* emb;                        /* [n_elem][F]                                 */
@@ -378,7 +379,8 @@ typedef struct nb200_schnet_weights {
     int32_t z_offset;                        /* 0                                            */
     float cutoff, rbf_coeff;                 /* 5.0 ; phi_k = exp(coeff (d - offsets[k])^2)  */
     float energy_shift_per_atom;             /* AddOffsets mean (eval)                       */
-    const float* rbf_offsets;                /* [K]                                          */
+    const float* rbf_offsets;                /* [K]; must be k dx, dx = cutoff / (K - 1): nb200_schnet_energy_forces evaluates only the
+                                              * 16 centres around bin floor(d / dx) (the training and Hessian entries evaluate all K) */
     const float* emb;                        /* [n_elem][F]                                  */
     const float* w_f1; const float* b_f1;    /* [L][K][F] (K-major), [L][F]  filter_network.0 (ssp) */
     const float* W_f2; const float* b_f2;    /* [L][F][F], [L][F]            filter_network.1 */
@@ -396,6 +398,25 @@ int nb200_schnet_energy_forces(nb200_engine* eng, const nb200_schnet_weights* w,
                                int32_t n_mol, int32_t n_atoms, int32_t e_cap,
                                void* workspace, int64_t workspace_bytes,
                                float* energy, float* forces, int32_t* status, void* stream);
+/* Test entry point, not a supported API: ONE launch of nb200_schnet_energy_forces (csrc/schnet.cu) on caller-built inputs, through the
+ * wrapper the engine calls (hence its launch configuration).  F = 128; per-edge rows [E][F] in CSR order, geom [E][4] with d in slot 3.  `op`:
+ *   FILTER1      geom status(= {n_edges, 0}) w_f1 b_f1 rbf_offsets n_layers n_rbf cutoff rbf_coeff e_stride, sort_scratch int32
+ *                [768 + n_edges] -> HH [n_layers][2][e_stride][F] (h, dh/dd; rows at and past n_edges untouched)
+ *   CFCONV_FWD   y G1 b2 geom row_ptr col cutoff n_atoms -> agg [n_atoms][F]
+ *   CFCONV_BWD   y G1 G2 b2 geom row_ptr col cutoff n_atoms gagg -> gy [n_atoms][F], egrad[4 e + 3] (accumulated)
+ *   LINEAR_ACT   X [m][F] W [F][F] bias [F] -> Y = X W^T + bias, act = ssp(Y)      (the GEMM the engine runs for f2out.0)
+ * NB200_EINVAL (nothing launched) for an unknown op, a NULL field the op uses, a pointer the float4 paths read or write that is not 16-byte
+ * aligned, a negative count or e_stride < n_edges; NB200_EUNSUPPORTED for n_rbf or rbf_coeff that nb200_schnet_energy_forces refuses. */
+enum { NB200_SC_FILTER1 = 0, NB200_SC_CFCONV_FWD, NB200_SC_CFCONV_BWD, NB200_SC_LINEAR_ACT, NB200_SC_N_OPS };
+typedef struct nb200_schnet_test_args {
+    int32_t op, n_layers, n_rbf, n_atoms, n_edges, e_stride, m;
+    float cutoff, rbf_coeff;
+    const int32_t *status, *row_ptr, *col;
+    int32_t* sort_scratch;
+    const float *geom, *rbf_offsets, *w_f1, *b_f1, *y, *G1, *G2, *b2, *gagg, *X, *W, *bias;
+    float *HH, *agg, *gy, *egrad, *Y, *act;
+} nb200_schnet_test_args;
+int nb200_schnet_test_op(const nb200_schnet_test_args* args, void* stream);
 
 /* SchNet parameter gradients of energy and force losses (config/model/schnet.yaml; BASELINE configs[0]; SURVEY.md section 8 a8 / a10 / a11).
  * Replaces `loss.backward()` through schnetpack's eager SchNet + Atomwise graph (config/model/schnet.yaml, nablaDFT/ase_model/task.py) for

@@ -111,6 +111,19 @@ class PainnNodeArgs(ctypes.Structure):
 PN_OPS = ("PREP", "NODE_FWD", "NODE_BWD", "EMBED", "ACT_BWD", "UPD_COMBINE_BWD", "UPD_NORM_BWD", "READOUT", "MOL_SUM", "READOUT_BWD", "POISON")
 
 
+class SchnetTestArgs(ctypes.Structure):
+    """Mirror of `struct nb200_schnet_test_args` (include/nabla_b200.h)."""
+
+    _fields_ = [(name, c_int32) for name in ("op", "n_layers", "n_rbf", "n_atoms", "n_edges", "e_stride", "m")] + [
+        ("cutoff", c_float), ("rbf_coeff", c_float)] + [(name, c_void_p) for name in (
+            "status", "row_ptr", "col", "sort_scratch", "geom", "rbf_offsets", "w_f1", "b_f1", "y", "G1", "G2", "b2", "gagg", "X", "W", "bias",
+            "HH", "agg", "gy", "egrad", "Y", "act")]
+
+
+# nb200_schnet_test_op ops (enum NB200_SC_*)
+SC_OPS = ("FILTER1", "CFCONV_FWD", "CFCONV_BWD", "LINEAR_ACT")
+
+
 class DimeNetWeights(ctypes.Structure):
     """Mirror of `struct nb200_dimenet_weights` (include/nabla_b200.h)."""
 
@@ -204,6 +217,7 @@ SIGNATURES = {
                                   c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_painn_test_tangent": (c_int32, [POINTER(PainnTanArgs), c_void_p]),
     "nb200_painn_test_node": (c_int32, [POINTER(PainnNodeArgs), c_void_p]),
+    "nb200_schnet_test_op": (c_int32, [POINTER(SchnetTestArgs), c_void_p]),
 
     "nb200_gemnet_oc_graph_bytes": (c_int64, [c_int32, c_int32]),
     "nb200_gemnet_oc_graph_count": (c_int32, [POINTER(GemNetOCWeights), c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int64,

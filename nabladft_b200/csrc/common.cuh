@@ -151,6 +151,14 @@ int nb_painn_msg_fwd_ex(const float* xh, const float* xh_bias, const float* q, c
 int nb_painn_msg_bwd_ex(const float* xh, const float* xh_bias, const float* mu, const float* W, const float* dW, int w_stride, const int32_t* rev,
                         const float* geom, const int32_t* row_ptr, const int32_t* col, int32_t n_atoms, const float* g_q, const float* g_mu,
                         float* g_xh, float* g_mu_in, float* egrad, cudaStream_t s, int bf16 = 0);
+// SchNet inference launches (schnet.cu), shared by nb200_schnet_energy_forces and its test entry nb200_schnet_test_op.  filter1: edges sorted by
+// distance bin into sort_scr, then HH[l][0|1][e][F] = h, dh/dd of every layer's first filter layer.  cfconv: one warp per atom over its CSR row.
+int nb_schnet_filter1(const float* geom, const int32_t* status, const float* w1, const float* b1, const float* offsets, int n_layers, int n_rbf,
+                      float cutoff, float coeff, size_t e_stride, int32_t* sort_scr, float* HH, cudaStream_t s);
+int nb_schnet_cfconv_fwd(const float* y, const float* G1, const float* b2, const float* geom, const int32_t* row_ptr, const int32_t* col, float cutoff,
+                         int n_atoms, float* agg, cudaStream_t s);
+int nb_schnet_cfconv_bwd(const float* y, const float* G1, const float* G2, const float* b2, const float* geom, const int32_t* row_ptr, const int32_t* col,
+                         float cutoff, int n_atoms, const float* gagg, float* gy, float* egrad, cudaStream_t s);
 bool nb_gemm_ps_wanted(int M, int N, int K);
 size_t nb_gemm_ps_ws_bytes(int N, int K);
 int nb_gemm_ps(int M, int N, int K, const float* A, int lda, const float* B, int ldb, int trans_b, float* C, int ldc, int accumulate,

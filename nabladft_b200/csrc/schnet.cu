@@ -256,6 +256,26 @@ bool s_weights_ok(const nb200_schnet_weights* w) {
 
 }  // namespace
 
+int nb_schnet_filter1(const float* geom, const int32_t* status, const float* w1, const float* b1, const float* offsets, int n_layers, int n_rbf,
+                      float cutoff, float coeff, size_t e_stride, int32_t* sort_scr, float* HH, cudaStream_t s) {
+    const float dx = cutoff / (float)(n_rbf - 1);
+    NB_TRY(nb_bin_sort(geom, status, 1.0f, 1.0f / dx, n_rbf, sort_scr, s));
+    k_schnet_filter1<<<dim3(n_rbf, SF1_SPLIT, n_layers), SF1_THREADS, 0, s>>>(geom, status, sort_scr, w1, b1, offsets, n_rbf, coeff, e_stride, HH);
+    return nb_check_launch();
+}
+
+int nb_schnet_cfconv_fwd(const float* y, const float* G1, const float* b2, const float* geom, const int32_t* row_ptr, const int32_t* col, float cutoff,
+                         int n_atoms, float* agg, cudaStream_t s) {
+    k_cfconv_fwd<<<(n_atoms + CF_WARPS - 1) / CF_WARPS, CF_THREADS, 0, s>>>(y, G1, b2, geom, row_ptr, col, cutoff, n_atoms, agg);
+    return nb_check_launch();
+}
+
+int nb_schnet_cfconv_bwd(const float* y, const float* G1, const float* G2, const float* b2, const float* geom, const int32_t* row_ptr, const int32_t* col,
+                         float cutoff, int n_atoms, const float* gagg, float* gy, float* egrad, cudaStream_t s) {
+    k_cfconv_bwd<<<(n_atoms + CF_WARPS - 1) / CF_WARPS, CF_THREADS, 0, s>>>(y, G1, G2, b2, geom, row_ptr, col, cutoff, n_atoms, gagg, gy, egrad);
+    return nb_check_launch();
+}
+
 extern "C" int64_t nb200_schnet_workspace_bytes(const nb200_schnet_weights* w, int32_t b_cap, int32_t n_cap, int32_t e_cap,
                                                 int32_t with_forces) {
     (void)b_cap;
@@ -281,22 +301,17 @@ extern "C" int nb200_schnet_energy_forces(nb200_engine* eng, const nb200_schnet_
     NB_TRY(nb200_neighbor_build(pos, mol_ptr, n_mol, N, w->cutoff, 0x7fffffff, e_cap, ws.row_ptr, ws.col, ws.rev, ws.geom, ws.deg, status, s)); }
     const size_t es = (size_t)e_cap;
     { Scope sc(eng, s, CAT_FILTER, 4);
-    NB_TRY(nb_bin_sort(ws.geom, status, 1.0f, 1.0f / dx, K, ws.sort_scr, s));
-    k_schnet_filter1<<<dim3(K, SF1_SPLIT, L), SF1_THREADS, 0, s>>>(ws.geom, status, ws.sort_scr, w->w_f1, w->b_f1, w->rbf_offsets, K, w->rbf_coeff, es,
-                                                                  ws.HH);
-    NB_TRY(nb_check_launch()); }
+    NB_TRY(nb_schnet_filter1(ws.geom, status, w->w_f1, w->b_f1, w->rbf_offsets, L, K, w->cutoff, w->rbf_coeff, es, ws.sort_scr, ws.HH, s)); }
     // second filter layer: one tall GEMM per layer over the stacked (h, dh/dd) rows
     for (int l = 0; l < L; ++l)
         NB_TRY(linear_fwd(eng, s, 2 * e_cap, F, F, ws.HH + (size_t)l * 2 * es * F, F, w->W_f2 + (size_t)l * F * F, F, ws.G + (size_t)l * 2 * es * F, F,
                           false, nullptr, nullptr));
     { Scope sc(eng, s, CAT_EMBED, 1); NB_TRY(nb_embed(z, w->emb, w->z_offset, w->n_elem, N, ws.x, ws.mu_dummy, status, s)); }
-    const int grid_cf = (N + CF_WARPS - 1) / CF_WARPS;
     for (int l = 0; l < L; ++l) {
         const float* G1 = ws.G + (size_t)l * 2 * es * F;
         NB_TRY(linear_fwd(eng, s, N, F, F, ws.x, F, w->I1 + (size_t)l * F * F, F, ws.y[l], F, false, nullptr, nullptr));
         { Scope sc(eng, s, CAT_MSG_FWD, 1);
-        k_cfconv_fwd<<<grid_cf, CF_THREADS, 0, s>>>(ws.y[l], G1, w->b_f2 + (size_t)l * F, ws.geom, ws.row_ptr, ws.col, w->cutoff, N, ws.agg);
-        NB_TRY(nb_check_launch()); }
+        NB_TRY(nb_schnet_cfconv_fwd(ws.y[l], G1, w->b_f2 + (size_t)l * F, ws.geom, ws.row_ptr, ws.col, w->cutoff, N, ws.agg, s)); }
         NB_TRY(linear_fwd(eng, s, N, F, F, ws.agg, F, w->P1 + (size_t)l * F * F, F, ws.t[l], F, false, w->p1 + (size_t)l * F, ws.act, NB_ACT_SSP));
         NB_TRY(linear_fwd(eng, s, N, F, F, ws.act, F, w->P2 + (size_t)l * F * F, F, ws.x, F, true, w->p2 + (size_t)l * F, nullptr));  // x += f2out(agg)
     }
@@ -304,7 +319,8 @@ extern "C" int nb200_schnet_energy_forces(nb200_engine* eng, const nb200_schnet_
     { Scope sc(eng, s, CAT_READOUT, 2);
     NB_TRY(nb_readout(ws.ro_pre, w->e1, w->R2, w->e2, N, F / 2, ws.eps, s));
     NB_TRY(nb_mol_sum(ws.eps, mol_ptr, n_mol, w->energy_shift_per_atom, energy, s)); }
-    if (!want_f) return NB200_OK;
+    // a failed graph build or embedding leaves finite numbers of an emptied graph behind: NaN them (as PaiNN) so that no error passes silently
+    if (!want_f) { Scope sc(eng, s, CAT_READOUT, 1); return nb_poison_on_error(status, energy, n_mol, nullptr, 0, s); }
 
     if (cudaMemsetAsync(ws.egrad, 0, es * 4 * sizeof(float), s) != cudaSuccess) return nb_check_launch();
     { Scope sc(eng, s, CAT_READOUT, 1); NB_TRY(nb_readout_bwd(ws.ro_pre, w->R2, N, F / 2, ws.g_ro, s)); }
@@ -316,11 +332,48 @@ extern "C" int nb200_schnet_energy_forces(nb200_engine* eng, const nb200_schnet_
         { Scope sc(eng, s, CAT_NODE, 1); NB_TRY(nb_act_bwd(ws.gt, ws.t[l], (int64_t)N * F, NB_ACT_SSP, s)); }
         NB_TRY(linear_bwd(eng, s, N, F, F, ws.gt, F, w->P1 + (size_t)l * F * F, F, ws.gagg, F, false));
         { Scope sc(eng, s, CAT_MSG_BWD, 1);
-        k_cfconv_bwd<<<grid_cf, CF_THREADS, 0, s>>>(ws.y[l], G1, G2, w->b_f2 + (size_t)l * F, ws.geom, ws.row_ptr, ws.col, w->cutoff, N, ws.gagg,
-                                                   ws.gy, ws.egrad);
-        NB_TRY(nb_check_launch()); }
+        NB_TRY(nb_schnet_cfconv_bwd(ws.y[l], G1, G2, w->b_f2 + (size_t)l * F, ws.geom, ws.row_ptr, ws.col, w->cutoff, N, ws.gagg, ws.gy, ws.egrad,
+                                    s)); }
         if (l > 0) NB_TRY(linear_bwd(eng, s, N, F, F, ws.gy, F, w->I1 + (size_t)l * F * F, F, ws.gx, F, true));
     }
-    { Scope sc(eng, s, CAT_FORCE, 1); NB_TRY(nb200_edge_forces(ws.egrad, ws.geom, ws.row_ptr, ws.rev, N, forces, s)); }
+    { Scope sc(eng, s, CAT_FORCE, 2); NB_TRY(nb200_edge_forces(ws.egrad, ws.geom, ws.row_ptr, ws.rev, N, forces, s));
+      NB_TRY(nb_poison_on_error(status, energy, n_mol, forces, (int64_t)3 * N, s)); }
     return NB200_OK;
+}
+
+// Test entry point (include/nabla_b200.h), not a supported API: one launch of nb200_schnet_energy_forces on caller-built inputs, through the
+// wrapper the engine calls, so that tests/test_gpu_schnet_kernels.py can compare each with a float64 reference.
+extern "C" int nb200_schnet_test_op(const nb200_schnet_test_args* a, void* stream) {
+    auto all = [](auto... p) { return ((p != nullptr) && ...); };
+    auto aligned = [](auto... p) { return ((reinterpret_cast<uintptr_t>(p) % 16 == 0) && ...); };
+    if (!a || a->n_layers < 0 || a->n_atoms < 0 || a->n_edges < 0 || a->e_stride < 0 || a->m < 0) return NB200_EINVAL;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int F = NB_F;
+    switch (a->op) {
+    case NB200_SC_FILTER1: {
+        if (!all(a->geom, a->status, a->w_f1, a->b_f1, a->rbf_offsets, a->sort_scratch, a->HH) || !aligned(a->w_f1, a->b_f1, a->HH)) return NB200_EINVAL;
+        if (a->e_stride < a->n_edges) return NB200_EINVAL;
+        const int K = a->n_rbf;
+        if (K < NB_BAND || K > NB_NBINS_MAX) return NB200_EUNSUPPORTED;
+        const float dx = a->cutoff / (float)(K - 1);  // as nb200_schnet_energy_forces
+        if (!(a->rbf_coeff < 0.f) || a->rbf_coeff * (7.0f * dx) * (7.0f * dx) > -23.0f) return NB200_EUNSUPPORTED;
+        if (a->n_layers == 0) return NB200_OK;
+        return nb_schnet_filter1(a->geom, a->status, a->w_f1, a->b_f1, a->rbf_offsets, a->n_layers, K, a->cutoff, a->rbf_coeff, (size_t)a->e_stride,
+                                 a->sort_scratch, a->HH, s);
+    }
+    case NB200_SC_CFCONV_FWD:
+        if (!all(a->y, a->G1, a->b2, a->geom, a->row_ptr, a->col, a->agg) || !aligned(a->y, a->G1, a->b2, a->agg)) return NB200_EINVAL;
+        if (a->n_atoms == 0) return NB200_OK;
+        return nb_schnet_cfconv_fwd(a->y, a->G1, a->b2, a->geom, a->row_ptr, a->col, a->cutoff, a->n_atoms, a->agg, s);
+    case NB200_SC_CFCONV_BWD:
+        if (!all(a->y, a->G1, a->G2, a->b2, a->geom, a->row_ptr, a->col, a->gagg, a->gy, a->egrad) || !aligned(a->y, a->G1, a->G2, a->b2, a->gagg, a->gy))
+            return NB200_EINVAL;
+        if (a->n_atoms == 0) return NB200_OK;
+        return nb_schnet_cfconv_bwd(a->y, a->G1, a->G2, a->b2, a->geom, a->row_ptr, a->col, a->cutoff, a->n_atoms, a->gagg, a->gy, a->egrad, s);
+    case NB200_SC_LINEAR_ACT:  // linear_fwd(..., act, NB_ACT_SSP) of f2out.0
+        if (!all(a->X, a->W, a->bias, a->Y, a->act) || !aligned(a->X, a->W, a->bias, a->Y, a->act)) return NB200_EINVAL;
+        if (a->m == 0) return NB200_OK;
+        return nb_gemm_tf32x3_ex(a->m, F, F, a->X, F, a->W, F, 0, a->Y, F, 0, a->bias, a->act, NB_ACT_SSP, s);
+    }
+    return NB200_EINVAL;
 }

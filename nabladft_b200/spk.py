@@ -86,6 +86,21 @@ class AddOffsets(nn.Module):
         super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
 
 
+def _banded_rbf_coeff(rep) -> float:
+    """`rbf_coeff` of the representation's Gaussian basis.  The filter kernels evaluate only the 16 centres around bin floor(d / dx),
+    dx = cutoff / (K - 1), so they need offsets[k] = k dx and widths equal to dx; a shifted basis (GaussianRBF(start != 0)) or another
+    width, e.g. from a checkpoint's buffers, would silently lose most of the filter."""
+    rbf, cutoff = rep.radial_basis, float(rep.cutoff_fn.cutoff.item())
+    K = rbf.n_rbf
+    dx = cutoff / (K - 1)
+    offsets, widths = rbf.offsets.detach().double().cpu(), rbf.widths.detach().double().cpu()
+    if (offsets - dx * torch.arange(K, dtype=torch.float64)).abs().max().item() > 1e-6 * cutoff:
+        raise NotImplementedError("Gaussian RBF offsets other than k * cutoff / (n_rbf - 1) (a basis that starts at 0 and ends at the cutoff)")
+    if (widths - dx).abs().max().item() > 1e-6 * dx:
+        raise NotImplementedError("Gaussian RBF widths other than the centre spacing cutoff / (n_rbf - 1)")
+    return float(-0.5 / widths[0].item() ** 2)
+
+
 def _dense(n_in, n_out, bias=True):
     lin = nn.Linear(n_in, n_out, bias=bias)
     nn.init.xavier_uniform_(lin.weight)
@@ -211,7 +226,7 @@ class NeuralNetworkPotential(nn.Module):
             for p in self.postprocessors:
                 if isinstance(p, AddOffsets) and p.add_mean:
                     shift += float(p.mean.item())
-        widths = rep.radial_basis.widths
+        rbf_coeff = _banded_rbf_coeff(rep)
         tensors = {
             "emb": c(rep.embedding.weight),
             "w_rbf": c(rep.filter_net.weight.view(L, 3 * n, K).transpose(1, 2)),  # [L*3n, K] -> [L, K, 3n]
@@ -231,7 +246,7 @@ class NeuralNetworkPotential(nn.Module):
         }
         scalars = dict(
             n_layers=L, n_feat=n, n_rbf=K, n_elem=rep.embedding.num_embeddings, radial_mode=RADIAL_SPK, z_offset=0,
-            cutoff=float(rep.cutoff_fn.cutoff.item()), epsilon=float(rep.epsilon), rbf_coeff=float(-0.5 / widths[0].item() ** 2), rbf_xscale=1.0,
+            cutoff=float(rep.cutoff_fn.cutoff.item()), epsilon=float(rep.epsilon), rbf_coeff=rbf_coeff, rbf_xscale=1.0,
             energy_shift_per_atom=shift, max_neighbors=INT32_MAX,
         )
         return tensors, scalars
@@ -254,6 +269,7 @@ class NeuralNetworkPotential(nn.Module):
         c = lambda t: (t.detach() if detach else t).to(f32).contiguous()
         stack = lambda ts: c(torch.stack(list(ts)))
         I = rep.interactions
+        rbf_coeff = _banded_rbf_coeff(rep)
         tensors = {
             "emb": c(rep.embedding.weight),
             "w_f1": stack(i.filter_network[0].weight.t() for i in I),  # [F, K] -> K-major [K, F]
@@ -268,7 +284,7 @@ class NeuralNetworkPotential(nn.Module):
         }
         scalars = dict(
             n_layers=rep.n_interactions, n_feat=rep.n_atom_basis, n_rbf=rep.radial_basis.n_rbf, n_elem=rep.embedding.num_embeddings,
-            z_offset=0, cutoff=float(rep.cutoff_fn.cutoff.item()), rbf_coeff=float(-0.5 / rep.radial_basis.widths[0].item() ** 2),
+            z_offset=0, cutoff=float(rep.cutoff_fn.cutoff.item()), rbf_coeff=rbf_coeff,
             energy_shift_per_atom=self._shift(postprocess),
         )
         return tensors, scalars

@@ -544,3 +544,91 @@ def test_spk_schnet_engine_matches_oracle():
     model._forces = False
     out_e = model(inp)
     assert "forces" not in out_e and torch.equal(out_e["energy"], out["energy"])
+
+
+def test_schnet_engine_edge_cases():
+    """SchNet keeps run_async's promise as PaiNN does (test_engine_edge_cases): an overflowing edge capacity or an atomic number outside the
+    embedding table makes every energy and force of the launch NaN, and the next check raises; energy-only calls included."""
+    from nabladft_b200._lib import NablaB200Error
+
+    model = _spk_schnet_model(2).to(dev())
+    z, pos, batch = load_fixture([20, 21], torch.float32)
+    inp = {"_atomic_numbers": z.to(dev()), "_positions": pos.to(dev()), "_idx_m": batch.to(dev()), "_n_atoms": torch.bincount(batch).to(dev())}
+    good = model(inp)
+    eng = model._engine
+    for forces in (True, False):
+        model._forces = forces
+        eng.check_pending(wait=True)
+        eng.e_cap, eng._validated_ratio, eng.e_cap_slack = 0, 1e-3, 8
+        out = model(inp)
+        assert torch.isnan(out["energy"]).all() and (not forces or torch.isnan(out["forces"]).all())
+        with pytest.raises(NablaB200Error, match="ECAPACITY"):
+            model.check()
+        eng.e_cap_slack = 1024
+        again = model(inp)
+        model.check()
+        assert torch.equal(again["energy"], good["energy"]) and (not forces or torch.equal(again["forces"], good["forces"]))
+        bad = dict(inp, _atomic_numbers=inp["_atomic_numbers"].clone())
+        bad["_atomic_numbers"][0] = 100  # the table has rows 0 .. 99
+        out = model(bad)
+        assert torch.isnan(out["energy"]).all() and (not forces or torch.isnan(out["forces"]).all())
+        with pytest.raises(NablaB200Error):
+            model.check()
+
+
+def test_schnet_c_entry_nans_outputs_on_overflow_and_refuses_other_widths():
+    """nb200_schnet_energy_forces itself: with a too-small e_cap, energy-only and E+F calls return all-NaN energies and forces (and
+    NB200_ECAPACITY in status); a Gaussian width other than the centre spacing is NB200_EUNSUPPORTED."""
+    from nabladft_b200 import _lib
+    from nabladft_b200.engine import mol_ptr_from_batch
+
+    model = _spk_schnet_model(2).to(dev())
+    eng = model.engine(True)
+    z, pos, batch = load_fixture([20, 21], torch.float32)
+    mol_ptr, n_mol = mol_ptr_from_batch(batch.to(dev()))
+    z, pos = z.to(dev()).int(), pos.to(dev())
+    for with_forces in (False, True):
+        energy, forces, status = eng.launch(z, pos, mol_ptr, n_mol, with_forces, e_cap=16)
+        torch.cuda.synchronize()
+        assert int(status[1]) == -4 and torch.isnan(energy).all() and (not with_forces or torch.isnan(forces).all())
+    w = _lib.SchnetWeights.from_buffer_copy(eng._weights)
+    w.rbf_coeff = -0.5 / (1.5 * 5.0 / 99) ** 2
+    ws = torch.zeros(1 << 20, dtype=torch.uint8, device=dev())
+    e = torch.zeros(n_mol, device=dev())
+    rc = eng.lib.nb200_schnet_energy_forces(eng._h, ctypes.byref(w), _lib.ptr(z), _lib.ptr(pos), _lib.ptr(mol_ptr), n_mol, z.shape[0], 4096,
+                                            _lib.ptr(ws), ws.numel(), _lib.ptr(e), None, _lib.ptr(torch.zeros(4, dtype=torch.int32, device=dev())),
+                                            _lib.current_stream())
+    assert rc == -2
+
+
+def test_spk_schnet_isolated_pair_and_dense_cluster_match_oracle():
+    """SchNet E+F against the float64 oracle on one batch of an isolated atom, a two-atom molecule and a dense 300-atom cluster whose rows
+    hold well over 100 edges (the fixture molecules reach a few tens)."""
+    from oracle.graph import ase_neighbor_list, batch_to_ptr
+    from oracle.spk import NeuralNetworkPotential as OracleNNP
+    from oracle.spk import SpkSchNet
+
+    model = _spk_schnet_model(6)
+    ref = OracleNNP(SpkSchNet()).double()
+    sd = model.state_dict()
+    ref.load_state_dict({k: sd[k].double() for k in ref.state_dict()}, strict=True)
+    g = torch.Generator().manual_seed(11)
+    grid = torch.stack(torch.meshgrid(*[torch.arange(7, dtype=torch.float64)] * 3, indexing="ij"), -1).reshape(-1, 3)[:300]
+    cluster = grid * 0.95 + (torch.rand(300, 3, generator=g, dtype=torch.float64) - 0.5) * 0.3  # ~1 A apart, a 6 A cube
+    pos = torch.cat([torch.zeros(1, 3, dtype=torch.float64), torch.tensor([[0.0, 0, 0], [0.0, 0.0, 1.2]], dtype=torch.float64), cluster])
+    z = torch.cat([torch.tensor([8, 1, 1]), torch.randint(1, 10, (300,), generator=g)])
+    batch = torch.cat([torch.tensor([0, 1, 1]), torch.full((300,), 2)])
+    idx_i, idx_j = ase_neighbor_list(pos, batch_to_ptr(batch), 5.0)
+    max_deg = int(torch.bincount(idx_i).max())
+    assert max_deg > 100
+    out_ref = ref({"_atomic_numbers": z, "_positions": pos.clone(), "_idx_i": idx_i, "_idx_j": idx_j, "_idx_m": batch})
+    model = model.to(dev())
+    out = model({"_atomic_numbers": z.to(dev()), "_positions": pos.float().to(dev()), "_idx_m": batch.to(dev()),
+                 "_n_atoms": torch.bincount(batch).to(dev())})
+    e_ref, f_ref = out_ref["energy"].detach(), out_ref["forces"]
+    de = (out["energy"].double().cpu() - e_ref).abs()
+    df = (out["forces"].double().cpu() - f_ref).abs().max().item()
+    print(f"schnet, isolated atom / pair / 300-atom cluster (max degree {max_deg}): |E| {e_ref.abs().tolist()}  dE {de.tolist()}  "
+          f"|F| <= {f_ref.abs().max().item():.2f}  dF {df:.2e}")
+    # fp32 sums over 300 atoms of ~250 edges each: the cluster's tolerances grow with its energy and largest force
+    assert (de < E_TOL + 1e-5 * e_ref.abs()).all() and df < F_TOL + 1e-5 * f_ref.abs().max().item()

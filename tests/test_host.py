@@ -123,10 +123,11 @@ def test_spk_export_matches_oracle_and_state_dict_names():
     assert torch.allclose(out["energy"], e1, atol=1e-5) and torch.allclose(out["forces"], f1, atol=1e-5)
 
 
-def test_spk_strict_load_of_schnetpack_shaped_checkpoint():
+def test_spk_strict_load_of_schnetpack_shaped_checkpoint_and_basis():
     """A schnetpack 2.0.4 checkpoint carries `postprocessors.0.atomref` (AddOffsets registers zeros[zmax] even without atomrefs) and the
     cutoff as a buffer; `load_state_dict(strict=True)` must accept it, a non-zero atomref must be refused, and the exported cutoff follows
-    the loaded buffer (ADVICE r1)."""
+    the loaded buffer (ADVICE r1).  A cutoff loaded without its Gaussian basis is refused: the filter's 16-centre band, chosen from
+    floor(d / (cutoff / (K - 1))), would miss up to 95 % of a basis still spread over 5 A (at d = 4.14 A)."""
     from nabladft_b200 import spk
 
     def make():
@@ -143,8 +144,13 @@ def test_spk_strict_load_of_schnetpack_shaped_checkpoint():
     net = make()
     net.load_state_dict(sd, strict=True)
     assert net.postprocessors[0].atomref.shape == (87,)
+    with pytest.raises(NotImplementedError, match="offsets"):  # Gaussians still spread over 5 A: the 16-centre band would miss them
+        net._export(True)
+    rbf = spk.GaussianRBF(n_rbf=100, cutoff=4.5)  # a checkpoint trained with cutoff 4.5 carries its basis too
+    sd["representation.radial_basis.offsets"], sd["representation.radial_basis.widths"] = rbf.offsets, rbf.widths
+    net.load_state_dict(sd, strict=True)
     _, scalars = net._export(True)
-    assert abs(scalars["cutoff"] - 4.5) < 1e-7
+    assert abs(scalars["cutoff"] - 4.5) < 1e-7 and abs(scalars["rbf_coeff"] + 0.5 / (4.5 / 99) ** 2) < 1e-3
     sd["postprocessors.0.atomref"] = torch.ones(87)
     with pytest.raises(NotImplementedError):
         make().load_state_dict(sd, strict=True)
